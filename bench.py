@@ -13,7 +13,10 @@ torchrun, one rank per GPU.  Rank 0 prints ONE JSON line.
 
 A "step" = one optimisation step of BAT_Car.yaml at batch 48 per GPU (BASELINE.json configs[1]); weak scaling.
 Timing hygiene: >= 3 warm-up steps, L2 flushed (256 MiB write) between timed steps and excluded from the timing,
-clocks sampled with nvidia-smi during the timed region.
+clocks sampled with nvidia-smi during the timed region.  Every device-timed step starts from the same training state (the
+seeded initial parameters, optimizer state and BatchNorm buffers, restored outside the timed region like the flush): the
+step's inputs, and so what it computes, are the same in every run.  Chained steps would not be: the backward's fp32 REDs
+and fp64 statistic atomics round in arrival order, and Adam compounds those last-bit differences over the steps.
 """
 import argparse
 import json
@@ -44,7 +47,7 @@ def parse():
     ap.add_argument("--cpu-steps", type=int, default=3)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--fused", type=int, default=None, help="override O3D_FUSED (1 = fused kernels, 0 = composed)")
-    ap.add_argument("--tc", type=int, default=None, help="override O3D_TC (0 = CUDA cores, 1 = tcgen05 fwd+dgrad, 3 = + wgrad)")
+    ap.add_argument("--tc", type=int, default=None, help="override O3D_TC (0 = CUDA cores, 1 = wgmma fwd+dgrad, 3 = + wgrad)")
     ap.add_argument("--no-graph", action="store_true", help="do not capture the step into a CUDA graph")
     ap.add_argument("--track", action="store_true", help="secondary mode: B=1 tracking frames/s (SURVEY.md 8f rank 2)")
     ap.add_argument("--sampler", action="store_true", help="secondary mode: on-device training-batch construction (8f rank 3)")
@@ -55,7 +58,16 @@ def parse():
                     "`ncu --profile-from-start off --metrics dram__bytes_read.sum,dram__bytes_write.sum`: DRAM bytes per step)")
     ap.add_argument("--cfg", default=None, help="other config to exercise (P2B_Car.yaml, M2_track_kitti.yaml, ...): a parity / "
                     "plumbing run of BASELINE.json configs[2..4], NOT the headline metric")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last device-timed training step returned (loss.npy) and the "
+                         "parameter gradients it computed (gradients.npy) as float32 .npy files under DIR, to compare two builds "
+                         "output for output")
+    a = ap.parse_args()
+    if a.dump_outputs and (a.track or a.sampler or a.impl != "ours" or a.ncu_step):
+        ap.error("--dump-outputs applies to the training-step benchmark only")
+    if a.dump_outputs and a.steps < 1:
+        ap.error("--dump-outputs needs at least one timed step (--steps >= 1)")
+    return a
 
 
 # ----------------------------------------------------------------------------------------------- clocks
@@ -185,9 +197,6 @@ def run_track(args):
     torch.cuda.set_device(dev)
     cfg = load_config(CFG_FILE if args.cfg is None else os.path.join(ROOT, "cfgs", args.cfg), {"up_axis": [0, 0, 1]})
     torch.manual_seed(0)
-    if os.environ.get("O3D_FORCE_MT"):
-        from open3dsot_b200 import _lib
-        _lib.lib().o3d_debug_set(0, int(os.environ["O3D_FORCE_MT"]))
     net = get_model(cfg.net_model)(cfg).to(dev).eval()
     frames, npts = max(args.steps + args.warmup + 1, 12), args.track_points
     seq = synthetic_sequence(n_frames=frames, n_points=npts, seed=20260924)
@@ -353,7 +362,7 @@ def measured_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback (H100 SXM data sheet, 700 W)"
 
 
 def gather_roofline(dev, batch_pairs):
@@ -395,12 +404,6 @@ def gather_roofline(dev, batch_pairs):
                                                    co[1].data_ptr(), co[2].data_ptr(), st), "o3d_lift_scatter"),
              g.numel() * 4 + P * (4 + 16) + 2 * z.numel() * 4)}
     peaks, how = measured_peaks()
-    traffic = {}
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2_irregular_traffic.json")) as f:
-            traffic = json.load(f)
-    except (OSError, ValueError):
-        pass
     out = []
     for name, (fn, nbytes) in runs.items():
         for _ in range(3):
@@ -417,20 +420,8 @@ def gather_roofline(dev, batch_pairs):
         ach = nbytes / (ms * 1e-3) / 1e9
         out.append({"kernel": name + f", SA2-search shape, B={B}: P={P}, {C0} channels", "bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"],
                     "peak_source": how + " (MEASURED_PEAKS.json hbm_gbs, burst copy)", "unit": "GB/s", "frac": ach / peaks["hbm_gbs"],
-                    "traffic": traffic.get(name.split(" ")[0]), "ms_per_launch": ms, "algorithmic_bytes_per_launch": nbytes})
+                    "ms_per_launch": ms, "algorithmic_bytes_per_launch": nbytes})
     return out
-
-
-def ncu_traffic(P, key="fwd"):
-    """DRAM bytes per launch of a roofline kernel as ncu measured them (dram__bytes_read.sum + dram__bytes_write.sum of
-    one `--set full` capture of the same kernel and shape, committed under profiles/); None when the shape differs."""
-    path = os.path.join(ROOT, "profiles", "r1_roofline_traffic.json")
-    try:
-        with open(path) as f:
-            rec = json.load(f)[key]
-        return float(rec["dram_bytes_per_launch"]) if f"P={P}," in rec["shape"] else None
-    except (OSError, ValueError, KeyError):
-        return None
 
 
 def roofline_probe(dev, batch_pairs):
@@ -468,19 +459,19 @@ def roofline_probe(dev, batch_pairs):
     ms = e0.elapsed_time(e1) / n
     peaks, how = measured_peaks()
     flops = 2.0 * P * K * N
-    alg_bytes = 4.0 * P * (K + N)                      # 403 MB per launch: larger than the 126 MB L2
+    alg_bytes = 4.0 * P * (K + N)                      # 403 MB per launch: larger than the 50 MB L2
     tf = flops / (ms * 1e-3) / 1e12
     gbs = alg_bytes / (ms * 1e-3) / 1e9
     tensor_peak = peaks["bf16_tflops"] / 2.0 / 3.0      # TF32 runs at half the bf16 rate; 3 passes per product
     t_tensor, t_hbm = flops / (tensor_peak * 1e12), alg_bytes / (peaks["hbm_gbs"] * 1e9)
     bound = "tensor" if t_tensor >= t_hbm else "hbm"
-    return {"kernel": "pw_tc_kernel<2,TcAct,TcFwdEpi> (SA3-search layer: P=%d, K=256, N=256, 3xTF32)" % P,
+    return {"kernel": "pw_tc_kernel<TcAct,TcFwdEpi> (SA3-search layer: P=%d, K=256, N=256, 3xTF32)" % P,
             "bound": bound, "achieved": tf if bound == "tensor" else gbs,
             "peak": tensor_peak if bound == "tensor" else peaks["hbm_gbs"],
             "unit": "TFLOP/s" if bound == "tensor" else "GB/s",
             "frac": (tf / tensor_peak) if bound == "tensor" else (gbs / peaks["hbm_gbs"]),
             "peak_source": how + " MEASURED_PEAKS.json: bf16_tflops/2/3 (TF32 rate, three passes) and hbm_gbs (burst)",
-            "traffic": ncu_traffic(P), "ms_per_launch": ms, "algorithmic_flops_per_launch": flops,
+            "ms_per_launch": ms, "algorithmic_flops_per_launch": flops,
             "algorithmic_bytes_per_launch": alg_bytes, "achieved_tflops_fp32_equiv": tf, "achieved_gbs": gbs,
             "frac_of_tensor_roof": tf / tensor_peak, "frac_of_hbm_roof": gbs / peaks["hbm_gbs"]}
 
@@ -520,8 +511,8 @@ def roofline_backward_probe(dev, batch_pairs):
                                       part.numel(), st), "o3d_pw_wgrad_tc2")
     peaks, how = measured_peaks()
     res = []
-    for name, fn, nbytes, key in (("pw_tc_kernel<1,TcDy,TcDgradEpi<128>> (dgrad)", dgrad, 4.0 * P * C * 4, "dgrad"),
-                                  ("pw_wgrad_tc2_kernel<1,1> + wgrad_reduce_kernel (wgrad, split-K, deterministic)", wgrad, 4.0 * P * C * 3, "wgrad")):
+    for name, fn, nbytes in (("pw_tc_kernel<TcDy,TcDgradEpi<128>> (dgrad)", dgrad, 4.0 * P * C * 4),
+                             ("pw_wgrad_tc_kernel + wgrad_reduce_kernel (wgrad, split-K, deterministic)", wgrad, 4.0 * P * C * 3)):
         for _ in range(3):
             fn()
         torch.cuda.synchronize()
@@ -535,7 +526,7 @@ def roofline_backward_probe(dev, batch_pairs):
         ms = e0.elapsed_time(e1) / n
         gbs = nbytes / (ms * 1e-3) / 1e9
         res.append({"kernel": name + ", SA2-search layer: P=%d, 128 -> 128 channels" % P, "bound": "hbm", "achieved": gbs,
-                    "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gbs / peaks["hbm_gbs"], "traffic": ncu_traffic(P, key),
+                    "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gbs / peaks["hbm_gbs"],
                     "ms_per_launch": ms, "algorithmic_bytes_per_launch": nbytes,
                     "peak_source": how + " (MEASURED_PEAKS.json hbm_gbs, burst copy)"})
     return res
@@ -563,6 +554,23 @@ def kernel_table(eng, batches, path, steps=3):
         f.write("#  share   ms/step  launches/step  kernel\n")
         for name, (n, us) in sorted(agg.items(), key=lambda kv: -kv[1][1]):
             f.write(f"{100 * us / total:7.2f}% {us / steps / 1e3:9.3f} {n / steps:8.1f}  {name[:150]}\n")
+
+
+def dump_outputs(out_dir, loss, grads, limit_bytes=64 << 20):
+    """The last timed step's loss and the parameter gradients it computed (the flat gradient bucket Adam consumed), float32.
+    The updated parameters are not written: from the restored state they are a fixed function of these gradients, and
+    Adam's first step (lr * g / (|g| + eps)) magnifies the last-bit noise of near-zero gradient elements by lr / eps.
+    The gradients go whole while they fit in `limit_bytes` (a BAT network's do); otherwise a fixed, seeded sample of them
+    (sorted indices, seed 0)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.reshape(1).float().cpu().numpy())
+    flat = grads.reshape(-1).float().cpu()
+    n = (limit_bytes - 4096) // 8
+    if flat.numel() * 4 > limit_bytes - 4096:
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:n].sort().values
+        flat = flat[idx]
+    np.save(os.path.join(out_dir, "gradients.npy"), flat.numpy())
 
 
 def run_ours(args):
@@ -593,6 +601,8 @@ def run_ours(args):
     net = get_model(cfg.net_model)(cfg).to(dev).train()
     from open3dsot_b200.engine import TrainStep
     eng = TrainStep(net, lr=cfg.lr, weight_decay=cfg.wd, use_graph=not args.no_graph, warmup=2)
+    train_state = [eng.flat.flat, eng.opt.exp_avg, eng.opt.exp_avg_sq, eng.opt.state, *net.buffers()]
+    initial_state = [t.clone() for t in train_state]
 
     # distinct host batches (pinned), one device-resident copy of each
     n_batches = 4
@@ -642,10 +652,15 @@ def run_ours(args):
     barrier()
     t_wall0 = time.perf_counter()
     for i in range(args.steps):
+        with torch.no_grad():                                   # the same starting state for every timed step; not timed
+            for t, t0 in zip(train_state, initial_state):
+                t.copy_(t0)
         flush.fill_(float(i))                                   # evict L2; not timed
         evs[i][0].record()
-        eng.step(resident[i % n_batches])
+        loss_timed = eng.step(resident[i % n_batches])
         evs[i][1].record()
+    if args.dump_outputs:                                       # the last timed step's results, before later steps overwrite them
+        dumped = (loss_timed.detach().clone(), eng.flat.grad.detach().clone())
     barrier()
     wall = time.perf_counter() - t_wall0
     launches = launches_per_step * args.steps
@@ -695,6 +710,8 @@ def run_ours(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)                          # max over ranks, taken after the timed region
     e2e_s = float(t.item())
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *dumped)
 
     if rank != 0:
         _shutdown(eng, world)
@@ -714,8 +731,8 @@ def run_ours(args):
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload, "global_batch": args.batch * world, "parallelism": f"dp{world}",
                        "mode": "fused" if runtime.fused_enabled() else "composed",
-                       "gemm_core": {0: "cuda-core-fp32", 1: "tcgen05-3xTF32 fwd+dgrad, cuda-core wgrad",
-                                     3: "tcgen05-3xTF32 fwd+dgrad+wgrad"}.get(runtime.tc_level(), str(runtime.tc_level())),
+                       "gemm_core": {0: "cuda-core-fp32", 1: "wgmma-3xTF32 fwd+dgrad, cuda-core wgrad",
+                                     3: "wgmma-3xTF32 fwd+dgrad+wgrad"}.get(runtime.tc_level(), str(runtime.tc_level())),
                        "cuda_graph": not args.no_graph,
                        "l2": "256 MiB flush write between timed steps, excluded from timing",
                        "optimizer": "Adam(0.5,0.999), one kernel over the flat parameter bucket", "last_loss": last,

@@ -1,5 +1,5 @@
 /*
- * o3d_b200.h — C ABI of libo3d_b200.so (hand-written sm_100a kernels for the Open3DSOT hot path).
+ * o3d_b200.h — C ABI of libo3d_b200.so (hand-written sm_90a kernels for the Open3DSOT hot path).
  *
  * Conventions (SURVEY.md §8b):
  *   - every pointer is a DEVICE pointer unless its name ends in `_host`; the caller owns all buffers,
@@ -13,7 +13,7 @@
  * The first block mirrors, one to one, the nine pybind entry points of `pointnet2_ops._ext` that the
  * reference binds at pointnet2/utils/pointnet2_utils.py:17 and calls at :56,:92,:98,:125,:162,:184,:217,
  * :237,:268 (tensor layouts and result conventions identical).  The second block holds the fused
- * supersets used by the B200-native modules (channels-last activations).
+ * supersets used by the native modules (channels-last activations).
  */
 #ifndef O3D_B200_H
 #define O3D_B200_H
@@ -185,7 +185,7 @@ int o3d_act_apply(const float* y, int ldy, const float* scale, const float* shif
 int o3d_dense_bwd_prep(const float* dout, int ldd, const float* out, int ldo, const float* y, int ldy, int relu, int P,
                        int C, float* g, int ldg, double* s1, double* s2y, void* stream);
 
-/* Tensor-core (tcgen05 / TMEM, 3xTF32) variants of o3d_pw_fwd / o3d_pw_dgrad for >= 128 output channels and
+/* Tensor-core (Hopper wgmma, 3xTF32) variants of o3d_pw_fwd / o3d_pw_dgrad for >= 128 output channels and
  * K >= 32.  The weight operand is passed pre-tiled: o3d_pw_tc_pretile() rewrites a row-major matrix
  * w[rows, ldw] (rows = the GEMM's output channels, K contiguous) into per-(128-row tile, 32-wide k-block)
  * shared-memory images [hi | lo], K-major SWIZZLE_128B, that the kernel streams with cp.async.bulk.
@@ -193,7 +193,7 @@ int o3d_dense_bwd_prep(const float* dout, int ldd, const float* out, int ldo, co
  * dgrad  :  rows = Cin,  K = Cout  (w = its transpose)                                                */
 long long o3d_pw_tc_wtile_bytes(int rows, int K);
 void o3d_pw_tc_set_reverse(int rev);              /* next o3d_pw_*_tc launch of this thread walks the position tiles backwards */
-void o3d_debug_set(int tc_debug, int force_mt);   /* profiling experiments only (results invalid when non-zero) */
+void o3d_debug_set(int tc_debug);   /* profiling experiments only (results invalid when non-zero) */
 int o3d_pw_tc_pretile(const float* w, int ldw, int rows, int K, void* wtiles, void* stream);
 int o3d_pw_fwd_tc(const float* x, int ldx, const float* in_scale, const float* in_shift, int in_relu, const void* wtiles,
                   const float* bias, int P, int K, int N, float* y, int ldy, double* sum, double* sumsq, int S,
@@ -247,7 +247,7 @@ typedef struct o3d_stack_t {
     int K0;         /* input row length (multiple of 4, zero padded)                             */
     int S;          /* pooling group size over consecutive positions (0 = dense output)          */
     int training;   /* BatchNorm uses batch statistics and updates the running ones              */
-    int use_tc;     /* allow the tcgen05 3xTF32 kernels where the shape qualifies                */
+    int use_tc;     /* allow the wgmma 3xTF32 kernels where    the shape qualifies                */
     int xyz_first;  /* layer-0 weight columns are [xyz(3) | features(c0)], input rows [features | dx dy dz 0] */
     int c0;         /* real feature channels of layer 0 when xyz_first                           */
     int dx_cols;    /* backward: only the first dx_cols input columns need a gradient (0 = all K0) */
@@ -320,13 +320,13 @@ int o3d_pw_wgrad_tc_lift(const float* g, int ldg, const float* y, int ldy, const
                          const float* in_scale, const float* in_shift, int in_relu, int P, int Cout, int Cin, float* dw,
                          int lddw, float* part, long long part_floats, void* stream);
 
-/* wgrad on the tensor core (MN-major SWIZZLE_128B operands, split over positions, fp32 RED into dw). */
+/* wgrad on the tensor core (operands transposed to K-major SWIZZLE_128B tiles, split over positions, fp32 RED into dw). */
 int o3d_pw_wgrad_tc(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
                     const float* dpool, const int32_t* sel, int S, int ldp, const float* x, int ldx,
                     const float* in_scale, const float* in_shift, int in_relu, int P, int Cout, int Cin, float* dw,
                     int lddw, void* stream);
 
-/* wgrad, wide tiles (up to 256 x 256 of dW per CTA, all of TMEM), split over positions; the per-split partial tiles go
+/* wgrad, 128 x 128 tiles of dW per CTA, split over positions; the per-split partial tiles go
  * to `part` (o3d_pw_wgrad_tc2_workspace_floats() floats) and a second kernel adds their sum into dw.              */
 long long o3d_pw_wgrad_tc2_workspace_floats(void);
 int o3d_pw_wgrad_tc2(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,

@@ -1,7 +1,7 @@
 """ctypes binding of libo3d_b200.so (the C ABI declared in include/o3d_b200.h).
 
 The product path has NO fallback: if the shared library is missing or a kernel reports an error, a
-RuntimeError is raised.  Build with `python -c "import __graft_entry__ as g; g.build()"` (nvcc, sm_100a).
+RuntimeError is raised.  Build with `python -c "import __graft_entry__ as g; g.build()"` (nvcc, sm_90a).
 """
 import ctypes
 import os
@@ -49,7 +49,7 @@ PROTOTYPES = {
     "o3d_act_apply": [_p, _i, _p, _p, _i, _i, _i, _p, _i, _p],
     "o3d_dense_bwd_prep": [_p, _i, _p, _i, _p, _i, _i, _i, _i, _p, _i, _p, _p, _p],
     "o3d_pw_tc_wtile_bytes": [_i, _i],
-    "o3d_debug_set": [_i, _i],
+    "o3d_debug_set": [_i],
     "o3d_pw_tc_set_reverse": [_i],
     "o3d_pw_tc_pretile": [_p, _i, _i, _i, _p, _p],
     "o3d_pw_fwd_tc": [_p, _i, _p, _p, _i, _p, _p, _i, _i, _i, _p, _i, _p, _p, _i, _p, _p, _p, _i, _p],

@@ -1,4 +1,4 @@
-"""Build libo3d_b200.so in-tree with nvcc for sm_100a (one translation unit per kernel family)."""
+"""Build libo3d_b200.so in-tree with nvcc for sm_90a (one translation unit per kernel family)."""
 import glob
 import os
 import subprocess
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libo3d_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

@@ -1,4 +1,4 @@
-// Ball query, and ball query fused with grouping, for sm_100a.
+// Ball query, and ball query fused with grouping, for sm_90a.
 //
 // Replaces `_ext.ball_query` (pointnet2/utils/pointnet2_utils.py:268) and the whole of
 // QueryAndGroup.forward (pointnet2/utils/pointnet2_utils.py:299-339: ball_query, 2x group_points,

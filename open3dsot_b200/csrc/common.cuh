@@ -1,4 +1,4 @@
-// open3dsot_b200 — shared device/host helpers for the sm_100a kernels.
+// open3dsot_b200 — shared device/host helpers for the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -42,7 +42,7 @@ static inline int o3d_num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (sms <= 0) sms = 148;
+        if (sms <= 0) sms = 132;
     }
     return sms;
 }

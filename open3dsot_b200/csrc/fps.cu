@@ -1,4 +1,4 @@
-// Furthest point sampling for sm_100a.
+// Furthest point sampling for sm_90a.
 //
 // Replaces `_ext.furthest_point_sampling` (reference call site pointnet2/utils/pointnet2_utils.py:56;
 // upstream kernel furthest_point_sampling_kernel<block> in pointnet2_ops, see oracle/pointnet2_ops_ref.c).
@@ -146,7 +146,7 @@ extern "C" int o3d_fps(const float* xyz, int B, int N, int npoint, int32_t* idx,
     while ((1 << prm.log2_block) < prm.block_ref) ++prm.log2_block;
     prm.cnt = (N + prm.block_ref - 1) / prm.block_ref;
     cudaStream_t st = (cudaStream_t)stream;
-    // measured on B200 (48 clouds): 128 threads x 8 points = 1,170 cycles per iteration at N = 1024; spreading the points over
+    // 128 threads x 8 points make a long per-thread chain per iteration at N = 1024; spreading the points over
     // more warps shortens the per-thread chain (the second-level reduction handles up to 32 warps in one step)
     if (N <= 128) return launch_fps<128, 1>(xyz, B, idx, prm, st);
     if (N <= 256) return launch_fps<128, 2>(xyz, B, idx, prm, st);

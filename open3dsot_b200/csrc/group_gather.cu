@@ -1,8 +1,8 @@
-// gather_points / group_points and their gradients in the reference's (B,C,N) layout, for sm_100a.
+// gather_points / group_points and their gradients in the reference's (B,C,N) layout, for sm_90a.
 //
 // Replaces `_ext.gather_points(_grad)` (pointnet2/utils/pointnet2_utils.py:92,98) and
 // `_ext.group_points(_grad)` (:217,:237).  These keep the reference tensor layout so that the
-// reference's own autograd Functions work unchanged on top of them (INTEGRATION.md); the B200-native
+// reference's own autograd Functions work unchanged on top of them (INTEGRATION.md); the native
 // modules use the channels-last fused kernels in ball_query.cu / pwmlp.cu instead.
 //
 // Design: the output is a dense (B*C, M*S) matrix whose rows are gathered from rows of N floats.

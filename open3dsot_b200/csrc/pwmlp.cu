@@ -20,7 +20,7 @@
 //
 // This file is the exact-fp32 CUDA-core implementation (128 x {64,128} x 16 tiles, 256 threads, 8x8 or 4x8
 // register blocks, register-prefetch double buffering).  It is the numerical ground truth for the tensor-core
-// (tcgen05, 3xTF32) variant in pwmlp_tc.cu, which shares these loaders' semantics and the epilogue contract.
+// (wgmma, 3xTF32) variant in pwmlp_tc.cu, which shares these loaders' semantics and the epilogue contract.
 #include "common.cuh"
 #include "../../include/o3d_b200.h"
 

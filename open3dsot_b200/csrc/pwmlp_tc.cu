@@ -1,30 +1,14 @@
-// Tensor-core (tcgen05 / TMEM) implementation of the point-wise MLP forward and data-gradient GEMMs, 3xTF32.
+// Tensor-core (Hopper wgmma) implementation of the point-wise MLP forward, data-gradient and weight-gradient GEMMs, 3xTF32.
 //
 // Same contract as pw_fwd_kernel / pw_dgrad_kernel in pwmlp.cu (which remain the exact-fp32 ground truth and
 // serve the shapes this kernel does not take: K < 32, ragged channel tails, very small P).
 //
-//   D[ch, pos] = sum_k  Wmat[ch, k] * Act[pos, k]          ch tile = 128 (UMMA M), pos tile = 128 (UMMA N)
+//   D[pos, ch] = sum_k  Act[pos, k] * Wmat[ch, k]          pos tile = 128 (2 warpgroups x m64), ch tile = 128 (wgmma N)
 //
 // with Act produced on the fly from global memory (forward: relu(bn(Y_prev)); dgrad: dY = a*g + b + c*Y) and split
 // into a TF32 "hi" part (the fp32 word with its 13 low mantissa bits cleared) and a "lo" part
-// (x - hi, exact), so that   Whi*Xhi + Wlo*Xhi + Whi*Xlo   carries ~21 mantissa bits — fp32-grade accuracy, which
-// the 1e-4 parity bar needs and a single TF32 pass (10 bits) cannot give.
-//
-// Roles of pw_tc_kernel (576 threads = 18 warps, one persistent CTA per SM, all roles walk the same static tile sequence):
-//   warp 0        allocates TMEM (double-buffered accumulators: 2 x MT x 128 fp32 columns) and, one elected lane, issues
-//                 tcgen05.mma.cta_group::1.kind::tf32 (M128 N128 K8), 12 per 32-channel k-block and channel tile, committing
-//                 each stage back to the producers and each finished tile to the epilogue through mbarriers
-//   warp 1        one lane streams the pre-tiled, pre-swizzled weight images (hi|lo, 32 KB per k-block and channel tile,
-//                 written once per call by stack.cu's pack kernel) with cp.async.bulk (UBLKCP) onto the stage's "full"
-//                 barrier, and asks for the next position tile's rows with cp.async.bulk.prefetch.L2
-//   warps 4-11    epilogue: tcgen05.ld 32 lanes x 16 columns; lane = output channel, columns = positions, so the batch
-//                 statistics, the group max/min/arg and the ReLU-mask sums are plain per-thread loops and every global
-//                 store of a warp is one coalesced 128-byte line (MT = 2: one warp group per channel tile;
-//                 MT = 1: the two groups split the columns)
-//   warps 2,3,12-17  operand producers (256 threads, 4 neighbouring rows each): coalesced 16-byte loads issued one
-//                 k-block ahead ("raw-first"), transform, hi/lo split, 128B-swizzled st.shared, fence.proxy.async, arrive
-// Shared memory: MT = 1: 3 stages x (W 32K | X 32K) = 192 KB;  MT = 2: 2 stages x (W 64K | X 32K) = 192 KB; K-major
-// SWIZZLE_128B tiles.  The wgrad kernels further down have their own role tables.
+// (x - hi, exact), so that   Xlo*Whi + Xhi*Wlo + Xhi*Whi   carries ~21 mantissa bits — fp32-grade accuracy, which
+// the 1e-4 parity bar needs and a single TF32 pass (10 bits) cannot give.  The role tables are with the kernels below.
 #include "common.cuh"
 #include "lift.cuh"
 #include "tc_ptx.cuh"
@@ -32,14 +16,10 @@
 
 namespace {
 
-constexpr int TC_STAGES = 3;
-constexpr int STAGE_BYTES = 4 * TILE_BYTES;            // Whi | Wlo | Xhi | Xlo
-
 // ---- operand descriptions (same semantics as ActIn / DyIn in pwmlp.cu) --------------------------------------
 // `prep(k)` fetches the per-channel coefficients of the thread's 4 channels once per k-block; `row(p)` then costs one
 // (forward) or two (dgrad) 16-byte loads.
 struct TcAct {
-    static constexpr int DEPTH = 2;   // items (k-blocks) of raw loads a producer thread keeps in flight
     const float* x; int ld; const float* scale; const float* shift; int relu;
     struct Coef { float4 s, t; bool on; };
     // raw operand rows of one thread for one k-block: rows p0 + i * stride, i < R
@@ -82,7 +62,6 @@ struct TcAct {
 // Same interface as TcAct; loads stay "raw-first": gidx -> Z row (two dependent loads; the row indices are fetched one call
 // ahead), the s.u terms / BN / ReLU happen in finish().
 struct TcLift {
-    static constexpr int DEPTH = 1;
     LiftView lv; const float* scale; const float* shift; int relu;
     int la;   // positions between two consecutive fetches of a thread (wgrad: the k-block length; 0: same rows again, next k-block)
     struct Coef { float4 s, t, u0, u1, u2, u3; bool on; };
@@ -158,7 +137,6 @@ struct TcLift {
 };
 
 struct TcDy {
-    static constexpr int DEPTH = 1;   // 32 raw registers per item: no room for a second one under the 96-register cap
     const float* g; int ldg; const float* y; int ldy; const float* a; const float* b; const float* cc;
     const float* dpool; const int32_t* sel; int S; int ldp;
     int sh;   // S == 1 << sh (pooling group sizes are powers of two on this path)
@@ -375,7 +353,7 @@ struct TcDgradEpi {
         }
     }
     // (an L2 prefetch of these rows one tile ahead was measured: 7-15 % slower, it competes with the loader's own window)
-    // issue the previous layer's raw outputs for this column group before waiting on TMEM (independent loads)
+    // issue the previous layer's raw outputs for this column group before reading the staged accumulators (independent loads)
     __device__ __forceinline__ void prefetch(int ch, int Nw, int pbase, int P) {
         if (ch >= Nw) return;
         if constexpr (LIFT) { prefetch_lift(ch, pbase, pbase & (TC_N - 1), P); return; }
@@ -440,175 +418,143 @@ struct TcDgradEpi {
 };
 
 // ------------------------------------------------------------------------------------------------------------
-// MT = number of 128-channel tiles one CTA accumulates for the same 128 positions (1 or 2).  With MT = 2 the
-// activation tile is produced once for 256 output channels: producer and epilogue work per MMA halve.
-//   warps: 0 MMA issuer (+TMEM alloc) | 1 weight streamer | 4-7, 8-11 epilogue | 2,3,12-17 producers   (576 threads)
-//   MT=2: epilogue warps 4-7 own channel tile 0, warps 8-11 tile 1 (all 128 columns each)
-//   MT=1: warps 4-7 take columns 0-63, warps 8-11 columns 64-127 of the single tile
-template <int MT> struct TcCfg {
-    static constexpr int STAGES = MT == 2 ? 2 : 3;
-    static constexpr int STAGE_BYTES_ = (2 * MT + 2) * TILE_BYTES;      // MT x (Whi|Wlo) | Xhi | Xlo
-    static constexpr int SMEM = STAGES * STAGE_BYTES_ + 1024 + 256 + 1024 + 4096;   // + alignment | barriers | gidx + s slices (lifted dgrad)
-    static constexpr uint32_t TMEM = MT == 2 ? 512 : 256;
-};
-constexpr int TC2_THREADS = 576;   // 18 warps: 0 MMA | 1 weights | 2,3,12-17 producers | 4-11 epilogue
+// pw_tc_kernel: one persistent CTA per SM and 128-channel tile; every role walks the same static sequence of 128-position
+// tiles.  512 threads = 16 warps:
+//   warps 0-3, 4-7  two consumer warpgroups.  Warpgroup h multiplies positions h*64 .. h*64+63 of the tile by the 128
+//                   channels of the weight tile (wgmma m64n128k8, 3xTF32: 12 per k-block, accumulators in registers),
+//                   stages the result in shared memory as [channel][position] and runs the epilogue on it: thread = one
+//                   output channel walking 64 positions in groups of 16, so the batch statistics, the group max/min/arg and
+//                   the ReLU-mask sums are plain per-thread loops and every global store of a warp is one coalesced line
+//   warps 8-15      operand producers (256 threads, 4 neighbouring rows each): coalesced 16-byte loads issued one k-block
+//                   ahead ("raw-first"), transform, hi/lo split, 128B-swizzled st.shared, fence.proxy.async, arrive.
+//                   Producer thread 0 also streams the stage's pre-tiled, pre-swizzled weight image (hi|lo, 32 KB per k-block,
+//                   written once per call by stack.cu's pack kernel) with cp.async.bulk onto the stage's "full" barrier, and
+//                   asks for the next position tile's rows with cp.async.bulk.prefetch.L2.  (A 17th warp for that would
+//                   cap every thread at 96 registers and make the consumers spill.)
+// Shared memory: 2 stages x (Whi | Wlo | Xhi | Xlo, 64 KB) + 2 x 34 KB epilogue staging + barriers / lifted slices = 202 KB.
+constexpr int TC_STAGES = 2;
+constexpr int TC_STAGE_BYTES = 4 * TILE_BYTES;         // Whi | Wlo | Xhi | Xlo
+constexpr int TC_EPI_LD = 68;                          // floats per staged channel row: 64 positions + 4 (no bank conflicts
+                                                       // for the accumulator stores nor for the epilogue's float4 reads)
+constexpr int TC_EPI_BYTES = TC_M * TC_EPI_LD * 4;     // one warpgroup's staging
+constexpr int TC_THREADS = 512;
+constexpr int TC_SMEM = TC_STAGES * TC_STAGE_BYTES + 2 * TC_EPI_BYTES + 1024 + 256 + 1024 + 4096;   // + alignment | barriers |
+                                                                                                    //   gidx + s slices (lifted dgrad)
 
-// dbg (profiling experiments only; results are wrong when set): 1 = stream weights for the first tile only,
-// 2 = producers skip the global loads, 4 = epilogue skips its global stores / loads
-template <int MT, class BLoad, class Epi>
-__global__ void __launch_bounds__(TC2_THREADS, 1)
+// accumulators of one warpgroup (m64 x N, rows = positions, columns = channels) -> stg[channel * TC_EPI_LD + position]
+template <int R>
+__device__ __forceinline__ void stage_acc(const float (&acc)[R], float* stg, int ld) {
+    const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll
+    for (int i = 0; i < R; ++i) {
+        const int row = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        stg[col * ld + row] = acc[i];
+    }
+}
+
+// dbg (profiling experiments only; results are wrong when set): 2 = producers skip the global loads, 4 = epilogue skips its
+// global stores / loads
+template <class BLoad, class Epi>
+__global__ void __launch_bounds__(TC_THREADS, 1)
     pw_tc_kernel(BLoad bl, const uint8_t* __restrict__ wtiles, int P, int K, int Nw, int nkb, Epi epi, int dbg, int rev) {
-    using C = TcCfg<MT>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES_);
-    uint64_t* full = bars;                        // [STAGES]  producers + weight copy -> MMA
-    uint64_t* empty = bars + C::STAGES;           // [STAGES]  MMA (tcgen05.commit) -> producers
-    uint64_t* tfull = bars + 2 * C::STAGES;       // [2]       MMA -> epilogue
-    uint64_t* tempty = bars + 2 * C::STAGES + 2;  // [2]       epilogue -> MMA
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * C::STAGES + 4);
+    uint8_t* tail = smem + TC_STAGES * TC_STAGE_BYTES + 2 * TC_EPI_BYTES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(tail);      // [STAGES]  producers (+ weight copy) -> consumers
+    uint64_t* empty = full + TC_STAGES;                       // [STAGES]  consumers (lane 0 of each of the 8 warps) -> producers
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int mt0 = blockIdx.y * MT;              // first 128-channel tile of this CTA
+    const int mt0 = blockIdx.y;                   // 128-channel tile of this CTA
     const int n_ptiles = (P + TC_N - 1) / TC_N;
     // `rev`: walk the position tiles from the last to the first.  Consecutive layers alternate the direction, so a layer
-    // starts on the part of its input that the previous kernel touched last and that is still resident in the 126 MB L2.
+    // starts on the part of its input that the previous kernel touched last and that is still resident in the 50 MB L2.
     auto tile_of = [&](int t) { return rev ? n_ptiles - 1 - t : t; };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < C::STAGES; ++s) {
+        for (int s = 0; s < TC_STAGES; ++s) {
             o3d_mbar_init(full + s, 256 + 1);
-            o3d_mbar_init(empty + s, 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            o3d_mbar_init(tfull + a, 1);
-            o3d_mbar_init(tempty + a, 256);
+            o3d_mbar_init(empty + s, 8);
         }
         o3d_fence_mbar_init();
     }
-    if (warp == 0) tmem_alloc(tmem_slot, C::TMEM);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        // ===================================================== MMA issuer
-        const uint32_t idesc = make_idesc(TC_M, TC_N);
-        int stage = 0, phase = 0, acc = 0, aphase = 0;
-        for (int t = blockIdx.x; t < n_ptiles; t += gridDim.x) {
-            o3d_mbar_wait(tempty + acc, aphase ^ 1);
-            tc_fence_after();
-            for (int kb = 0; kb < nkb; ++kb) {
-                o3d_mbar_wait(full + stage, phase);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t sb = o3d_smem_u32(smem + stage * C::STAGE_BYTES_);
-                    const uint64_t xhi = make_desc(sb + 2 * MT * TILE_BYTES), xlo = make_desc(sb + (2 * MT + 1) * TILE_BYTES);
-#pragma unroll
-                    for (int m = 0; m < MT; ++m) {
-                        const uint32_t d_tmem = tmem_base + (uint32_t)((acc * MT + m) * TC_N);
-                        const uint64_t whi = make_desc(sb + 2 * m * TILE_BYTES), wlo = make_desc(sb + (2 * m + 1) * TILE_BYTES);
-#pragma unroll
-                        for (int ks = 0; ks < TC_K / 8; ++ks) {
-                            const uint64_t adv = (uint64_t)((ks * 32) >> 4);   // +32 bytes along K inside the 128B swizzle row
-                            umma_tf32(d_tmem, wlo + adv, xhi + adv, idesc, (kb | ks) != 0);
-                            umma_tf32(d_tmem, whi + adv, xlo + adv, idesc, 1u);
-                            umma_tf32(d_tmem, whi + adv, xhi + adv, idesc, 1u);
-                        }
-                    }
-                    umma_commit(empty + stage);                           // frees the stage when these MMAs retire
-                    if (kb == nkb - 1) umma_commit(tfull + acc);          // accumulators complete -> epilogue
-                }
-                __syncwarp();
-                if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-            }
-            if (++acc == 2) { acc = 0; aphase ^= 1; }
-        }
-    } else if (warp == 1) {
-        // ===================================================== weight-tile streamer (bulk copy engine)
-        if (lane == 0) {
-            int stage = 0, phase = 0;
-            if (!(dbg & 8) && (int)blockIdx.x < n_ptiles) {
-                bl.prefetch_rows(tile_of(blockIdx.x) * TC_N, TC_N, P);
-            }
-            for (int t = blockIdx.x; t < n_ptiles; t += gridDim.x) {
-                if (!(dbg & 8) && t + (int)gridDim.x < n_ptiles) {
-                    bl.prefetch_rows(tile_of(t + (int)gridDim.x) * TC_N, TC_N, P);   // next tile of this CTA -> L2
-                }
-                for (int kb = 0; kb < nkb; ++kb) {
-                    o3d_mbar_wait(empty + stage, phase ^ 1);
-                    if ((dbg & 1) && t != (int)blockIdx.x) {
-                        o3d_mbar_arrive(full + stage);
-                    } else {
-                        o3d_mbar_expect_tx(full + stage, MT * 2 * TILE_BYTES);
-#pragma unroll
-                        for (int m = 0; m < MT; ++m)
-                            o3d_bulk_g2s(smem + stage * C::STAGE_BYTES_ + 2 * m * TILE_BYTES,
-                                         wtiles + ((size_t)(mt0 + m) * nkb + kb) * (2 * TILE_BYTES), 2 * TILE_BYTES, full + stage);
-                    }
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp >= 4 && warp < 12) {
-        // ===================================================== epilogue (8 warps)
-        const int q = warp & 3;                       // TMEM lane quarter this warp may access
-        const int grp = (warp - 4) >> 2;              // 0: warps 4-7, 1: warps 8-11
-        const int m = MT == 2 ? grp : 0;              // channel tile inside the CTA
-        const int cg0 = MT == 2 ? 0 : grp * 4, cg1 = MT == 2 ? 8 : grp * 4 + 4;   // 16-column groups to handle
-        const int ch = (mt0 + m) * TC_M + q * 32 + lane;
+    if (warp < 8) {
+        // ===================================================== consumers: wgmma + epilogue (2 warpgroups)
+        const int h = warp >> 2;                      // warpgroup: positions h*64 .. h*64+63 of each tile
+        const int tw = threadIdx.x & 127;
+        const int ch = mt0 * TC_M + tw;
+        float* stg = reinterpret_cast<float*>(smem + TC_STAGES * TC_STAGE_BYTES + h * TC_EPI_BYTES);
+        int32_t* gsm = reinterpret_cast<int32_t*>(tail + 256);           // [2][TC_N] row indices
+        float4* ssm = reinterpret_cast<float4*>(tail + 256 + 1024);      // [2][TC_N] per-position scalars
         epi.begin(ch, Nw);
         const int Nw_e = (dbg & 4) ? 0 : Nw;          // dbg: ch >= Nw_e -> the epilogue body is skipped
-        int acc = 0, aphase = 0;
-        int32_t* gsm = reinterpret_cast<int32_t*>(smem + C::STAGES * C::STAGE_BYTES_ + 256);   // [2][TC_N] row indices
-        float4* ssm = reinterpret_cast<float4*>(smem + C::STAGES * C::STAGE_BYTES_ + 256 + 1024);   // [2][TC_N] per-position scalars
+        int stage = 0, phase = 0, buf = 0;
         for (int t = blockIdx.x; t < n_ptiles; t += gridDim.x) {
             const int pt0 = tile_of(t) * TC_N;
             {
-                // lifted previous layer: stage the tile's 128 row indices (warps 4-7) and per-position scalars (warps 8-11) once,
-                // all 8 epilogue warps read them; the named barrier of tile t+1 orders the re-use of the slices by tile t+2
+                // lifted previous layer: stage the tile's 128 row indices (warpgroup 0) and per-position scalars (warpgroup 1)
+                // once, both read them; the named barrier of tile t+1 orders the re-use of the slices by tile t+2
                 const int32_t* gi = epi.lift_gidx();
                 const float* si = epi.lift_s();
                 if (gi || si) {
-                    const int pp = min(pt0 + q * 32 + lane, P - 1);
-                    if (gi && grp == 0) gsm[acc * TC_N + q * 32 + lane] = __ldg(gi + pp);
-                    if (si && grp == 1) ssm[acc * TC_N + q * 32 + lane] = ld4g(si + (size_t)pp * 4);
+                    const int pp = min(pt0 + tw, P - 1);
+                    if (gi && h == 0) gsm[buf * TC_N + tw] = __ldg(gi + pp);
+                    if (si && h == 1) ssm[buf * TC_N + tw] = ld4g(si + (size_t)pp * 4);
                     asm volatile("bar.sync 1, 256;" ::: "memory");
-                    epi.set_tile(gsm + acc * TC_N, ssm + acc * TC_N);
+                    epi.set_tile(gsm + buf * TC_N, ssm + buf * TC_N);
                 }
             }
-            epi.prefetch(ch, Nw_e, pt0 + cg0 * 16, P);
-            o3d_mbar_wait(tfull + acc, aphase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((acc * MT + m) * TC_N);
-#pragma unroll 1
-            for (int cg = cg0; cg < cg1; ++cg) {
-                uint32_t r[16];
-                tmem_ld16(taddr + cg * 16, r);
-                epi.group(r, ch, Nw_e, pt0 + cg * 16, P);
-                if (cg + 1 < cg1) epi.prefetch(ch, Nw_e, pt0 + (cg + 1) * 16, P);
+            const int pb = pt0 + h * 64;
+            epi.prefetch(ch, Nw_e, pb, P);
+            float acc[64];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+            for (int kb = 0; kb < nkb; ++kb) {
+                o3d_mbar_wait(full + stage, phase);
+                const uint32_t sb = o3d_smem_u32(smem + stage * TC_STAGE_BYTES);
+                const uint32_t xb = sb + 2 * TILE_BYTES + h * (TILE_BYTES / 2);    // rows h*64.. of the activation tile
+                wgmma_fence_acc(acc);
+                wgmma_fence();
+                wgmma_3xtf32_kblock<128>(acc, make_desc(xb), make_desc(xb + TILE_BYTES), make_desc(sb), make_desc(sb + TILE_BYTES),
+                                         kb == 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(acc);
+                if (lane == 0) o3d_mbar_arrive(empty + stage);
+                if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
             }
-            tc_fence_before();
-            o3d_mbar_arrive(tempty + acc);
-            if (++acc == 2) { acc = 0; aphase ^= 1; }
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + h) : "memory");     // the previous tile's epilogue is done with stg
+            stage_acc(acc, stg, TC_EPI_LD);
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + h) : "memory");
+            const float* row = stg + tw * TC_EPI_LD;
+#pragma unroll 1
+            for (int cg = 0; cg < 4; ++cg) {
+                uint32_t r[16];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float4 v = *reinterpret_cast<const float4*>(row + cg * 16 + 4 * j);
+                    r[4 * j] = __float_as_uint(v.x); r[4 * j + 1] = __float_as_uint(v.y);
+                    r[4 * j + 2] = __float_as_uint(v.z); r[4 * j + 3] = __float_as_uint(v.w);
+                }
+                epi.group(r, ch, Nw_e, pb + cg * 16, P);
+                if (cg + 1 < 4) epi.prefetch(ch, Nw_e, pb + (cg + 1) * 16, P);
+            }
+            buf ^= 1;
         }
         epi.end(ch, Nw);
     } else {
         // ===================================================== activation-operand producers (8 warps, 256 threads)
         // Per k-block: [raw rows of kb already in registers] -> wait for the stage -> transform, hi/lo split, swizzled
         // st.shared -> fence + arrive -> issue the raw loads of kb+1 (all back to back, nothing depends on them until
-        // the next iteration, so they fly while the MMA warp works through the stages ahead).
-        const int pw = warp < 4 ? warp - 2 : warp - 10;   // producer warp 0..7
-        const int pt = pw * 32 + lane;                    // 0..255
+        // the next iteration, so they fly while the consumers work through the stages ahead).
+        const int pt = (warp - 8) * 32 + lane;            // 0..255
         const int chunk = pt & 7;                         // 16-byte chunk (4 channels) inside the 128-byte row
         const int row0 = (pt >> 3) * 4;                   // 4 neighbouring rows row0 + i, i < 4 (one pooling group)
         int stage = 0, phase = 0;
         if (dbg & 2) P = 0;                               // dbg: nothing is loaded
-        // The (tile, k-block) nest is walked as one flat sequence of items so that the raw loads of the items ahead — also
-        // when they belong to the next position tile — are in flight while the current one is being stored.  A loader with
-        // DEPTH == 2 (the forward operand: 16 raw registers per item) keeps two items in flight per thread: one k-block
-        // of loads per thread does not cover the memory latency at two pipeline stages (tensor pipe 61 % busy).
+        // The (tile, k-block) nest is walked as one flat sequence of items so that the raw loads of the item ahead — also
+        // when it belongs to the next position tile — are in flight while the current one is being stored.
         struct Cur { int t, kb, p0; };
         auto advance = [&](Cur& c) {
             if (++c.kb == nkb) {
@@ -624,440 +570,171 @@ __global__ void __launch_bounds__(TC2_THREADS, 1)
             cf = bl.prep(k, K);
             if (P > 0) bl.fetch(r, c.p0 + row0, 1, P, k, K);
         };
-        auto emit = [&](const Batch4& r, const typename BLoad::Coef& cf, const Cur& c) {
+        Cur c0{(int)blockIdx.x, 0, 0};
+        if (c0.t < n_ptiles) c0.p0 = tile_of(c0.t) * TC_N;
+        Batch4 r0{};      // value-initialised: TcLift keeps a look-ahead tag in the batch
+        typename BLoad::Coef f0 = bl.prep(chunk * 4, K);
+        issue(r0, f0, c0);
+        if (pt == 0 && c0.t < n_ptiles) bl.prefetch_rows(c0.p0, TC_N, P);
+        while (c0.t < n_ptiles) {
             o3d_mbar_wait(empty + stage, phase ^ 1);
-            uint8_t* xhi = smem + stage * C::STAGE_BYTES_ + 2 * MT * TILE_BYTES;
+            if (pt == 0) {
+                o3d_mbar_expect_tx(full + stage, 2 * TILE_BYTES);
+                o3d_bulk_g2s(smem + stage * TC_STAGE_BYTES, wtiles + ((size_t)mt0 * nkb + c0.kb) * (2 * TILE_BYTES), 2 * TILE_BYTES,
+                             full + stage);
+                const int tn = c0.t + (int)gridDim.x;
+                if (c0.kb == 0 && tn < n_ptiles) bl.prefetch_rows(tile_of(tn) * TC_N, TC_N, P);   // next tile of this CTA -> L2
+            }
+            uint8_t* xhi = smem + stage * TC_STAGE_BYTES + 2 * TILE_BYTES;
             uint8_t* xlo = xhi + TILE_BYTES;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                const float4 v = P > 0 ? bl.finish(r, cf, i, c.p0 + row0 + i, P) : make_float4(0.f, 0.f, 0.f, 0.f);
+                const float4 v = P > 0 ? bl.finish(r0, f0, i, c0.p0 + row0 + i, P) : make_float4(0.f, 0.f, 0.f, 0.f);
                 const uint32_t off = sw128(row0 + i, chunk);
                 *reinterpret_cast<float4*>(xhi + off) = hi_part(v);
                 *reinterpret_cast<float4*>(xlo + off) = lo_part(v);
             }
             o3d_fence_proxy_async();              // generic-proxy stores -> visible to the tensor core (async proxy)
             o3d_mbar_arrive(full + stage);
-            if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        };
-        Cur c0{(int)blockIdx.x, 0, 0};
-        if (c0.t < n_ptiles) c0.p0 = tile_of(c0.t) * TC_N;
-        Batch4 r0{};      // value-initialised: TcLift keeps a look-ahead tag in the batch
-        typename BLoad::Coef f0 = bl.prep(chunk * 4, K);
-        issue(r0, f0, c0);
-        if constexpr (BLoad::DEPTH == 2 && MT == 2) {   // measured: +5 % on the 256-channel layers, -8 % on the narrow ones
-            Cur c1 = c0;
-            if (c1.t < n_ptiles) advance(c1);
-            Batch4 r1{};
-            typename BLoad::Coef f1 = f0;
-            issue(r1, f1, c1);
-            while (c0.t < n_ptiles) {
-                emit(r0, f0, c0);
-                c0 = c1;
-                advance(c0);                      // two items ahead of the one just stored
-                issue(r0, f0, c0);
-                if (c1.t >= n_ptiles) break;
-                emit(r1, f1, c1);
-                c1 = c0;
-                if (c1.t < n_ptiles) advance(c1);
-                issue(r1, f1, c1);
-            }
-        } else {
-            while (c0.t < n_ptiles) {
-                emit(r0, f0, c0);
-                advance(c0);
-                issue(r0, f0, c0);
-            }
+            if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
+            advance(c0);
+            issue(r0, f0, c0);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, C::TMEM);
     }
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// wgrad on the tensor core:  dW[m, n] += sum_p dY[p, m] * X[p, n]  over this CTA's slice of positions.
-// Both operands are position-major in global memory (channels contiguous), i.e. "MN-major" for a GEMM whose K is the
-// position index.  For 32-bit (tf32) MN-major operands the tensor core accepts exactly one shared-memory layout,
-// SWIZZLE_128B_BASE32B (cute::UMMA::Layout_MN_SW128_32B_Atom): atoms of 4 positions x 32 channels (512 B; one
-// position = one 128-byte row), the 32-byte chunk index XOR-ed with (position % 4).  The producers copy coalesced
-// float4 rows straight into it — no transposition — and the instruction descriptor marks A and B as MN-major.
-//   tile [32 positions x 128 channels]:  atom(cb, pq) at (cb + 4*pq) * 512,  cb = channel/32, pq = position/4
-//   descriptor for k-step ks (8 positions = 2 atoms along K): start = tile + ks*4096,
-//   LBO = 512 (next 32-channel block), SBO = 2048 (next 4 positions)
-constexpr int WG_THREADS = 640;   // warps: 0 MMA | 1 L2 prefetch | 2,3 idle | 4-11 dY producers (4-7 also epilogue) | 12-19 X producers
-constexpr int WG_SMEM = TC_STAGES * STAGE_BYTES + 1024 + 256;
+// wgrad on the tensor core:  dW[m, n] += sum_p dY[p, m] * X[p, n]  over this CTA's slice of positions, one 128 x 128 tile
+// of dW per CTA.  Both operands are position-major in global memory (channels contiguous) while wgmma takes tf32 operands
+// K-major only, K being the position here: the producers transpose while they store, writing [128 channels x 32 positions]
+// K-major SWIZZLE_128B tiles (element (c, p) at sw128(c, p / 4) + 4 (p % 4)) with 4-byte st.shared.  A warp loads 8
+// positions x 16 channels (64-byte row segments) so that its transposed stores hit 16 banks (2-way conflicts).
+//   warps 0-3, 4-7  consumers: warpgroup h accumulates rows m0 + h*64 .. of the tile (wgmma m64n128k8, 3xTF32), then writes
+//                   its partial tile: plain stores into the split-K workspace part[split][m][n] (summed in a fixed order by
+//                   wgrad_reduce_kernel: deterministic), or fp32 REDs into dW when no workspace is given
+//   warps 8-15      producers: each thread owns 4 channels x 4 positions of both operands per k-block; producer thread 0
+//                   also keeps the L2 prefetch of the slice's rows WG_AHEAD k-blocks ahead of the stores (requesting the whole
+//                   slice up front asks for more than the L2 holds across the grid, and the lines are evicted again before
+//                   their k-block comes up)
+constexpr int WG_STAGES = 3;
+constexpr int WG_AHEAD = 4;
+constexpr int WG_THREADS = 512;
+constexpr int WG_SMEM = WG_STAGES * 4 * TILE_BYTES + 1024 + 256;
 
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)(512 >> 4) << 16;    // leading byte offset: between 32-channel blocks
-    d |= (uint64_t)(2048 >> 4) << 32;   // stride byte offset : between 4-position blocks
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)1 << 61;             // SWIZZLE_128B_BASE32B
-    return d;
-}
-__host__ __device__ constexpr uint32_t make_idesc_mn(int M, int N) {
-    return make_idesc(M, N) | (1u << 15) | (1u << 16);
-}
-__device__ __forceinline__ uint32_t sw128_mn(int p_local, int c4) {   // c4 = float4 index along the 128 channels
-    const int cb = c4 >> 3, c32 = (c4 & 7) >> 1, half = c4 & 1, j0 = p_local & 3;
-    return (uint32_t)((cb + 4 * (p_local >> 2)) * 512 + j0 * 128 + ((c32 ^ j0) << 5) + (half << 4));
-}
-
-// One operand's producer loop of the wgrad kernel: raw loads of k-block kb+1 are issued right after k-block kb has been
-// handed to the tensor core; transform + hi/lo split happen at store time.
-template <class L, class KPos>
-__device__ __forceinline__ void wgrad_produce(const L& ld, uint8_t* smem, int tile_off, uint64_t* full, uint64_t* empty,
-                                              int pt, int c_base, int CH, KPos kpos, int pend, int nkb, int dbg) {
-    const int c4 = pt & 31, prow0 = pt >> 5;      // 256 threads per operand: rows prow0 + 8*i, i < 4
-    const int ch0 = c_base + c4 * 4;
-    const typename L::Coef cf = ld.prep(ch0, CH);
-    typename L::template Batch<4> raw = {};
-    int stage = 0, phase = 0;
-    if (nkb > 0 && !(dbg & 2)) ld.fetch(raw, kpos(0) + prow0, 8, pend, ch0, CH);
-    for (int kb = 0; kb < nkb; ++kb) {
-        o3d_mbar_wait(empty + stage, phase ^ 1);
-        uint8_t* hi = smem + stage * STAGE_BYTES + tile_off;
-        uint8_t* lo = hi + TILE_BYTES;
+template <class L>
+__device__ __forceinline__ void store_transposed(const L& ld, const typename L::template Batch<4>& raw, const typename L::Coef& cf,
+                                                 uint8_t* hi, int c_local, int p_first, int prow0, int pend) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float4 v = ld.finish(raw, cf, i, kpos(kb) + prow0 + 8 * i, pend);
-            const uint32_t off = sw128_mn(prow0 + 8 * i, c4);
-            *reinterpret_cast<float4*>(hi + off) = hi_part(v);
-            *reinterpret_cast<float4*>(lo + off) = lo_part(v);
-        }
-        o3d_fence_proxy_async();
-        o3d_mbar_arrive(full + stage);
-        if (kb + 1 < nkb && !(dbg & 2)) ld.fetch(raw, kpos(kb + 1) + prow0, 8, pend, ch0, CH);
-        if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-    }
-}
-
-
-// L2 prefetch of one CTA's slice of position rows, paced by the MMA warp's progress (rows consumed, published in shared
-// memory): at most WINDOW rows ahead.  Prefetching the whole slice up front asks for several hundred MB across the grid —
-// more than the 126 MB L2 — and the lines are evicted again before their k-block comes up (measured: DRAM reads 1.7x the
-// algorithmic bytes with a 384-row window, L2 hit rate 11 %).
-template <class LA, class LB>
-__device__ __forceinline__ void paced_prefetch(const LA& da, const LB& xb, int pbeg, int pend, volatile int* progress) {
-    constexpr int CH = 32, WINDOW = 4 * CH;   // 148 CTAs x 3 operands x 128 rows x <= 1 KB stays well inside the L2
-    int issued = pbeg;
-    while (issued < pend) {
-        const int target = pbeg + *progress + WINDOW;
-        if (issued < target) {
-            da.prefetch_rows(issued, CH, pend);
-            xb.prefetch_rows(issued, CH, pend);
-            issued += CH;
-        } else {
-            __nanosleep(256);
+    for (int i = 0; i < 4; ++i) {
+        const int pl = prow0 + 8 * i;
+        const float4 v = ld.finish(raw, cf, i, p_first + pl, pend);
+        const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const uint32_t off = sw128(c_local + j, pl >> 2) + (uint32_t)((pl & 3) * 4);
+            const float h = hi1(e[j]);
+            *reinterpret_cast<float*>(hi + off) = h;
+            *reinterpret_cast<float*>(hi + TILE_BYTES + off) = e[j] - h;
         }
     }
 }
 
 template <class XB>
 __global__ void __launch_bounds__(WG_THREADS, 1)
-    pw_wgrad_tc_kernel(TcDy da, XB xb, int P, int M, int N, int chunk, float* __restrict__ dW, int lddw, int dbg) {
+    pw_wgrad_tc_kernel(TcDy da, XB xb, int P, int M, int N, int chunk, float* __restrict__ dW, int lddw, float* __restrict__ part,
+                       int dbg) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TC_STAGES * STAGE_BYTES);
-    uint64_t* full = bars;
-    uint64_t* empty = bars + TC_STAGES;
-    uint64_t* tfull = bars + 2 * TC_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * TC_STAGES + 1);
-    volatile int* progress = reinterpret_cast<volatile int*>(tmem_slot + 1);   // rows handed to the tensor core so far
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * 4 * TILE_BYTES);
+    uint64_t* empty = full + WG_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.z * TC_M, n0 = blockIdx.y * TC_N;
-    // every split owns one contiguous slice of positions (DRAM-friendly; a round-robin deal of k-blocks measured slower)
+    // every split owns one contiguous slice of positions (DRAM-friendly)
     const int pbeg = blockIdx.x * chunk, pend = min(P, pbeg + chunk);
     const int nkb = pend > pbeg ? (pend - pbeg + TC_K - 1) / TC_K : 0;
     auto kpos = [&](int i) { return pbeg + i * TC_K; };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < TC_STAGES; ++s) {
-            o3d_mbar_init(full + s, 512);
-            o3d_mbar_init(empty + s, 1);
+        for (int s = 0; s < WG_STAGES; ++s) {
+            o3d_mbar_init(full + s, 256);
+            o3d_mbar_init(empty + s, 8);
         }
-        o3d_mbar_init(tfull, 1);
-        *progress = 0;
         o3d_fence_mbar_init();
     }
-    if (warp == 0) tmem_alloc(tmem_slot, 128);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        const uint32_t idesc = (dbg & 16) ? make_idesc(TC_M, TC_N) : make_idesc_mn(TC_M, TC_N);
+    if (warp < 8) {
+        const int h = warp >> 2, w = warp & 3;
+        float acc[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
         int stage = 0, phase = 0;
         for (int kb = 0; kb < nkb; ++kb) {
             o3d_mbar_wait(full + stage, phase);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sb = o3d_smem_u32(smem + stage * STAGE_BYTES);
-#pragma unroll
-                for (int pb = 0; pb < TC_K / 8; ++pb) {
-                    const uint32_t o = pb * 4096;
-                    const uint64_t ahi = make_desc_mn(sb + o), alo = make_desc_mn(sb + TILE_BYTES + o);
-                    const uint64_t bhi = make_desc_mn(sb + 2 * TILE_BYTES + o), blo = make_desc_mn(sb + 3 * TILE_BYTES + o);
-                    if (dbg & 32) continue;
-                    umma_tf32(tmem_base, alo, bhi, idesc, (kb | pb) != 0);
-                    umma_tf32(tmem_base, ahi, blo, idesc, 1u);
-                    umma_tf32(tmem_base, ahi, bhi, idesc, 1u);
-                }
-                umma_commit(empty + stage);
-                if (kb == nkb - 1) umma_commit(tfull);
-                *progress = (kb + 1) * TC_K;
-            }
-            __syncwarp();
-            if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
+            const uint32_t sb = o3d_smem_u32(smem + stage * 4 * TILE_BYTES);
+            const uint32_t ab = sb + h * (TILE_BYTES / 2);                 // dY rows (channels) m0 + h*64 ..
+            wgmma_fence_acc(acc);
+            wgmma_fence();
+            if (!(dbg & 32))
+                wgmma_3xtf32_kblock<128>(acc, make_desc(ab), make_desc(ab + TILE_BYTES), make_desc(sb + 2 * TILE_BYTES),
+                                         make_desc(sb + 3 * TILE_BYTES), kb == 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
+            if (lane == 0) o3d_mbar_arrive(empty + stage);
+            if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            if (dbg & 64) {   // dbg: the old behaviour, whole slice requested up front
-                for (int p = pbeg; p < pend; p += 512) {
-                    da.prefetch_rows(p, 512, pend);
-                    xb.prefetch_rows(p, 512, pend);
-                }
-            } else {
-                paced_prefetch(da, xb, pbeg, pend, progress);
-            }
-        }
-    } else if (warp >= 4) {
-        // producers, 16 warps: 4-11 -> A (dY, channels m0..), 12-19 -> B (X, channels n0..); each thread owns 4 of a
-        // k-block's 32 rows.  (One warp per scheduler and operand could not issue the split + swizzled stores fast enough.)
-        const int pt = (threadIdx.x - 128) & 255;
-        if (warp < 12) wgrad_produce(da, smem, 0, full, empty, pt, m0, M, kpos, pend, nkb, dbg);
-        else wgrad_produce(xb, smem, 2 * TILE_BYTES, full, empty, pt, n0, N, kpos, pend, nkb, dbg);
-        if (warp < 8 && nkb > 0) {   // epilogue: warps 4-7 own TMEM lane quadrants 0-3
-            const int q = warp & 3;
-            const int ch = m0 + q * 32 + lane;
-            o3d_mbar_wait(tfull, 0);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-            for (int cg = 0; cg < TC_N / 32; ++cg) {
-                uint32_t r[32];
-                tmem_ld32(taddr + cg * 32, r);
-                if (ch < M) {
+        const int Mt = TC_M * (int)gridDim.z, Nt = TC_N * (int)gridDim.y;
+        float* __restrict__ out = part ? part + (size_t)blockIdx.x * Mt * Nt : nullptr;
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const int n = n0 + cg * 32 + j;
-                        if (n < N) atomicAdd(dW + (size_t)ch * lddw + n, __uint_as_float(r[j]));
-                    }
-                }
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 128);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// wgrad, wide-tile variant: one CTA accumulates a (128*MH) x (128*NH) block of dW (MH*NH accumulators = up to all 512
-// TMEM columns) over its slice of positions, 16 positions per stage.  Relative to the 128x128 kernel above every loaded
-// activation row feeds twice as many MMAs, which halves the L2->SM traffic per FLOP — the limiter of that kernel — and
-// the split-K partial tiles are written with plain coalesced stores into a workspace and summed by a second kernel
-// instead of 65k float REDs per CTA.
-//   operand tile [16 positions x 128*H channels], MN-major SWIZZLE_128B_BASE32B: atom(cb, pq) at (cb + 4*H*pq) * 512
-//   descriptor (channel half h, k-step ks): start = tile + h*2048 + ks*2*SBO, LBO = 512, SBO = 4*H*512
-// positions per pipeline stage: each producer thread must keep >= 2 float4 per operand in flight, or the bytes in flight per SM
-// (512 threads x 32 B at 16 positions x 128 channels) cap the kernel near 2.3 TB/s — measured on the 128x128 variant at the SA1
-// shapes (ncu, profiles/r2_step_dram_final.txt: 278 us for 629 MB); the single-accumulator variant therefore takes 32 positions
-template <int MH, int NH> constexpr int wg2_k() { return MH * NH == 1 ? 32 : 16; }
-constexpr int WG2_STAGES = 3;
-constexpr int WG2_THREADS = 576;   // warps: 0 MMA | 1 prefetch | 2-17 producers (4-11 also run the epilogue)
-
-template <int MH, int NH> struct Wg2Cfg {
-    static constexpr int K = wg2_k<MH, NH>();
-    static constexpr int A_BYTES = K * 128 * MH * 4;            // one of hi / lo
-    static constexpr int B_BYTES = K * 128 * NH * 4;
-    static constexpr int STAGE = 2 * A_BYTES + 2 * B_BYTES;
-    static constexpr int SMEM = WG2_STAGES * STAGE + 1024 + 256;
-    static constexpr uint32_t TMEM = (MH * NH * 128) <= 128 ? 128 : ((MH * NH * 128) <= 256 ? 256 : 512);
-};
-
-__device__ __forceinline__ uint64_t make_desc_mn2(uint32_t smem_addr, int H) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)(512 >> 4) << 16;
-    d |= (uint64_t)((4 * H * 512) >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)1 << 61;
-    return d;
-}
-template <int H>
-__device__ __forceinline__ uint32_t sw_mn2(int p_local, int c4) {   // c4 = float4 index along the 128*H channels
-    const int cb = c4 >> 3, c32 = (c4 & 7) >> 1, half = c4 & 1, j0 = p_local & 3;
-    return (uint32_t)((cb + 4 * H * (p_local >> 2)) * 512 + j0 * 128 + ((c32 ^ j0) << 5) + (half << 4));
-}
-
-template <int MH, int NH, class XB>
-__global__ void __launch_bounds__(WG2_THREADS, 1)
-    pw_wgrad_tc2_kernel(TcDy da, XB xb, int P, int M, int N, int chunk, float* __restrict__ part, int dbg) {
-    using C = Wg2Cfg<MH, NH>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + WG2_STAGES * C::STAGE);
-    uint64_t* full = bars;
-    uint64_t* empty = bars + WG2_STAGES;
-    uint64_t* tfull = bars + 2 * WG2_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * WG2_STAGES + 1);
-    volatile int* progress = reinterpret_cast<volatile int*>(tmem_slot + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.z * 128 * MH, n0 = blockIdx.y * 128 * NH;
-    const int pbeg = blockIdx.x * chunk, pend = min(P, pbeg + chunk);
-    constexpr int WG2_K = C::K;
-    const int nkb = pend > pbeg ? (pend - pbeg + WG2_K - 1) / WG2_K : 0;
-    auto kpos = [&](int i) { return pbeg + i * WG2_K; };
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < WG2_STAGES; ++s) {
-            o3d_mbar_init(full + s, 512);
-            o3d_mbar_init(empty + s, 1);
-        }
-        o3d_mbar_init(tfull, 1);
-        *progress = 0;
-        o3d_fence_mbar_init();
-    }
-    if (warp == 0) tmem_alloc(tmem_slot, C::TMEM);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        const uint32_t idesc = make_idesc_mn(TC_M, TC_N);
-        int stage = 0, phase = 0;
-        for (int kb = 0; kb < nkb; ++kb) {
-            o3d_mbar_wait(full + stage, phase);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sb = o3d_smem_u32(smem + stage * C::STAGE);
-                const uint32_t a_hi = sb, a_lo = sb + C::A_BYTES, b_hi = sb + 2 * C::A_BYTES, b_lo = b_hi + C::B_BYTES;
+        for (int i = 0; i < 64; i += 4) {
 #pragma unroll
-                for (int ks = 0; ks < WG2_K / 8; ++ks) {
-                    const uint32_t ao = ks * 2 * (4 * MH * 512), bo = ks * 2 * (4 * NH * 512);
-#pragma unroll
-                    for (int mh = 0; mh < MH; ++mh)
-#pragma unroll
-                        for (int nh = 0; nh < NH; ++nh) {
-                            const uint32_t d_tmem = tmem_base + (uint32_t)((mh * NH + nh) * 128);
-                            const uint64_t ahi = make_desc_mn2(a_hi + mh * 2048 + ao, MH), alo = make_desc_mn2(a_lo + mh * 2048 + ao, MH);
-                            const uint64_t bhi = make_desc_mn2(b_hi + nh * 2048 + bo, NH), blo = make_desc_mn2(b_lo + nh * 2048 + bo, NH);
-                            umma_tf32(d_tmem, alo, bhi, idesc, (kb | ks) != 0);
-                            umma_tf32(d_tmem, ahi, blo, idesc, 1u);
-                            umma_tf32(d_tmem, ahi, bhi, idesc, 1u);
-                        }
+            for (int rr = 0; rr < 2; ++rr) {
+                const int m = m0 + h * 64 + 16 * w + (lane >> 2) + 8 * rr, n = n0 + 8 * (i >> 2) + 2 * (lane & 3);
+                const float v0 = acc[i + 2 * rr], v1 = acc[i + 2 * rr + 1];
+                if (out) {
+                    *reinterpret_cast<float2*>(out + (size_t)m * Nt + n) = make_float2(v0, v1);   // zeros when the slice is empty
+                } else if (nkb > 0 && m < M) {
+                    if (n < N) atomicAdd(dW + (size_t)m * lddw + n, v0);
+                    if (n + 1 < N) atomicAdd(dW + (size_t)m * lddw + n + 1, v1);
                 }
-                umma_commit(empty + stage);
-                if (kb == nkb - 1) umma_commit(tfull);
-                *progress = (kb + 1) * WG2_K;
-            }
-            __syncwarp();
-            if (++stage == WG2_STAGES) { stage = 0; phase ^= 1; }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            if (dbg & 64) {
-                for (int p = pbeg; p < pend; p += 512) {
-                    da.prefetch_rows(p, 512, pend);
-                    xb.prefetch_rows(p, 512, pend);
-                }
-            } else {
-                paced_prefetch(da, xb, pbeg, pend, progress);
             }
         }
     } else {
-        // producers (16 warps, 2-17): every thread serves both operands, raw loads first
-        const int pt = threadIdx.x - 64;                                // 0..511
-        constexpr int CA = 32 * MH, CB = 32 * NH;                       // float4 per position row
-        constexpr int RA = WG2_K * CA / 512, RB = WG2_K * CB / 512;     // float4 per thread per stage (1 or 2)
-        const int ca4 = pt % CA, pa0 = pt / CA, sa = 512 / CA;          // A: rows pa0 + sa*i
-        const int cb4 = pt % CB, pb0 = pt / CB, sbs = 512 / CB;
-        const TcDy::Coef cfa = da.prep(m0 + ca4 * 4, M);
-        const typename XB::Coef cfb = xb.prep(n0 + cb4 * 4, N);
-        TcDy::Batch<RA> ra = {};
-        typename XB::template Batch<RB> rb = {};
+        // producers: 8 warps x (8 positions x 4 float4); thread: channels 4*c4 .. 4*c4+3, positions prow0 + 8*i, i < 4
+        const int pw = warp - 8;
+        const int c4 = pw * 4 + (lane & 3), prow0 = lane >> 2;
+        const bool pt0 = pw == 0 && lane == 0;
+        TcDy::Batch<4> ra = {};
+        typename XB::template Batch<4> rb = {};
         auto fetch = [&](int kb) {
             if (dbg & 2) return;
-            da.fetch(ra, kpos(kb) + pa0, sa, pend, m0 + ca4 * 4, M);
-            xb.fetch(rb, kpos(kb) + pb0, sbs, pend, n0 + cb4 * 4, N);
+            da.fetch(ra, kpos(kb) + prow0, 8, pend, m0 + c4 * 4, M);
+            xb.fetch(rb, kpos(kb) + prow0, 8, pend, n0 + c4 * 4, N);
+        };
+        auto prefetch = [&](int kb) {
+            if (pt0 && kb < nkb) {
+                da.prefetch_rows(kpos(kb), TC_K, pend);
+                xb.prefetch_rows(kpos(kb), TC_K, pend);
+            }
         };
         int stage = 0, phase = 0;
+        for (int kb = 0; kb < WG_AHEAD; ++kb) prefetch(kb);
         if (nkb > 0) fetch(0);
         for (int kb = 0; kb < nkb; ++kb) {
+            prefetch(kb + WG_AHEAD);
             o3d_mbar_wait(empty + stage, phase ^ 1);
-            uint8_t* a_hi = smem + stage * C::STAGE;
-            uint8_t* a_lo = a_hi + C::A_BYTES;
-            uint8_t* b_hi = a_hi + 2 * C::A_BYTES;
-            uint8_t* b_lo = b_hi + C::B_BYTES;
-#pragma unroll
-            for (int i = 0; i < RA; ++i) {
-                const int pl = pa0 + sa * i;
-                const float4 v = da.finish(ra, cfa, i, kpos(kb) + pl, pend);
-                const uint32_t off = sw_mn2<MH>(pl, ca4);
-                *reinterpret_cast<float4*>(a_hi + off) = hi_part(v);
-                *reinterpret_cast<float4*>(a_lo + off) = lo_part(v);
-            }
-#pragma unroll
-            for (int i = 0; i < RB; ++i) {
-                const int pl = pb0 + sbs * i;
-                const float4 v = xb.finish(rb, cfb, i, kpos(kb) + pl, pend);
-                const uint32_t off = sw_mn2<NH>(pl, cb4);
-                *reinterpret_cast<float4*>(b_hi + off) = hi_part(v);
-                *reinterpret_cast<float4*>(b_lo + off) = lo_part(v);
-            }
+            uint8_t* sbase = smem + stage * 4 * TILE_BYTES;
+            // the per-channel coefficients are re-read (L1-resident) per k-block: kept live across the loop they push the
+            // lifted operand's producer past the 128-register budget
+            store_transposed(da, ra, da.prep(m0 + c4 * 4, M), sbase, c4 * 4, kpos(kb), prow0, pend);
+            store_transposed(xb, rb, xb.prep(n0 + c4 * 4, N), sbase + 2 * TILE_BYTES, c4 * 4, kpos(kb), prow0, pend);
             o3d_fence_proxy_async();
             o3d_mbar_arrive(full + stage);
             if (kb + 1 < nkb) fetch(kb + 1);
-            if (++stage == WG2_STAGES) { stage = 0; phase ^= 1; }
+            if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
         }
-        if (warp >= 4 && warp < 12) {
-            // epilogue: partial tile -> workspace part[split][m][n] (plain coalesced stores; zeros when this slice is empty)
-            const int q = warp & 3, grp = (warp - 4) >> 2;                 // grp 0: warps 4-7, 1: warps 8-11
-            const int Mt = 128 * MH * (int)gridDim.z, Nt = 128 * NH * (int)gridDim.y;
-            float* __restrict__ out = part + (size_t)blockIdx.x * Mt * Nt;
-            if (nkb > 0) {
-                o3d_mbar_wait(tfull, 0);
-                tc_fence_after();
-            }
-            for (int t = grp; t < MH * NH; t += 2) {                       // accumulators shared between the two warp groups
-                const int mh = t / NH, nh = t % NH;
-                const int row = m0 + mh * 128 + q * 32 + lane;
-                float* __restrict__ orow = out + (size_t)row * Nt + n0 + nh * 128;
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(t * 128);
-    #pragma unroll 1
-                for (int cg = 0; cg < 8; ++cg) {
-                    uint32_t r[16];
-                    if (nkb > 0) {
-                        tmem_ld16(taddr + cg * 16, r);
-                    } else {
-    #pragma unroll
-                        for (int j = 0; j < 16; ++j) r[j] = 0u;
-                    }
-    #pragma unroll
-                    for (int j = 0; j < 16; j += 4)
-                        *reinterpret_cast<float4*>(orow + cg * 16 + j) =
-                            make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-                }
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, C::TMEM);
     }
 }
 
@@ -1090,7 +767,7 @@ __global__ void __launch_bounds__(256)
     }
 }
 
-// Pre-tile a weight matrix W[rows, ld] (rows = UMMA M channels, k contiguous) into the per-(m_tile, k-block) shared-memory
+// Pre-tile a weight matrix W[rows, ld] (rows = output channels, k contiguous) into the per-(m_tile, k-block) shared-memory
 // images the kernel bulk-copies: [hi 16 KB | lo 16 KB], K-major SWIZZLE_128B, zero padded.
 __global__ void w_pretile_kernel(const float* __restrict__ W, int ld, int rows, int K, int nkb, uint8_t* __restrict__ out) {
     const int m_tile = blockIdx.y, kb = blockIdx.x;
@@ -1106,7 +783,7 @@ __global__ void w_pretile_kernel(const float* __restrict__ W, int ld, int rows, 
     }
 }
 
-int g_tc_debug = 0, g_tc_force_mt = 0;
+int g_tc_debug = 0;
 }  // namespace
 extern int o3d_g_fps_wide;
 extern int o3d_g_sa_fused_dbg;
@@ -1114,44 +791,22 @@ namespace {
 inline int ilog2_exact(int v) { int l = 0; while ((1 << l) < v) ++l; return l; }
 thread_local int g_tc_rev = 0;   // direction of the next launch (set by the stack sequencer)
 
-template <int MT, class BLoad, class Epi>
-int launch_tc_mt(BLoad bl, const uint8_t* wtiles, int P, int K, int Nw, Epi epi, cudaStream_t st, const char* name) {
-    auto kern = pw_tc_kernel<MT, BLoad, Epi>;
-    O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<MT>::SMEM), name);
-    const int mt = (Nw + TC_M - 1) / TC_M;
-    const int gy = (mt + MT - 1) / MT;
+template <class BLoad, class Epi>
+int launch_tc(BLoad bl, const uint8_t* wtiles, int P, int K, int Nw, Epi epi, cudaStream_t st, const char* name) {
+    auto kern = pw_tc_kernel<BLoad, Epi>;
+    O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM), name);
+    const int gy = (Nw + TC_M - 1) / TC_M;
     const int nkb = (K + TC_K - 1) / TC_K;
     const int n_ptiles = (P + TC_N - 1) / TC_N;
     int gx = o3d_num_sms() / gy;
     if (gx < 1) gx = 1;
     if (gx > n_ptiles) gx = n_ptiles;
-    kern<<<dim3(gx, gy), TC2_THREADS, TcCfg<MT>::SMEM, st>>>(bl, wtiles, P, K, Nw, nkb, epi, g_tc_debug, g_tc_rev);
+    kern<<<dim3(gx, gy), TC_THREADS, TC_SMEM, st>>>(bl, wtiles, P, K, Nw, nkb, epi, g_tc_debug, g_tc_rev);
     O3D_CHECK_LAUNCH(name);
     return O3D_OK;
 }
 
-// Nw must be a multiple of 128 when more than one channel tile exists with MT = 2 (weight tiles are read pairwise).
-// ... and only when there are enough position tiles to fill the machine: a B = 1 tracking frame has <= 32 of them, and two
-// CTAs per tile (MT = 1, each streaming half of the weight image) finish a layer in 10.8 us instead of 14.9 us (measured).
-inline bool tc_two_tiles(int Nw, int P = 1 << 30) {
-    const int mt = (Nw + TC_M - 1) / TC_M, n_ptiles = (P + TC_N - 1) / TC_N;
-    return mt % 2 == 0 && g_tc_force_mt != 1 && (long long)n_ptiles * mt > o3d_num_sms();
-}
-
-// MTMASK: which MT variants this (loader, epilogue) pair is instantiated for (bit 0: MT = 1, bit 1: MT = 2)
-template <int MTMASK, class BLoad, class Epi>
-int launch_tc(BLoad bl, const uint8_t* wtiles, int P, int K, int Nw, Epi epi, cudaStream_t st, const char* name) {
-    if constexpr ((MTMASK & 2) != 0) {
-        if (tc_two_tiles(Nw, P)) return launch_tc_mt<2>(bl, wtiles, P, K, Nw, epi, st, name);
-    }
-    if constexpr ((MTMASK & 1) != 0) {
-        if (!tc_two_tiles(Nw, P)) return launch_tc_mt<1>(bl, wtiles, P, K, Nw, epi, st, name);
-    }
-    o3d_set_error("%s: no kernel variant for %d output channels", name, Nw);
-    return O3D_ERR_ARG;
-}
-
-template <int LD, int MTMASK, class BLoad>
+template <int LD, class BLoad>
 int launch_fwd(const BLoad& bl, const void* wtiles, const float* bias, int P, int K, int Nw, float* y, int ldy, double* sum,
                double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp, cudaStream_t st) {
     TcFwdEpi<LD> ep{};
@@ -1159,30 +814,28 @@ int launch_fwd(const BLoad& bl, const void* wtiles, const float* bias, int P, in
     ep.S = S; ep.ymax = ymax; ep.ymin = ymin; ep.arg = arg; ep.ldp = ldp;
     ep.log2S = 0;
     while ((1 << ep.log2S) < S) ++ep.log2S;
-    return launch_tc<MTMASK>(bl, (const uint8_t*)wtiles, P, K, Nw, ep, st, "o3d_pw_fwd_tc");
+    return launch_tc(bl, (const uint8_t*)wtiles, P, K, Nw, ep, st, "o3d_pw_fwd_tc");
 }
 
-template <int LD, int MTMASK, bool LIFT = false>
+template <int LD, bool LIFT = false>
 int launch_dgrad(const TcDy& bl, const void* wtiles_t, int P, int Cout, int Cin, float* out, int ldo, const float* yprev,
                  int ldyp, const float* pscale, const float* pshift, int prelu, double* s1, double* s2y, cudaStream_t st,
                  const LiftView* lv = nullptr) {
     if constexpr (!LIFT) {
-        if (lv) return launch_dgrad<LD, MTMASK, true>(bl, wtiles_t, P, Cout, Cin, out, ldo, yprev, ldyp, pscale, pshift, prelu, s1, s2y,
-                                                      st, lv);
+        if (lv) return launch_dgrad<LD, true>(bl, wtiles_t, P, Cout, Cin, out, ldo, yprev, ldyp, pscale, pshift, prelu, s1, s2y, st, lv);
     }
     TcDgradEpi<LD, LIFT> ep{};
     if (lv) ep.lv = *lv;
     ep.out = out; ep.ldo = ldo; ep.yprev = yprev; ep.ldyp = ldyp; ep.scale = pscale; ep.shift = pshift; ep.relu = prelu;
     ep.s1g = s1; ep.s2y = s2y;
-    // GEMM: D[cin, pos] = sum_cout Wt[cin, cout] * dY[pos, cout]  ->  "K" = Cout, "Nw" = Cin
-    return launch_tc<MTMASK>(bl, (const uint8_t*)wtiles_t, P, Cout, Cin, ep, st, "o3d_pw_dgrad_tc");
+    // GEMM: D[pos, cin] = sum_cout dY[pos, cout] * Wt[cin, cout]  ->  "K" = Cout, "Nw" = Cin
+    return launch_tc(bl, (const uint8_t*)wtiles_t, P, Cout, Cin, ep, st, "o3d_pw_dgrad_tc");
 }
 
 }  // namespace
 
-extern "C" void o3d_debug_set(int tc_debug, int force_mt) {
+extern "C" void o3d_debug_set(int tc_debug) {
     g_tc_debug = tc_debug;
-    g_tc_force_mt = force_mt;
     o3d_g_no_skinny = (tc_debug & 128) != 0;
     o3d_g_fps_wide = (tc_debug & 1024) != 0;
     o3d_g_sa_fused_dbg = (tc_debug >> 11) & 15;
@@ -1216,12 +869,11 @@ extern "C" int o3d_pw_fwd_tc(const float* x, int ldx, const float* in_scale, con
     TcAct bl{x, ldx, in_scale, in_shift, in_relu};
     // the usual activation widths get a compile-time row stride (immediate store offsets in the epilogue)
     cudaStream_t st = (cudaStream_t)stream;
-    const bool two = tc_two_tiles(Nw, P);
 #define O3D_FWD_ARGS bl, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, st
-    if (ldy == 64 && !two) return launch_fwd<64, 1>(O3D_FWD_ARGS);
-    if (ldy == 128 && !two) return launch_fwd<128, 1>(O3D_FWD_ARGS);
-    if (ldy == 256 && two) return launch_fwd<256, 2>(O3D_FWD_ARGS);
-    return launch_fwd<0, 3>(O3D_FWD_ARGS);
+    if (ldy == 64) return launch_fwd<64>(O3D_FWD_ARGS);
+    if (ldy == 128) return launch_fwd<128>(O3D_FWD_ARGS);
+    if (ldy == 256) return launch_fwd<256>(O3D_FWD_ARGS);
+    return launch_fwd<0>(O3D_FWD_ARGS);
 #undef O3D_FWD_ARGS
 }
 
@@ -1235,13 +887,12 @@ int dgrad_tc_impl(const float* g, int ldg, const float* y, int ldy, const float*
     if (P == 0) return O3D_OK;
     TcDy bl{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1), g_tc_debug};
     cudaStream_t st = (cudaStream_t)stream;
-    const bool two = tc_two_tiles(Cin, P);
     const int ld = (!yprev || ldyp == ldo) ? ldo : 0;   // one compile-time stride serves both out and yprev
 #define O3D_DG_ARGS bl, wtiles_t, P, Cout, Cin, out, ldo, yprev, ldyp, pscale, pshift, prelu, s1, s2y, st, lv
-    if (ld == 64 && !two) return launch_dgrad<64, 1>(O3D_DG_ARGS);
-    if (ld == 128 && !two) return launch_dgrad<128, 1>(O3D_DG_ARGS);
-    if (ld == 256 && two) return launch_dgrad<256, 2>(O3D_DG_ARGS);
-    return launch_dgrad<0, 3>(O3D_DG_ARGS);
+    if (ld == 64) return launch_dgrad<64>(O3D_DG_ARGS);
+    if (ld == 128) return launch_dgrad<128>(O3D_DG_ARGS);
+    if (ld == 256) return launch_dgrad<256>(O3D_DG_ARGS);
+    return launch_dgrad<0>(O3D_DG_ARGS);
 #undef O3D_DG_ARGS
 }
 }  // namespace
@@ -1268,18 +919,37 @@ extern "C" int o3d_pw_dgrad_tc_lift(const float* g, int ldg, const float* y, int
 }
 
 namespace {
+// part == nullptr: every split adds its tile into dw with fp32 REDs; otherwise the splits write partial tiles into `part`
+// (part_floats long) and wgrad_reduce_kernel sums them in split order (deterministic)
 template <class XB>
-int launch_wgrad1(const TcDy& da, const XB& xb, int P, int Cout, int Cin, float* dw, int lddw, cudaStream_t st) {
+int launch_wgrad(const TcDy& da, const XB& xb, int P, int Cout, int Cin, float* dw, int lddw, float* part, long long part_floats,
+                 cudaStream_t st) {
     auto kern = pw_wgrad_tc_kernel<XB>;
-    O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM), "o3d_pw_wgrad_tc");
+    const char* name = part ? "o3d_pw_wgrad_tc2" : "o3d_pw_wgrad_tc";
+    O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM), name);
     const int mt = (Cout + TC_M - 1) / TC_M, nt = (Cin + TC_N - 1) / TC_N;
+    const int Mt = mt * TC_M, Nt = nt * TC_N;
     int splits = o3d_num_sms() / (mt * nt);
     if (splits < 1) splits = 1;
+    if (part) {
+        const long long cap = part_floats / ((long long)Mt * Nt);
+        if (splits > cap) splits = (int)cap;
+        // small problems (the heads: a few thousand positions): every split writes and the reduction re-reads a whole
+        // Mt x Nt partial tile, so at least 128 positions per split
+        const int by_size = (P + 127) / 128;
+        if (splits > by_size) splits = by_size;
+        O3D_REQUIRE(splits >= 1, O3D_ERR_ARG, "o3d_pw_wgrad_tc2: workspace too small");
+    }
     int chunk = (P + splits - 1) / splits;
     chunk = ((chunk + TC_K - 1) / TC_K) * TC_K;
     splits = (P + chunk - 1) / chunk;
-    kern<<<dim3(splits, nt, mt), WG_THREADS, WG_SMEM, st>>>(da, xb, P, Cout, Cin, chunk, dw, lddw, g_tc_debug);
-    O3D_CHECK_LAUNCH("o3d_pw_wgrad_tc");
+    kern<<<dim3(splits, nt, mt), WG_THREADS, WG_SMEM, st>>>(da, xb, P, Cout, Cin, chunk, dw, lddw, part, g_tc_debug);
+    O3D_CHECK_LAUNCH(name);
+    if (part) {
+        dim3 rg((Cin / 4 + 31) / 32, Cout);
+        wgrad_reduce_kernel<<<rg, 256, 0, st>>>(part, splits, Mt, Nt, Cout, Cin, dw, lddw);
+        O3D_CHECK_LAUNCH("o3d_pw_wgrad_tc2: reduce");
+    }
     return O3D_OK;
 }
 inline TcLift make_tclift(const o3d_lift_t* lf, const int32_t* gidx, const float* scale, const float* shift, int relu) {
@@ -1297,52 +967,11 @@ extern "C" int o3d_pw_wgrad_tc(const float* g, int ldg, const float* y, int ldy,
     if (P == 0) return O3D_OK;
     TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1), g_tc_debug};
     TcAct xb{x, ldx, in_scale, in_shift, in_relu};
-    return launch_wgrad1(da, xb, P, Cout, Cin, dw, lddw, (cudaStream_t)stream);
+    return launch_wgrad(da, xb, P, Cout, Cin, dw, lddw, nullptr, 0, (cudaStream_t)stream);
 }
-
-namespace {
-template <int MH, int NH, class XB>
-int launch_wgrad2(const TcDy& da, const XB& xb, int P, int Cout, int Cin, float* dw, int lddw, float* part,
-                  long long part_floats, cudaStream_t st) {
-    using C = Wg2Cfg<MH, NH>;
-    auto kern = pw_wgrad_tc2_kernel<MH, NH, XB>;
-    O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM), "o3d_pw_wgrad_tc2");
-    const int mt = (Cout + 128 * MH - 1) / (128 * MH), nt = (Cin + 128 * NH - 1) / (128 * NH);
-    const int Mt = mt * 128 * MH, Nt = nt * 128 * NH;
-    int splits = o3d_num_sms() / (mt * nt);
-    if (splits < 1) splits = 1;
-    const long long cap = part_floats / ((long long)Mt * Nt);
-    if (splits > cap) splits = (int)cap;
-    // small problems (the heads: a few thousand positions): every split writes and the reduction re-reads a whole Mt x Nt partial
-    // tile (256 KB for 256 x 256), so 148 splits of ~40 positions each move 77 MB for a 6,144-position layer — more than the
-    // layer itself.  At least 128 positions per split (512 was measured and is worse: the split's pipeline is a serial chain of
-    // k-blocks, 0.75 us each, and a dozen CTAs cannot hide it).
-    const int by_size = (P + 127) / 128;
-    if (splits > by_size) splits = by_size;
-    O3D_REQUIRE(splits >= 1, O3D_ERR_ARG, "o3d_pw_wgrad_tc2: workspace too small");
-    int chunk = (P + splits - 1) / splits;
-    chunk = ((chunk + C::K - 1) / C::K) * C::K;
-    splits = (P + chunk - 1) / chunk;
-    kern<<<dim3(splits, nt, mt), WG2_THREADS, C::SMEM, st>>>(da, xb, P, Cout, Cin, chunk, part, g_tc_debug);
-    O3D_CHECK_LAUNCH("o3d_pw_wgrad_tc2");
-    dim3 rg((Cin / 4 + 31) / 32, Cout);
-    wgrad_reduce_kernel<<<rg, 256, 0, st>>>(part, splits, Mt, Nt, Cout, Cin, dw, lddw);
-    O3D_CHECK_LAUNCH("o3d_pw_wgrad_tc2: reduce");
-    return O3D_OK;
-}
-template <class XB>
-int dispatch_wgrad2(const TcDy& da, const XB& xb, int P, int Cout, int Cin, float* dw, int lddw, float* part,
-                    long long part_floats, cudaStream_t st) {
-    const bool m2 = Cout > 128, n2 = Cin > 128;
-    if (m2 && n2) return launch_wgrad2<2, 2>(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, st);
-    if (m2) return launch_wgrad2<2, 1>(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, st);
-    if (n2) return launch_wgrad2<1, 2>(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, st);
-    return launch_wgrad2<1, 1>(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, st);
-}
-}  // namespace
 
 extern "C" long long o3d_pw_wgrad_tc2_workspace_floats(void) {
-    return (long long)o3d_num_sms() * 256 * 256;   // splits * Mt * Nt never exceeds (#SMs / tiles) * tiles * 256 * 256
+    return (long long)o3d_num_sms() * TC_M * TC_N;   // splits <= #SMs / tiles of dW, so splits * Mt * Nt <= #SMs * 128 * 128
 }
 
 extern "C" int o3d_pw_wgrad_tc2(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b,
@@ -1355,7 +984,7 @@ extern "C" int o3d_pw_wgrad_tc2(const float* g, int ldg, const float* y, int ldy
     if (P == 0) return O3D_OK;
     TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1), g_tc_debug};
     TcAct xb{x, ldx, in_scale, in_shift, in_relu};
-    return dispatch_wgrad2(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
+    return launch_wgrad(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
 }
 
 // ---- lifted first layer (o3d_lift_t): the next layer's GEMMs read Y0 through TcLift / the lifted dgrad epilogue ----------
@@ -1370,9 +999,8 @@ extern "C" int o3d_pw_wgrad_tc_lift(const float* g, int ldg, const float* y, int
     if (P == 0) return O3D_OK;
     TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1), g_tc_debug};
     TcLift xb = make_tclift(lf, gidx, in_scale, in_shift, in_relu);
-    xb.la = part ? ((Cout > 128 || Cin > 128) ? 16 : 32) : TC_K;      // a producer thread's next fetch lies one k-block of positions further
-    if (part) return dispatch_wgrad2(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
-    return launch_wgrad1(da, xb, P, Cout, Cin, dw, lddw, (cudaStream_t)stream);
+    xb.la = TC_K;      // a producer thread's next fetch lies one k-block of positions further
+    return launch_wgrad(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
 }
 
 extern "C" int o3d_pw_fwd_tc_lift(const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift,
@@ -1387,11 +1015,10 @@ extern "C" int o3d_pw_fwd_tc_lift(const o3d_lift_t* lf, const int32_t* gidx, con
     const int Nw = (N + 3) & ~3;
     const TcLift bl = make_tclift(lf, gidx, in_scale, in_shift, in_relu);
     cudaStream_t st = (cudaStream_t)stream;
-    const bool two = tc_two_tiles(Nw, P);
 #define O3D_FWD_ARGS bl, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, st
-    if (ldy == 64 && !two) return launch_fwd<64, 1>(O3D_FWD_ARGS);
-    if (ldy == 128 && !two) return launch_fwd<128, 1>(O3D_FWD_ARGS);
-    if (ldy == 256 && two) return launch_fwd<256, 2>(O3D_FWD_ARGS);
-    return launch_fwd<0, 3>(O3D_FWD_ARGS);
+    if (ldy == 64) return launch_fwd<64>(O3D_FWD_ARGS);
+    if (ldy == 128) return launch_fwd<128>(O3D_FWD_ARGS);
+    if (ldy == 256) return launch_fwd<256>(O3D_FWD_ARGS);
+    return launch_fwd<0>(O3D_FWD_ARGS);
 #undef O3D_FWD_ARGS
 }

@@ -11,19 +11,18 @@
 //      as ball_query.cu) and keeps idx[64] and (dx, dy, dz)[64] in shared memory;
 //   B. the 64 neighbour feature rows are gathered (coalesced 128-byte segments), split into TF32 hi / lo parts and stored as
 //      the K-major SWIZZLE_128B activation operand (k-blocks of 32 channels: hi [64 x 128 B] | lo [64 x 128 B]);
-//   C. per layer, the MMA warp issues 3xTF32 tcgen05.mma (M = 128 output channels, N = 64 positions, K = 8) over all
-//      k-blocks, weights arriving as pre-tiled hi | lo images (o3d_sa_fused_prepare) through a bulk-copy ring that runs
-//      ahead across layers; accumulators live in TMEM (64 columns per 128-channel tile).  The eight epilogue warps read them
-//      back (tcgen05.ld), add the coordinate term of the first layer W0[:, 0:3] . (dx, dy, dz) with plain FMAs (exact fp32 —
-//      the same split as the training path's lifted first layer), apply the folded BatchNorm + ReLU and write the result, hi /
-//      lo split, over the activation operand IN PLACE: the layer's output never leaves the SM;
-//   D. the last layer's epilogue max-pools over each centre's nsample positions in registers and stores one channels-last
-//      row per centre.
+//   C. per layer, the two warpgroups issue 3xTF32 wgmma (M = the 64 positions, K = 8; warpgroup h takes output channels
+//      h*64 .. h*64+63 of a one-tile layer, or the whole 128-channel tile h of a two-tile layer) over all k-blocks, weights
+//      arriving as pre-tiled hi | lo images (o3d_sa_fused_prepare) through a bulk-copy ring that runs ahead across layers;
+//      accumulators live in registers.  The epilogue adds the coordinate term of the first layer W0[:, 0:3] . (dx, dy, dz)
+//      with plain FMAs (exact fp32 — the same split as the training path's lifted first layer), applies the folded
+//      BatchNorm + ReLU and writes the result, hi / lo split, over the activation operand IN PLACE once every MMA of the
+//      layer has retired: the layer's output never leaves the SM;
+//   D. the last layer's result is staged [position][channel] over the (then dead) operand and weight ring, and one thread
+//      per channel max-pools each centre's nsample positions and stores one channels-last row per centre.
 // HBM / L2 traffic per CTA: the cloud's coordinates, 64 feature rows, the weight images, 64 / nsample output rows.
 //
-//   warps 0-7: query / gather / epilogue (warp % 4 = the TMEM lane quarter it may read) | 8: MMA issuer, TMEM alloc |
-//   9: weight streamer
-#include <type_traits>
+//   warps 0-7: query / gather / MMA / epilogue (two warpgroups) | 8: weight streamer
 #include "common.cuh"
 #include "ball_query.cuh"
 #include "tc_ptx.cuh"
@@ -34,22 +33,11 @@ int o3d_g_sa_fused_dbg = 0;   // experiments (o3d_debug_set bits 11-14): 1 = eve
 namespace {
 
 constexpr int SF_POS = 64;                  // positions per CTA
-constexpr int SF_THREADS = 320;
+constexpr int SF_THREADS = 288;
 constexpr int SF_ACT_KB = 2 * SF_POS * 128; // bytes per activation k-block: hi | lo
 constexpr int SF_WTILE = 2 * TILE_BYTES;    // one weight tile (128 channels x 32 k): hi | lo
 constexpr int SF_MAX_SLOTS = 6;
-constexpr int SF_MISC = 128 + SF_POS * 4 + SF_POS * 16;   // barriers + TMEM slot | idx | rel
-constexpr uint32_t SF_TMEM_COLS = 128;      // two 128-channel tiles x 64 positions
-
-__device__ __forceinline__ void sts_f32(uint32_t a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); }
-__device__ __forceinline__ void sts_v4(uint32_t a, const float4& v) {
-    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-__device__ __forceinline__ float4 lds_v4(uint32_t a) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
-    return v;
-}
+constexpr int SF_MISC = 128 + SF_POS * 4 + SF_POS * 16;   // barriers | idx | rel
 
 struct SfLayer {
     int cout, n_mt, nkb, relu, mma;
@@ -65,7 +53,108 @@ struct SfParams {
     SfLayer l[O3D_MAX_LAYERS];
 };
 
-__global__ void __launch_bounds__(SF_THREADS, 2)
+__device__ __forceinline__ float2 ld2g(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
+__device__ __forceinline__ void sts_v4(uint32_t a, const float4& v) {
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+
+// One layer on the two warpgroups.  NT = output channels per warpgroup: 64 (a one-tile layer, split) or 128 (tile h).
+// Every warpgroup walks every weight tile of the layer (waits for it, releases it) so that the ring's phases stay in step.
+template <int NT>
+__device__ __forceinline__ void sf_layer(const SfParams& prm, int l, uint8_t* act, uint8_t* ring, uint64_t* full, uint64_t* empty,
+                                         int& slot, int& phase, const uint8_t* __restrict__ block, const float4* s_rel, int g0,
+                                         float* __restrict__ out, int ldo) {
+    const SfLayer& L = prm.l[l];
+    const int h = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    float acc[NT / 2];
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+    if (L.mma) {
+        for (int mt = 0; mt < L.n_mt; ++mt) {
+            for (int kb = 0; kb < L.nkb; ++kb) {
+                o3d_mbar_wait(full + slot, phase);
+                if ((NT == 64 || mt == h) && !(prm.dbg & 4)) {
+                    const uint32_t wb = o3d_smem_u32(ring + slot * SF_WTILE) + (NT == 64 ? h * (TILE_BYTES / 2) : 0);
+                    const uint32_t ab = o3d_smem_u32(act + kb * SF_ACT_KB);
+                    wgmma_fence_acc(acc);
+                    wgmma_fence();
+                    wgmma_3xtf32_kblock<NT>(acc, make_desc(ab), make_desc(ab + SF_ACT_KB / 2), make_desc(wb), make_desc(wb + TILE_BYTES),
+                                            kb == 0);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_acc(acc);
+                }
+                __syncwarp();
+                if (lane == 0) o3d_mbar_arrive(empty + slot);
+                if (++slot == prm.nslot) { slot = 0; phase ^= 1; }
+            }
+        }
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");   // every MMA reading the operand has retired: it may be overwritten
+    const bool first = l == 0, last = l == prm.n - 1;
+    const int next_nkb = last ? 0 : prm.l[l + 1].nkb;
+    const int ldv = L.n_mt * 128;                     // scale | shift (and W0's coordinate columns) per channel
+    const int lds = ldv + 8;                          // last layer: staged [position][channel] row stride
+    const float* vecs = reinterpret_cast<const float*>(block);
+    float* stg = reinterpret_cast<float*>(act);
+    const float floor_v = L.relu ? 0.f : -INFINITY;
+    float4 rel[2] = {};
+    if (first) {
+        rel[0] = s_rel[16 * w + (lane >> 2)];
+        rel[1] = s_rel[16 * w + (lane >> 2) + 8];
+    }
+    if (!(prm.dbg & 8)) {
+#pragma unroll
+        for (int j = 0; j < NT / 8; ++j) {
+            const int ch = h * NT + 8 * j + 2 * (lane & 3);   // this thread's channels ch, ch + 1
+            if (!last && (ch >> 5) >= next_nkb) continue;     // padding no later layer reads (uniform over the warp)
+            const float2 sc = ld2g(vecs + L.vec_off + ch), sh = ld2g(vecs + L.vec_off + ldv + ch);
+            float2 wx0 = make_float2(0.f, 0.f), wx1 = wx0, wx2 = wx0;
+            if (first) {
+                wx0 = ld2g(vecs + prm.wx_off + ch);
+                wx1 = ld2g(vecs + prm.wx_off + ldv + ch);
+                wx2 = ld2g(vecs + prm.wx_off + 2 * ldv + ch);
+            }
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int pos = 16 * w + (lane >> 2) + 8 * r;
+                float a0 = acc[4 * j + 2 * r], a1 = acc[4 * j + 2 * r + 1];
+                if (first) {
+                    a0 = fmaf(wx2.x, rel[r].z, fmaf(wx1.x, rel[r].y, fmaf(wx0.x, rel[r].x, a0)));
+                    a1 = fmaf(wx2.y, rel[r].z, fmaf(wx1.y, rel[r].y, fmaf(wx0.y, rel[r].x, a1)));
+                }
+                const float v0 = fmaxf(fmaf(a0, sc.x, sh.x), floor_v), v1 = fmaxf(fmaf(a1, sc.y, sh.y), floor_v);
+                if (!last) {
+                    uint8_t* dst = act + (ch >> 5) * SF_ACT_KB + sw128(pos, (ch & 31) >> 2) + (ch & 3) * 4;
+                    const float h0 = hi1(v0), h1 = hi1(v1);
+                    *reinterpret_cast<float2*>(dst) = make_float2(h0, h1);
+                    *reinterpret_cast<float2*>(dst + SF_ACT_KB / 2) = make_float2(v0 - h0, v1 - h1);
+                } else {
+                    *reinterpret_cast<float2*>(stg + pos * lds + ch) = make_float2(v0, v1);
+                }
+            }
+        }
+    }
+    if (!last) {
+        o3d_fence_proxy_async();                      // generic-proxy stores -> visible to the next layer's wgmma
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        return;
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    // ---- D. max-pool over each centre's nsample positions: thread = channel
+    const int ch = threadIdx.x;
+    const int S = prm.S;
+    if (prm.dbg & 8 || ch >= ((L.cout + 31) & ~31) || ch >= ldo) return;
+    const bool real = ch < L.cout;
+    for (int g = 0; g < SF_POS / S; ++g) {
+        float mx = -INFINITY;
+        for (int p = g * S; p < (g + 1) * S; ++p) mx = fmaxf(mx, stg[p * lds + ch]);
+        const int gg = g0 + g;
+        if (gg < prm.BM) out[(size_t)gg * ldo + ch] = real ? mx : 0.f;
+    }
+}
+
+__global__ void __launch_bounds__(SF_THREADS, 1)
     sa_fused_kernel(const SfParams prm, const uint8_t* __restrict__ block, const float* __restrict__ xyz,
                     const float* __restrict__ new_xyz, const float* __restrict__ feat, float* __restrict__ out, int ldo,
                     int32_t* __restrict__ idx_out) {
@@ -75,10 +164,7 @@ __global__ void __launch_bounds__(SF_THREADS, 2)
     uint8_t* ring = smem + prm.act_bytes;
     uint8_t* misc = ring + prm.nslot * SF_WTILE;
     uint64_t* full = reinterpret_cast<uint64_t*>(misc);       // [SF_MAX_SLOTS] weight tile landed
-    uint64_t* empty = full + SF_MAX_SLOTS;                    // [SF_MAX_SLOTS] MMAs reading the slot retired
-    uint64_t* act_ready = empty + SF_MAX_SLOTS;               // activation operand of the next layer written (256 arrivals)
-    uint64_t* layer_done = act_ready + 1;                     // every MMA of the layer retired
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(layer_done + 1);
+    uint64_t* empty = full + SF_MAX_SLOTS;                    // [SF_MAX_SLOTS] both warpgroups are done with the slot
     int32_t* s_idx = reinterpret_cast<int32_t*>(misc + 128);
     float4* s_rel = reinterpret_cast<float4*>(misc + 128 + SF_POS * 4);
 
@@ -89,56 +175,14 @@ __global__ void __launch_bounds__(SF_THREADS, 2)
     if (threadIdx.x == 0) {
         for (int s = 0; s < SF_MAX_SLOTS; ++s) {
             o3d_mbar_init(full + s, 1);
-            o3d_mbar_init(empty + s, 1);
+            o3d_mbar_init(empty + s, 8);
         }
-        o3d_mbar_init(act_ready, 256);
-        o3d_mbar_init(layer_done, 1);
         o3d_fence_mbar_init();
     }
-    if (warp == 8) tmem_alloc(tmem_slot, SF_TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 8) {
-        // ===================================================== MMA issuer
-        const uint32_t idesc = make_idesc(TC_M, SF_POS);
-        int slot = 0, phase = 0, ar = 0;
-        for (int l = 0; l < prm.n; ++l) {
-            const SfLayer& L = prm.l[l];
-            if (!L.mma) continue;
-            o3d_mbar_wait(act_ready, ar);
-            ar ^= 1;
-            tc_fence_after();
-            for (int mt = 0; mt < L.n_mt; ++mt) {
-                for (int kb = 0; kb < L.nkb; ++kb) {
-                    o3d_mbar_wait(full + slot, phase);
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint32_t wb = o3d_smem_u32(ring + slot * SF_WTILE);
-                        const uint32_t ab = o3d_smem_u32(act + kb * SF_ACT_KB);
-                        const uint64_t whi = make_desc(wb), wlo = make_desc(wb + TILE_BYTES);
-                        const uint64_t xhi = make_desc(ab), xlo = make_desc(ab + SF_ACT_KB / 2);
-                        const uint32_t d_tmem = tmem_base + (uint32_t)(mt * SF_POS);
-#pragma unroll
-                        for (int ks = 0; ks < TC_K / 8; ++ks) {
-                            if (prm.dbg & 4) break;
-                            const uint64_t adv = (uint64_t)((ks * 32) >> 4);   // +32 bytes along K inside the 128-byte swizzle row
-                            umma_tf32(d_tmem, wlo + adv, xhi + adv, idesc, (kb | ks) != 0);
-                            umma_tf32(d_tmem, whi + adv, xlo + adv, idesc, 1u);
-                            umma_tf32(d_tmem, whi + adv, xhi + adv, idesc, 1u);
-                        }
-                        umma_commit(empty + slot);
-                        if (mt == L.n_mt - 1 && kb == L.nkb - 1) umma_commit(layer_done);
-                    }
-                    __syncwarp();
-                    if (++slot == nslot) { slot = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 9) {
-        // ===================================================== weight streamer: runs ahead of the MMA warp, across layers
+        // ===================================================== weight streamer: runs ahead of the MMAs, across layers
         if (lane == 0) {
             const uint8_t* src = block + prm.tiles_off;
             int slot = 0, phase = 0;
@@ -164,7 +208,7 @@ __global__ void __launch_bounds__(SF_THREADS, 2)
             }
         }
     } else {
-        // ===================================================== query / gather / epilogue (256 threads)
+        // ===================================================== query / gather / MMA / epilogue (256 threads)
         const int tid = threadIdx.x;
         const int S = prm.S, N = prm.N, M = prm.M;
         const int cpc = SF_POS / S;                     // centres of this CTA
@@ -231,108 +275,15 @@ __global__ void __launch_bounds__(SF_THREADS, 2)
                     sts_v4(lo + o1, lo_part(v1[j]));
                 }
             }
-            o3d_fence_proxy_async();
-            o3d_mbar_arrive(act_ready);
         }
-        // ---- C / D. per layer: accumulators -> (+ coordinate term) -> BatchNorm + ReLU -> next operand | max-pool
-        // (the inner loop is issue-bound — 8 K..16 K outputs per layer on 8 warps — so everything that does not depend on the
-        //  column is hoisted: shared-space addresses with compile-time offsets, the XOR swizzle as 8 per-thread constants,
-        //  shift / mask instead of division by nsample, one instantiation per (first, last, has-MMA) combination)
-        const int q = warp & 3, half = warp >> 2;
-        const float* vecs = reinterpret_cast<const float*>(block);
-        const uint32_t act_s = o3d_smem_u32(act), rel_s = o3d_smem_u32(s_rel);
-        const int logS = 31 - __clz(S);                 // nsample divides 64: a power of two
-        uint32_t xo[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) xo[i] = (uint32_t)(((lane >> 2) ^ i) << 4) + (uint32_t)(i * 128);
-        int ld_phase = 0;
+        o3d_fence_proxy_async();
+        asm volatile("bar.sync 1, 256;" ::: "memory");   // the first layer's operand is complete
+        // ---- C / D. per layer: MMAs -> (+ coordinate term) -> BatchNorm + ReLU -> next operand | max-pool
+        int slot = 0, phase = 0;
         for (int l = 0; l < prm.n; ++l) {
-            const SfLayer& L = prm.l[l];
-            const bool last = l == prm.n - 1;
-            const bool wide = L.n_mt == 2;
-            const bool all_cols = wide || S > 32;       // one warp walks all 64 columns (a pooling group never spans two warps)
-            const int m = wide ? half : 0;
-            const int kb_out = m * 4 + q;               // the k-block of the next operand this warp's 32 channels form
-            // channels past the layer's width are padding: nothing reads them
-            const bool work = (wide || S <= 32 || half == 0) && (last ? kb_out * 32 < L.cout : kb_out < prm.l[l + 1].nkb) && !(prm.dbg & 8);
-            const int col0 = all_cols ? 0 : half * 32, ncol = all_cols ? 64 : 32;
-            const int chl = kb_out * 32 + lane;         // this thread's output channel
-            float sc = 0.f, sh = 0.f, wx0 = 0.f, wx1 = 0.f, wx2 = 0.f;
-            if (work) {
-                sc = __ldg(vecs + L.vec_off + chl);
-                sh = __ldg(vecs + L.vec_off + L.n_mt * 128 + chl);
-                if (l == 0) {
-                    const float* wx = vecs + prm.wx_off;
-                    const int ldw = L.n_mt * 128;
-                    wx0 = __ldg(wx + chl);
-                    wx1 = __ldg(wx + ldw + chl);
-                    wx2 = __ldg(wx + 2 * ldw + chl);
-                }
-            }
-            const float floor_v = L.relu ? 0.f : -INFINITY;
-            if (L.mma) {
-                o3d_mbar_wait(layer_done, ld_phase);
-                ld_phase ^= 1;
-                tc_fence_after();
-            }
-            if (work) {
-                const uint32_t dst_s = act_s + (uint32_t)(kb_out * SF_ACT_KB + (lane & 3) * 4);
-                const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(m * SF_POS);
-                const bool out_on = chl < ldo;
-                const bool real = chl < L.cout;
-                auto run = [&](auto first_, auto last_, auto mma_) {
-                    constexpr bool FIRST = decltype(first_)::value, LAST = decltype(last_)::value, MMA = decltype(mma_)::value;
-                    float mx = -INFINITY;
-                    for (int cc = col0; cc < col0 + ncol; cc += 16) {
-                        uint32_t r[16];
-                        if constexpr (MMA) tmem_ld16(t_addr + (uint32_t)cc, r);
-                        const uint32_t rowbase = dst_s + (uint32_t)((cc >> 3) * 1024);
-                        const uint32_t relbase = rel_s + (uint32_t)(cc * 16);
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            float a = MMA ? __uint_as_float(r[j]) : 0.f;
-                            if constexpr (FIRST) {
-                                const float4 rel = lds_v4(relbase + j * 16);
-                                a = fmaf(wx2, rel.z, fmaf(wx1, rel.y, fmaf(wx0, rel.x, a)));
-                            }
-                            const float v = fmaxf(fmaf(a, sc, sh), floor_v);
-                            if constexpr (!LAST) {
-                                const uint32_t off = rowbase + (uint32_t)((j >> 3) * 1024) + xo[j & 7];
-                                const float h = hi1(v);
-                                sts_f32(off, h);
-                                sts_f32(off + SF_ACT_KB / 2, v - h);
-                            } else {
-                                mx = fmaxf(mx, v);
-                                if (((cc + j + 1) & (S - 1)) == 0) {
-                                    const int g = g0 + ((cc + j) >> logS);
-                                    if (out_on && g < prm.BM) out[(size_t)g * ldo + chl] = real ? mx : 0.f;
-                                    mx = -INFINITY;
-                                }
-                            }
-                        }
-                    }
-                };
-                using T = std::true_type;
-                using F = std::false_type;
-                if (l == 0) {
-                    if (L.mma) { if (last) run(T{}, T{}, T{}); else run(T{}, F{}, T{}); }
-                    else { if (last) run(T{}, T{}, F{}); else run(T{}, F{}, F{}); }
-                } else {
-                    if (last) run(F{}, T{}, T{}); else run(F{}, F{}, T{});
-                }
-            }
-            if (!last) {
-                o3d_fence_proxy_async();
-                tc_fence_before();
-                o3d_mbar_arrive(act_ready);
-            }
+            if (prm.l[l].n_mt == 2) sf_layer<128>(prm, l, act, ring, full, empty, slot, phase, block, s_rel, g0, out, ldo);
+            else sf_layer<64>(prm, l, act, ring, full, empty, slot, phase, block, s_rel, g0, out, ldo);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 8) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, SF_TMEM_COLS);
     }
 }
 
@@ -493,14 +444,10 @@ extern "C" int o3d_sa_fused_forward(const o3d_stack_t* d, const void* block, con
     if (nslot > SF_MAX_SLOTS) nslot = SF_MAX_SLOTS;
     int tiles = 0;
     for (int l = 0; l < prm.n; ++l) tiles += prm.l[l].mma ? prm.l[l].n_mt * prm.l[l].nkb : 0;
-    if (nslot > tiles && tiles >= 2) nslot = tiles;       // a short stack needs no deeper ring: leaves room for a second CTA per SM
+    if (nslot > tiles && tiles >= 2) nslot = tiles;       // a short stack needs no deeper ring
     O3D_REQUIRE(nslot >= 2, O3D_ERR_ARG, "o3d_sa_fused_forward: N=%d points per cloud do not fit the shared-memory staging", N);
     const int cpc = SF_POS / nsample;
     const int grid = (B * M) / cpc;
-    if (grid > o3d_num_sms()) {       // more CTAs than SMs: a shallower ring lets two CTAs share an SM (228 KB, 1 KB reserved per CTA)
-        const int fit = (113 * 1024 - 1024 - SF_MISC - act) / SF_WTILE;
-        if (fit >= 2 && fit < nslot) nslot = fit;
-    }
     prm.nslot = nslot;
     prm.dbg = o3d_g_sa_fused_dbg;
     const int smem = 1024 + act + nslot * SF_WTILE + SF_MISC;

@@ -3,7 +3,7 @@
 // Python dispatch cost dominated the first fused version (hundreds of tiny torch ops per step just to pad / transpose
 // weights and slice workspaces), so the per-layer sequencing lives here: the caller hands over one descriptor with the
 // raw parameter pointers of the reference modules (weights in their checkpoint layout), one workspace buffer, and gets
-// every kernel of the stack enqueued on the stream: weight packing, per-layer GEMM (+tcgen05 variant), batch-norm
+// every kernel of the stack enqueued on the stream: weight packing, per-layer GEMM (+wgmma variant), batch-norm
 // finalisation, pooling / activation, and on the way back the BN-backward finalisation, wgrad, dgrad and the
 // un-packing of the weight gradients into the checkpoint layout.  Nothing is allocated and nothing synchronises, so a
 // stack can be captured into a CUDA graph.

@@ -1,79 +1,68 @@
-// tcgen05 / TMEM PTX wrappers, UMMA shared-memory / instruction descriptors and the TF32 hi/lo split shared by the tensor-core
-// kernels (pwmlp_tc.cu: forward / dgrad / wgrad GEMMs of the training path; sa_fused.cu: the single-kernel inference SA layer).
+// Hopper warpgroup MMA (wgmma) PTX wrappers, the shared-memory matrix descriptor and the TF32 hi/lo split shared by the
+// tensor-core kernels (pwmlp_tc.cu: forward / dgrad / wgrad GEMMs of the training path; sa_fused.cu: the single-kernel
+// inference SA layer).
+//
+// Every GEMM here is  D[64 rows, N] (+)= A[64 rows, k] . B[N rows, k]^T  per warpgroup, both operands K-major in shared
+// memory with the 128-byte swizzle (tf32 operands must be K-major for wgmma).  D lives in registers, fp32: with w = warp
+// in the warpgroup and l = lane, register i holds row 16 w + l / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (l & 3) + (i & 1).
 #pragma once
 #include "common.cuh"
 
 namespace {
 
-constexpr int TC_M = 128;       // channels per tile
+constexpr int TC_M = 128;       // rows per operand tile
 constexpr int TC_N = 128;       // positions per tile
 constexpr int TC_K = 32;        // tf32 elements per k-block = 128 bytes per row
 constexpr int TILE_BYTES = TC_M * TC_K * 4;            // 16 KB
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator registers across the asynchronous MMA's issue / wait
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(o3d_smem_u32(smem_dst)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, tf32 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D (+)= A[smem desc] * B[smem desc]^T, tf32 inputs, fp32 accumulate in registers (accumulate = 0: D is overwritten)
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(o3d_smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 | LBO=1 (ignored for
-// swizzled K-major) | SBO = 1024 B between 8-row groups | version 1 | layout 2 (SWIZZLE_128B).
+
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (wgmma): start >> 4 | LBO = 1 (unused for swizzled K-major) |
+// SBO = 1024 B between 8-row groups | layout type 1 (SWIZZLE_128B) at bits 62-63.  Tiles start on 1024-byte boundaries;
+// +32 bytes along K (one k-step of 8 tf32) inside the swizzle row is +2 on the start field.
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
-}
-// instruction descriptor: D=F32 (bits 4-5 = 1), A=B=TF32 (2 at bits 7-9 / 10-12), K-major both, N>>3 at 17, M>>4 at 24
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 // byte offset of the 16-byte chunk `c` (0..7) of row `r` inside a [rows x 32 tf32] SWIZZLE_128B K-major tile
@@ -90,5 +79,24 @@ __device__ __forceinline__ float4 lo_part(const float4& v) {
 }
 __device__ __forceinline__ float4 ld4g(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 
+// 3xTF32 product of one 32-wide k-block: D += Alo.Bhi + Ahi.Blo + Ahi.Bhi over 4 k-steps (descriptors of the k-block's
+// first column).  `first`: D starts from zero.
+template <int N>
+__device__ __forceinline__ void wgmma_3xtf32_kblock(float (&d)[N / 2], uint64_t ahi, uint64_t alo, uint64_t bhi, uint64_t blo,
+                                                    bool first) {
+#pragma unroll
+    for (int ks = 0; ks < TC_K / 8; ++ks) {
+        const uint64_t adv = (uint64_t)((ks * 32) >> 4);
+        if constexpr (N == 64) {
+            wgmma_tf32_n64(d, alo + adv, bhi + adv, (first && ks == 0) ? 0u : 1u);
+            wgmma_tf32_n64(d, ahi + adv, blo + adv, 1u);
+            wgmma_tf32_n64(d, ahi + adv, bhi + adv, 1u);
+        } else {
+            wgmma_tf32_n128(d, alo + adv, bhi + adv, (first && ks == 0) ? 0u : 1u);
+            wgmma_tf32_n128(d, ahi + adv, blo + adv, 1u);
+            wgmma_tf32_n128(d, ahi + adv, bhi + adv, 1u);
+        }
+    }
+}
 
 }  // namespace

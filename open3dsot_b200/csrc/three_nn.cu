@@ -1,4 +1,4 @@
-// three_nn / three_interpolate (+grad) and the fused three_nn+interpolate, for sm_100a.
+// three_nn / three_interpolate (+grad) and the fused three_nn+interpolate, for sm_90a.
 //
 // Replaces `_ext.three_nn` (pointnet2/utils/pointnet2_utils.py:125), `_ext.three_interpolate(_grad)`
 // (:162,:184) and — fused — the body of PointnetFPModule.forward (pointnet2/utils/pointnet2_modules.py:187-195).

@@ -1,4 +1,4 @@
-// Template-search cross-correlation front ends (models/head/xcorr.py), sm_100a.
+// Template-search cross-correlation front ends (models/head/xcorr.py), sm_90a.
 //
 //   o3d_xcorr_boxaware_fwd   BoxAwareXCorr (xcorr.py:81-88): for every search point the k template points whose 9-D box
 //                            clouds are nearest.  The reference computes `torch.cdist` (64 x 128 points -> its

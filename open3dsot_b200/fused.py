@@ -1,4 +1,4 @@
-"""Fused execution of the reference's MLP stacks on the sm_100a point-wise kernels (csrc/pwmlp.cu).
+"""Fused execution of the reference's MLP stacks on the sm_90a point-wise kernels (csrc/pwmlp.cu).
 
 A *stack* is what the reference builds with `pt_utils.SharedMLP` / `pt_utils.Seq` / a bare `nn.Conv1d`:
 a chain of 1x1 convolutions, each optionally followed by BatchNorm and ReLU, optionally ending in a max over
@@ -725,7 +725,7 @@ _SIDE_STREAMS = {}
 
 def fps_ahead(points, npoint):
     """Launch furthest-point sampling of `points` (B,N,3+) on a side stream and return (idx, join).  FPS is a serial chain
-    of npoint steps that occupies one CTA per cloud (48 of 148 SMs at config 2); started before the template branch it
+    of npoint steps that occupies one CTA per cloud (48 of 132 SMs at config 2); started before the template branch it
     runs underneath that branch's GEMMs.  `join()` makes the current stream wait for it (graph-capture safe fork/join)."""
     cur = torch.cuda.current_stream()
     dev = points.device.index

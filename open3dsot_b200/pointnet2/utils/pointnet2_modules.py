@@ -6,7 +6,7 @@ PointnetSAModuleMSG (:82-117), PointnetSAModule (:120-149), PointnetFPModule (:1
 (FlowEmbedding / PointNetSetUpConv, :215-334, are unused by every model and broken upstream; they are kept
 importable as thin compositions of the same primitives.)
 
-Two execution modes, both on the sm_100a kernels (there is no CPU path):
+Two execution modes, both on the sm_90a kernels (there is no CPU path):
   * fused   (default) — open3dsot_b200.fused: ball-query + gather feed the point-wise MLP kernels directly
               (channels-last activations, BN statistics and max-pool in the GEMM epilogues);
   * composed — the reference's op-by-op composition over the nine `_ext` kernels + torch conv/BN, kept as

@@ -2,7 +2,7 @@
 
 Mirror of pointnet2/utils/pointnet2_utils.py: FurthestPointSampling (:35-65), GatherOperation (:68-102),
 ThreeNN (:105-134), ThreeInterpolate (:137-191), GroupingOperation (:194-242), BallQuery (:245-277),
-QueryAndGroup (:280-339), GroupAll (:342-385), knn_point (:388-402).  Every op dispatches to the sm_100a
+QueryAndGroup (:280-339), GroupAll (:342-385), knn_point (:388-402).  Every op dispatches to the sm_90a
 kernels behind the C ABI (open3dsot_b200._ext == the `pointnet2_ops._ext` call surface); there is no
 PyTorch or CPU fallback — CPU tensors raise RuntimeError exactly like upstream ("CPU not supported").
 """

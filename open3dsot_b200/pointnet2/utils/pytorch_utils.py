@@ -6,7 +6,7 @@ What matters for drop-in use is the *state-dict surface* (SURVEY.md §8b):
     <mlp>.layer{i}.conv.weight, <mlp>.layer{i}.bn.bn.{weight,bias,running_mean,running_var,num_batches_tracked}
     <seq>.{i}.conv.{weight,bias}, <seq>.{i}.bn.bn.*
 and the construction rules: bias only when no BN, kaiming-normal conv weights, BN gamma=1 / beta=0.
-The classes are plain containers; the B200 modules read their parameters and run the fused sm_100a
+The classes are plain containers; the native modules read their parameters and run the fused sm_90a
 kernels (open3dsot_b200/fused.py) instead of iterating the container.
 """
 from typing import List

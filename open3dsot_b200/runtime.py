@@ -5,7 +5,7 @@ import os
 _FUSED = os.environ.get("O3D_FUSED", "1") != "0"
 
 
-# tcgen05 3xTF32 GEMM core for the point-wise layers: bit 0 = forward + dgrad, bit 1 = wgrad  (0 = exact-fp32 CUDA cores)
+# wgmma 3xTF32 GEMM core for the point-wise layers: bit 0 = forward + dgrad, bit 1 = wgrad  (0 = exact-fp32 CUDA cores)
 _TC = int(os.environ.get("O3D_TC", "3"))
 
 

@@ -237,25 +237,22 @@ def gen_m2track(out):
     out["m2_eval_boxes"] = np_(ep["estimation_boxes"])
 
 
-def gen_checkpoint_eval(out):
-    """SURVEY.md §8f rank 1: the reference's shipped `pretrained_models/bat_kitti_car.ckpt` through the reference's own BAT in
-    eval mode on a fixed synthetic pair -> outputs (committed) + the state dict as a plain npz under tests/golden/_ckpt/
-    (git-ignored: trained weights are not source; the GPU box receives the file with the working tree)."""
+def gen_bat_eval_full(out):
+    """The reference's own BAT (BAT_Car.yaml) in eval mode at full size (template 512 / search 1024, two pairs) on the
+    seeded weights of tests/_params.py:det_state_dict(seed=41), which the GPU test rebuilds without any outside file.
+    Kept small: pred_search_bc for its first 32 points only, sample_idxs as int16."""
     from models import get_model
-    from open3dsot_b200.checkpoint import load_lightning_checkpoint
-    ck = load_lightning_checkpoint(os.path.join(REF, "pretrained_models", "bat_kitti_car.ckpt"))
     cfg = EasyDict(load_yaml(os.path.join(ROOT, "cfgs", "BAT_Car.yaml")))
     net = get_model(cfg.net_model)(cfg)
-    missing = net.load_state_dict(ck["state_dict"], strict=False)
-    assert not [k for k in missing.missing_keys if not k.split(".")[0] in ("prec", "success")], missing
+    net.load_state_dict(det_state_dict(net.state_dict(), seed=41), strict=False)
     net.eval()
     batch = synthetic_siamese_batch(2, 512, 1024, seed=4242, box_aware=True)
     with torch.no_grad():
         ep = net({k: v.clone() for k, v in batch.items()})
-    for k in ("estimation_boxes", "estimation_cla", "vote_xyz", "center_xyz", "sample_idxs", "pred_search_bc"):
-        out[f"ckpt_bat_car_{k}"] = np_(ep[k])
-    os.makedirs(os.path.join(HERE, "_ckpt"), exist_ok=True)
-    np.savez(os.path.join(HERE, "_ckpt", "bat_kitti_car_state.npz"), **{k: np_(v) for k, v in ck["state_dict"].items()})
+    for k in ("estimation_boxes", "estimation_cla", "vote_xyz", "center_xyz"):
+        out[k] = np_(ep[k])
+    out["sample_idxs"] = np_(ep["sample_idxs"]).astype(np.int16)
+    out["pred_search_bc"] = np_(ep["pred_search_bc"][:, :32])
 
 
 def main():
@@ -269,9 +266,11 @@ def main():
     gen_model("bat", "BAT_Car.yaml", 2, 256, 512, models, seed=21)
     gen_model("p2b", "P2B_Car.yaml", 2, 256, 512, models, seed=22)   # BASELINE.json configs[0] shape; B=2 (B=1 is a degenerate BatchNorm case)
     gen_m2track(models)
-    gen_checkpoint_eval(models)
     np.savez_compressed(os.path.join(HERE, "ref_models.npz"), **models)
-    for f in ("ref_modules.npz", "ref_models.npz"):
+    full = {}
+    gen_bat_eval_full(full)
+    np.savez_compressed(os.path.join(HERE, "ref_bat_eval_full.npz"), **full)
+    for f in ("ref_modules.npz", "ref_models.npz", "ref_bat_eval_full.npz"):
         print(f, os.path.getsize(os.path.join(HERE, f)) // 1024, "KiB")
 
 

@@ -1,5 +1,7 @@
 """Drop-in check of the checkpoint surface (SURVEY.md §8f rank 1): the reference's shipped BAT / M2-Track checkpoints
-load, key for key, into our modules.  Runs only where /root/reference exists (the authoring container)."""
+load, key for key, into our modules.  The checkpoints are read from tests/golden/ckpt/: the reference's files with their
+keys, order, shapes, dtypes and hyper-parameters intact but every tensor stored as one broadcast element
+(tests/golden/make_ckpt_fixtures.py; Adam moments dropped), since the originals are 17-27 MB each."""
 import os
 
 import pytest
@@ -10,8 +12,7 @@ from open3dsot_b200.config import load_config
 from open3dsot_b200.models import get_model
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CKPT_DIR = "/root/reference/pretrained_models"
-pytestmark = pytest.mark.skipif(not os.path.isdir(CKPT_DIR), reason="reference checkpoints not present on this box")
+CKPT_DIR = os.path.join(ROOT, "tests", "golden", "ckpt")
 
 
 @pytest.mark.parametrize("ckpt,cfg_file", [("bat_kitti_car.ckpt", "BAT_Car.yaml"),

@@ -140,7 +140,7 @@ def test_running_stats_follow_torch_batchnorm():
     assert int(specs[0].bn.num_batches_tracked) == 1
 
 
-# ---------------------------------------------------------------------------------------------- tcgen05 core
+# ---------------------------------------------------------------------------------------------- wgmma core
 TC_CASES = [
     ("tc_sa2", [132, 128, 128, 256], 32 * 64, 32),
     ("tc_sa3", [260, 256, 256, 256], 32 * 37, 32),      # ragged P (1184 = 9.25 tiles), K = 260 (9 k-blocks, tail)
@@ -153,7 +153,7 @@ TC_CASES = [
 @pytest.mark.parametrize("level", [1, 3])
 @pytest.mark.parametrize("name,chans,P,S", TC_CASES + [("tc_wgrad_big", [260, 256, 256, 256], 32 * 160, 32)])
 def test_tensor_core_stack_matches_fp64_reference(name, chans, P, S, level):
-    """tcgen05 3xTF32 forward + dgrad against the fp64 statement: same 1e-4 bar as the exact-fp32 kernels."""
+    """wgmma 3xTF32 forward + dgrad against the fp64 statement: same 1e-4 bar as the exact-fp32 kernels."""
     from open3dsot_b200 import runtime
     torch.manual_seed(3)
     mod = pt.SharedMLP(list(chans), bn=True)

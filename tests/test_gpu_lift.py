@@ -5,7 +5,7 @@ first 1x1 convolution applied to the source points (no grouped tensor) against
   (b) the materialising path of round 1 (O3D_LIFT=0: ball-query+group kernel, then a GEMM over the grouped rows),
 
 forward and every gradient, on shapes that take the CUDA-core fallback (Y0 stored) and on shapes that take the tensor-core
-path (Y0 virtual: gathered inside the tcgen05 operand loaders / dgrad epilogue)."""
+path (Y0 virtual: gathered inside the wgmma operand loaders / dgrad epilogue)."""
 import pytest
 import torch
 
@@ -57,7 +57,7 @@ SA_CASES = [
     ("small_xyzgrad", 2, 96, 8, [8, 16, 16, 32], 24, 0.35, 16, False, True),
     ("sa1_nofeat", 8, 512, 0, [0, 64, 64, 128], 256, 0.3, 32, True, False),         # tensor-core path, K1 = 64
     ("sa2", 8, 256, 128, [128, 128, 128, 256], 128, 0.5, 32, False, False),        # K1 = 128
-    ("sa3", 8, 128, 256, [256, 256, 256, 256], 64, 0.7, 32, False, False),         # K1 = 256, MT = 2
+    ("sa3", 8, 128, 256, [256, 256, 256, 256], 64, 0.7, 32, False, False),         # K1 = 256, two channel tiles
     ("rpn_vote", 12, 128, 257, [257, 256, 256, 256], 64, 0.3, 16, False, True),    # nsample 16, ragged channels, d/d xyz
 ]
 

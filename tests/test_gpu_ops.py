@@ -1,4 +1,4 @@
-"""GPU parity of the sm_100a kernels (through the C ABI) against the oracle: bit-exact indices, 1e-4-relative
+"""GPU parity of the sm_90a kernels (through the C ABI) against the oracle: bit-exact indices, 1e-4-relative
 floats (north_star).  Edge cases per SURVEY.md §8c: duplicates, near-origin points, all-zero clouds, N not a
 multiple of the block, N < block, empty balls, on-radius points, > nsample hits, m < 3, repeated indices."""
 import numpy as np

@@ -183,10 +183,8 @@ def test_full_size_parity_with_injected_choices(name, cfg_file, B, M, N):
     worst = sorted(relg.items(), key=lambda kv: -kv[1])[:3]
     print(f"[{name}] gradient error vs the float64 oracle over all {len(pnames)} parameters: CUDA path {e_cuda:.1e}, "
           f"float32 oracle {e_o32:.1e}; worst CUDA tensors: " + ", ".join(f"{k} {v:.1e} (oracle32 {relo[k]:.1e})" for k, v in worst))
-    # Measured (profiles/r2_gradient_noise_analysis.txt): BAT 48 pairs 1.4e-3 (oracle32 3.3e-3), P2B 8 pairs 6.8e-3 (3.2e-3), BAT
-    # pedestrian 16 pairs 2.1e-2 (1.6e-3) — the last one a single marginal unit in the 1,024-position proposal head that any 1e-7
-    # perturbation tips (three unrelated stacks, each exact in isolation, produce the same 2.04e-2; the exact-fp32 run is at 8e-4).
-    # Flip noise has a heavy tail, so the whole-model bound is a coarse one; the sharp gradient checks are the per-module ones
+    # A single marginal unit (e.g. in the 1,024-position proposal head of the pedestrian case) that any 1e-7 perturbation tips
+    # moves the whole-model gradient error by ~1e-2 at once, whatever computed it.  Flip noise has a heavy tail, so the whole-model bound is a coarse one; the sharp gradient checks are the per-module ones
     # below (test_module_gradients_against_float64_oracle), where no chain of forty masks sits between the kernel and the number.
     assert e_cuda < max(4 * e_o32, 3e-2), (e_cuda, e_o32)
 
@@ -224,10 +222,9 @@ SA_SHAPES = [  # B, N, C, mlp, npoint, nsample, radius   (SA1 / SA2 / SA3 of the
 
 @pytest.mark.parametrize("shape", SA_SHAPES, ids=[f"B{s[0]}_N{s[1]}_C{s[2]}" for s in SA_SHAPES])
 def test_sa_layer_gradients_against_float64_oracle(shape):
-    """One set-abstraction layer (ball query + lifted first layer + tcgen05 GEMMs + max-pool), forward and EVERY gradient, against
-    the oracle composition evaluated in float64.  Without a flipped ReLU / arg-max decision the error is ~1e-6 .. 1e-5; every
-    decision at its threshold adds ~1e-4 (profiles/r2_gradient_noise_analysis.txt) and the 48-cloud shapes (up to 1.6e6 positions
-    x 3 layers of units) collect a handful: measured 8e-6 .. 6.4e-4 for the parameters, up to 1.0e-3 for the feature gradient.
+    """One set-abstraction layer (ball query + lifted first layer + wgmma GEMMs + max-pool), forward and EVERY gradient, against
+    the oracle composition evaluated in float64.  Without a flipped ReLU / arg-max decision the error is at fp32 round-off; every
+    decision at its threshold adds ~1e-4, and the 48-cloud shapes (up to 1.6e6 positions x 3 layers of units) collect a handful.
     The bar is 2e-3; a wrong kernel shows as O(1e-1)."""
     from open3dsot_b200.pointnet2.utils.pointnet2_modules import PointnetSAModule
     B, N, C, mlp, npoint, S, r = shape

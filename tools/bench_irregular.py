@@ -36,7 +36,7 @@ def main():
     B = a.batch
     if a.dbg:
         from open3dsot_b200 import _lib
-        _lib.lib().o3d_debug_set(a.dbg, 0)
+        _lib.lib().o3d_debug_set(a.dbg)
     b = synthetic_siamese_batch(B, 512, 1024, seed=20260924)
     search = b["search_points"].to(dev)
     tmpl = b["template_points"].to(dev)

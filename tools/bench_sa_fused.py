@@ -65,7 +65,7 @@ def main():
     a = ap.parse_args()
     if a.dbg:
         from open3dsot_b200 import _lib
-        _lib.lib().o3d_debug_set(a.dbg, 0)
+        _lib.lib().o3d_debug_set(a.dbg)
     torch.manual_seed(0)
     res = {}
     with torch.no_grad(), runtime.static_weights_scope():

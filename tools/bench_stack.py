@@ -27,7 +27,6 @@ def main():
     ap.add_argument("--dbg", default="0", help="comma-separated o3d_debug_set values, one measurement per value")
     ap.add_argument("--profile", action="store_true", help="print per-kernel device times of one fwd+bwd (CUPTI)")
     ap.add_argument("--no-dx", action="store_true", help="the stack input needs no gradient (first SA level)")
-    ap.add_argument("--force-mt", type=int, default=0)
     a = ap.parse_args()
     chans, P, S = SHAPES[a.shape]
     from open3dsot_b200 import _lib
@@ -42,7 +41,7 @@ def main():
     bwd_fl = sum(2 * nw[i + 1] + 2 * nw[i] for i in range(len(nw) - 1)) + sum(2 * nw[i + 1] + nw[i] for i in range(len(nw) - 1))
     gb_f, gb_b = 4e-9 * P * fwd_fl, 4e-9 * P * bwd_fl
     for lv, dbg in [(int(v), int(d)) for v in a.levels.split(",") for d in a.dbg.split(",")]:
-        _lib.lib().o3d_debug_set(dbg, a.force_mt)
+        _lib.lib().o3d_debug_set(dbg)
         runtime.set_tc(lv)
         xin = x.clone().requires_grad_(not a.fwd_only and not a.no_dx)
         for _ in range(2):
