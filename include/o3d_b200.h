@@ -356,6 +356,23 @@ int o3d_crop_box_frame(const float* scans, const long long* count, const long lo
 int o3d_resample(const float* points, const unsigned char* keep, const float* u_perm, const float* u_pick, int B, int N, int size,
                  int32_t* scratch, float* out, long long* src, long long* n_out, void* stream);
 
+/* Block 6 — split evaluation with K tracklets in flight (tracking/batched_tracker.py).
+ *
+ * o3d_keyed_uniform: out [K, n] uniform [0, 1) draws of one stream.  Slot k's element e is a pure function of
+ *   (seed, tracklet[k], frame[k], stream, e): Philox4x32-10 (cuRAND's constants) with key = (seed, (uint32) tracklet[k]) and
+ *   counter = (e / 4, (uint32) frame[k], stream, 0); word e % 4 of the block -> (w >> 8) * 2^-24.  tracklet / frame [K] int64.
+ *   K <= 65535.
+ * o3d_track_metrics: utils/metrics.py estimateOverlap(gt, result, dim, up_axis) and estimateAccuracy(...) in fp64, one slot per
+ *   thread.  The result box is the slot's fp32 state: center [K, 3], rot [K, 9] (row-major), wlh [K, 3]; the ground truth is fp64,
+ *   indexed by the slot's pool frame: gt_center [F, 3], gt_rot [F, 9], gt_wlh [F, 3], frame [K] int64 (< 0 = idle slot: writes
+ *   nothing).  dim = 2 (bird's-eye IoU, distance over the up axis components) or 3.  up_mask: bit i set <=> up_axis[i] != 0.
+ *   Writes overlap[frame[k]] and distance[frame[k]] ([F] fp64).                                                               */
+int o3d_keyed_uniform(const long long* tracklet, const long long* frame, int K, unsigned int seed, int stream, int n, float* out,
+                      void* cuda_stream);
+int o3d_track_metrics(const float* center, const float* rot, const float* wlh, const double* gt_center, const double* gt_rot,
+                      const double* gt_wlh, const long long* frame, int K, int dim, int up_mask, double* overlap, double* distance,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -77,6 +77,8 @@ PROTOTYPES = {
     "o3d_sa_fused_prepared_bytes": [_p],
     "o3d_sa_fused_prepare": [_p, _p, _p],
     "o3d_sa_fused_forward": [_p, _p, _p, _p, _p, _i, _i, _i, _i, ctypes.c_float, _i, _i, _p, _i, _p, _p],
+    "o3d_keyed_uniform": [_p, _p, _i, ctypes.c_uint, _i, _i, _p, _p],
+    "o3d_track_metrics": [_p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p],
 }
 _RESTYPE = {"o3d_last_error": ctypes.c_char_p, "o3d_pw_tc_wtile_bytes": ctypes.c_longlong,
             "o3d_stack_workspace_bytes": ctypes.c_longlong, "o3d_stack_prepared_bytes": ctypes.c_longlong,

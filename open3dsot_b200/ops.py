@@ -248,3 +248,43 @@ def crop_box_frame(scans, center, rot, half, frame=None, count=None):
           None if frame is None else frame.data_ptr(), center.data_ptr(), rot.data_ptr(), half.data_ptr(), B, N,
           local.data_ptr(), keep.data_ptr(), _stream())
     return local, keep
+
+
+# ------------------------------------------------------------------ split evaluation, K tracklets in flight (tracking/batched_tracker.py)
+def keyed_uniform(tracklet, frame, seed, stream, n, out=None):
+    """Counter-based uniform [0, 1) draws (csrc/track_eval.cu): tracklet (K,) / frame (K,) int64 CUDA -> out (K, n) fp32, row k a pure
+    function of (seed, tracklet[k], frame[k], stream, element): Philox4x32-10, key (seed, tracklet), counter (e // 4, frame, stream, 0)."""
+    for t, name in ((tracklet, "tracklet"), (frame, "frame")):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.int64 or not t.is_contiguous():
+            raise RuntimeError(f"{name} must be a contiguous int64 CUDA tensor")
+    K = tracklet.shape[0]
+    assert frame.shape == (K,)
+    if out is None:
+        out = torch.empty(K, int(n), device=tracklet.device)
+    _chk_f(out, "out")
+    assert out.shape == (K, int(n))
+    _call("o3d_keyed_uniform", tracklet.data_ptr(), frame.data_ptr(), K, int(seed) & 0xFFFFFFFF, int(stream), int(n), out.data_ptr(),
+          _stream())
+    return out
+
+
+def up_mask(up_axis):
+    """Bit i set <=> up_axis[i] != 0 (the axes utils/metrics.py selects with `np.array(up_axis) != 0`)."""
+    return sum(1 << i for i, a in enumerate(up_axis) if a != 0)
+
+
+def track_metrics(center, rot, wlh, gt_center, gt_rot, gt_wlh, frame, dim, up_axis, overlap, distance):
+    """estimateOverlap(gt, result, dim, up_axis) / estimateAccuracy in fp64 per slot (csrc/track_eval.cu): result box center (K, 3),
+    rot (K, 3, 3), wlh (K, 3) fp32; ground truth gt_* (F, 3) / (F, 3, 3) / (F, 3) fp64; frame (K,) int64 pool frame of each slot
+    (< 0 = idle).  Writes overlap[frame[k]] / distance[frame[k]] of the fp64 (F,) records in place."""
+    for t, name in ((center, "center"), (rot, "rot"), (wlh, "wlh")):
+        _chk_f(t, name)
+    for t, name in ((gt_center, "gt_center"), (gt_rot, "gt_rot"), (gt_wlh, "gt_wlh"), (overlap, "overlap"), (distance, "distance")):
+        if not t.is_cuda or t.dtype != torch.float64 or not t.is_contiguous():
+            raise RuntimeError(f"{name} must be a contiguous float64 CUDA tensor")
+    if not frame.is_cuda or frame.dtype != torch.int64 or not frame.is_contiguous():
+        raise RuntimeError("frame must be a contiguous int64 CUDA tensor")
+    K = center.shape[0]
+    assert rot.shape == (K, 3, 3) and wlh.shape == (K, 3) and frame.shape == (K,)
+    _call("o3d_track_metrics", center.data_ptr(), rot.data_ptr(), wlh.data_ptr(), gt_center.data_ptr(), gt_rot.data_ptr(),
+          gt_wlh.data_ptr(), frame.data_ptr(), K, int(dim), up_mask(up_axis), overlap.data_ptr(), distance.data_ptr(), _stream())

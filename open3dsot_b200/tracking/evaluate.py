@@ -16,3 +16,53 @@ def evaluate(model, sequences, progress=None):
         if progress is not None:
             progress(i, succ.compute(), prec.compute())
     return {"success": succ.compute(), "precision": prec.compute(), "frames": frames, "results": results}
+
+
+def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 << 30, use_graph=True):
+    """`evaluate()` with `slots` tracklets in flight on the device (tracking/batched_tracker.py): one graph replay per frame
+    step for all of them, overlap and centre distance computed on the device, one device-to-host copy per chunk of tracklets
+    whose padded frames fit `max_resident_bytes` (a tracklet is never split).  The random draws of a tracklet are keyed by
+    (seed, its index in `sequences`, frame), so its result does not depend on `slots`.
+    Returns the keys of `evaluate()` ("results": a data_classes.Box list per tracklet, in input order) plus the per-frame
+    "overlaps" / "distances" (lists per tracklet).  Frame 0 of every tracklet is scored on the host, as the reference does:
+    its ground truth against itself sits exactly on Success's top threshold."""
+    import numpy as np
+
+    from ..datasets import data_classes
+    from ..utils.metrics import estimateAccuracy, estimateOverlap
+    from .batched_tracker import BatchedDeviceTracker, plan_chunks, pool_frame_bytes
+
+    sequences = list(sequences)
+    cfg = model.config
+    dim, up = cfg.IoU_space, cfg.up_axis
+    n = len(sequences)
+    lengths = [len(s) for s in sequences]
+    overlaps, distances, results = [[] for _ in range(n)], [[] for _ in range(n)], [[] for _ in range(n)]
+    for j, seq in enumerate(sequences):
+        if lengths[j]:
+            gt0 = seq[0]["3d_bbox"]
+            overlaps[j].append(estimateOverlap(gt0, gt0, dim=dim, up_axis=up))
+            distances[j].append(estimateAccuracy(gt0, gt0, dim=dim, up_axis=up))
+            results[j].append(gt0)
+    if any(n_ > 1 for n_ in lengths):
+        npts = max(f["pc"].points.shape[1] for s in sequences for f in s)
+        for chunk in plan_chunks(lengths, pool_frame_bytes(npts), max_resident_bytes):
+            if all(lengths[j] < 2 for j in chunk):
+                continue
+            trk = BatchedDeviceTracker(model, [sequences[j] for j in chunk], slots, seed=seed, ids=chunk, max_points=npts,
+                                       use_graph=use_graph)
+            ov, di, cen, rot = trk.run()
+            offsets = trk.plan["offsets"]
+            del trk
+            for i, j in enumerate(chunk):
+                o, L = int(offsets[i]), lengths[j]
+                wlh = np.asarray(sequences[j][0]["3d_bbox"].wlh, dtype=np.float32).astype(np.float64)   # the fp32 state's size
+                overlaps[j] += ov[o + 1: o + L].tolist()
+                distances[j] += di[o + 1: o + L].tolist()
+                results[j] += [data_classes.Box(cen[o + t], wlh, rot[o + t]) for t in range(1, L)]
+    succ, prec = Success(), Precision()
+    for j in range(n):
+        succ(overlaps[j])
+        prec(distances[j])
+    return {"success": succ.compute(), "precision": prec.compute(), "frames": sum(lengths), "results": results,
+            "overlaps": overlaps, "distances": distances}
