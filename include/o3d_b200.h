@@ -192,8 +192,6 @@ int o3d_dense_bwd_prep(const float* dout, int ldd, const float* out, int ldo, co
  * forward:  rows = Cout, K = Cin   (w = the padded conv weight)
  * dgrad  :  rows = Cin,  K = Cout  (w = its transpose)                                                */
 long long o3d_pw_tc_wtile_bytes(int rows, int K);
-void o3d_pw_tc_set_reverse(int rev);              /* next o3d_pw_*_tc launch of this thread walks the position tiles backwards */
-void o3d_debug_set(int tc_debug);   /* profiling experiments only (results invalid when non-zero) */
 int o3d_pw_tc_pretile(const float* w, int ldw, int rows, int K, void* wtiles, void* stream);
 int o3d_pw_fwd_tc(const float* x, int ldx, const float* in_scale, const float* in_shift, int in_relu, const void* wtiles,
                   const float* bias, int P, int K, int N, float* y, int ldy, double* sum, double* sumsq, int S,
@@ -247,7 +245,7 @@ typedef struct o3d_stack_t {
     int K0;         /* input row length (multiple of 4, zero padded)                             */
     int S;          /* pooling group size over consecutive positions (0 = dense output)          */
     int training;   /* BatchNorm uses batch statistics and updates the running ones              */
-    int use_tc;     /* allow the wgmma 3xTF32 kernels where    the shape qualifies                */
+    int use_tc;     /* allow the wgmma 3xTF32 kernels where the shape qualifies: bit 0 = forward + dgrad, bit 1 = wgrad */
     int xyz_first;  /* layer-0 weight columns are [xyz(3) | features(c0)], input rows [features | dx dy dz 0] */
     int c0;         /* real feature channels of layer 0 when xyz_first                           */
     int dx_cols;    /* backward: only the first dx_cols input columns need a gradient (0 = all K0) */
@@ -304,7 +302,7 @@ int o3d_sa_fused_forward(const o3d_stack_t* d, const void* block, const float* x
  * o3d_lift_scatter: dY0 = a*g + b + cc*Y0 (a == NULL: dY0 = g) scattered into lf->d_z / d_cc / d_s / d_u (see o3d_lift_t);
  *                  y0 NULL = re-gather Y0 from Z.
  * o3d_pw_*_tc_lift: the tensor-core GEMMs of the layer AFTER the lifted one, reading Y0 through gidx (never stored).
- *                  wgrad: part != NULL selects the wide-tile split-K kernel (deterministic), NULL the 128x128 RED kernel.   */
+ *                  wgrad: split-K into the workspace `part`, as o3d_pw_wgrad_tc2.                                       */
 int o3d_lift_stats(const o3d_lift_t* lf, int P, int C0, int32_t* gidx, float* y0, double* sum, double* sumsq, void* stream);
 int o3d_lift_scatter(const o3d_lift_t* lf, int P, int C0, const int32_t* gidx, const float* y0, const float* g, int ldg,
                      const float* a, const float* b, const float* cc, void* stream);
@@ -320,14 +318,9 @@ int o3d_pw_wgrad_tc_lift(const float* g, int ldg, const float* y, int ldy, const
                          const float* in_scale, const float* in_shift, int in_relu, int P, int Cout, int Cin, float* dw,
                          int lddw, float* part, long long part_floats, void* stream);
 
-/* wgrad on the tensor core (operands transposed to K-major SWIZZLE_128B tiles, split over positions, fp32 RED into dw). */
-int o3d_pw_wgrad_tc(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
-                    const float* dpool, const int32_t* sel, int S, int ldp, const float* x, int ldx,
-                    const float* in_scale, const float* in_shift, int in_relu, int P, int Cout, int Cin, float* dw,
-                    int lddw, void* stream);
-
-/* wgrad, 128 x 128 tiles of dW per CTA, split over positions; the per-split partial tiles go
- * to `part` (o3d_pw_wgrad_tc2_workspace_floats() floats) and a second kernel adds their sum into dw.              */
+/* wgrad on the tensor core (operands transposed to K-major SWIZZLE_128B tiles), 128 x 128 tiles of dW per CTA, split over
+ * positions; the per-split partial tiles go to `part` (o3d_pw_wgrad_tc2_workspace_floats() floats) and a second kernel adds
+ * their sum into dw in a fixed order (deterministic).                                                               */
 long long o3d_pw_wgrad_tc2_workspace_floats(void);
 int o3d_pw_wgrad_tc2(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
                      const float* dpool, const int32_t* sel, int S, int ldp, const float* x, int ldx,

@@ -133,7 +133,10 @@ __device__ __forceinline__ uint32_t o3d_lanemask_lt() {
     asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));
     return m;
 }
-// debug switch (o3d_debug_set bit 7): few-column wgrads go through the tiled CUDA-core kernel instead of the streaming one
-extern int o3d_g_no_skinny;
+// o3d_pw_fwd_tc (pwmlp_tc.cu) with the direction of its walk over the position tiles: reverse = last tile first.  The
+// exported entry always walks forward; the stack sequencer (stack.cu) alternates the direction from layer to layer.
+int o3d_pw_fwd_tc_dir(const float* x, int ldx, const float* in_scale, const float* in_shift, int in_relu, const void* wtiles,
+                      const float* bias, int P, int K, int N, float* y, int ldy, double* sum, double* sumsq, int S, float* ymax,
+                      float* ymin, int32_t* arg, int ldp, void* stream, bool reverse);
 
 #endif

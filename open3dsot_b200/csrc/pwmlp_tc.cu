@@ -140,7 +140,6 @@ struct TcDy {
     const float* g; int ldg; const float* y; int ldy; const float* a; const float* b; const float* cc;
     const float* dpool; const int32_t* sel; int S; int ldp;
     int sh;   // S == 1 << sh (pooling group sizes are powers of two on this path)
-    int dbg;  // profiling experiments: 256 = no sel / dpool loads, 512 = no y load
     struct Coef { float4 a, b, c; bool on; };
     // raw operand rows of one thread for one k-block: rows p0 + i * stride, i < R (R >= 2).
     // Pooled gradient: when all R rows fall into one pooling group — the usual case, a thread's rows are neighbours — the
@@ -166,13 +165,9 @@ struct TcDy {
             if (R >= 2 && (pf >> sh) == (pl >> sh)) {   // the two tables live in g[0], g[1]
                 bt.shared = true;
                 const size_t go = (size_t)(pf >> sh) * ldp + kk;
-                if (!(dbg & 256)) {
-                    bt.g[0] = ld4g(dpool + go);
-                    const int4 sl = __ldg(reinterpret_cast<const int4*>(sel + go));
-                    bt.g[R >= 2 ? 1 : 0] = make_float4(__int_as_float(sl.x), __int_as_float(sl.y), __int_as_float(sl.z), __int_as_float(sl.w));
-                } else {
-                    bt.g[0] = bt.g[R >= 2 ? 1 : 0] = make_float4(0.f, 0.f, 0.f, 0.f);
-                }
+                bt.g[0] = ld4g(dpool + go);
+                const int4 sl = __ldg(reinterpret_cast<const int4*>(sel + go));
+                bt.g[R >= 2 ? 1 : 0] = make_float4(__int_as_float(sl.x), __int_as_float(sl.y), __int_as_float(sl.z), __int_as_float(sl.w));
             } else {
 #pragma unroll
                 for (int i = 0; i < R; ++i) {
@@ -194,7 +189,7 @@ struct TcDy {
 #pragma unroll
         for (int i = 0; i < R; ++i) {
             const int p = p0 + i * stride;
-            bt.y[i] = (a && !(dbg & 512)) ? ld4g(y + (size_t)(p < P ? p : P - 1) * ldy + kk) : make_float4(0.f, 0.f, 0.f, 0.f);
+            bt.y[i] = a ? ld4g(y + (size_t)(p < P ? p : P - 1) * ldy + kk) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
     }
     template <int R>
@@ -452,11 +447,9 @@ __device__ __forceinline__ void stage_acc(const float (&acc)[R], float* stg, int
     }
 }
 
-// dbg (profiling experiments only; results are wrong when set): 2 = producers skip the global loads, 4 = epilogue skips its
-// global stores / loads
 template <class BLoad, class Epi>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-    pw_tc_kernel(BLoad bl, const uint8_t* __restrict__ wtiles, int P, int K, int Nw, int nkb, Epi epi, int dbg, int rev) {
+    pw_tc_kernel(BLoad bl, const uint8_t* __restrict__ wtiles, int P, int K, int Nw, int nkb, Epi epi, int rev) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* tail = smem + TC_STAGES * TC_STAGE_BYTES + 2 * TC_EPI_BYTES;
@@ -488,7 +481,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         int32_t* gsm = reinterpret_cast<int32_t*>(tail + 256);           // [2][TC_N] row indices
         float4* ssm = reinterpret_cast<float4*>(tail + 256 + 1024);      // [2][TC_N] per-position scalars
         epi.begin(ch, Nw);
-        const int Nw_e = (dbg & 4) ? 0 : Nw;          // dbg: ch >= Nw_e -> the epilogue body is skipped
         int stage = 0, phase = 0, buf = 0;
         for (int t = blockIdx.x; t < n_ptiles; t += gridDim.x) {
             const int pt0 = tile_of(t) * TC_N;
@@ -506,7 +498,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                 }
             }
             const int pb = pt0 + h * 64;
-            epi.prefetch(ch, Nw_e, pb, P);
+            epi.prefetch(ch, Nw, pb, P);
             float acc[64];
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
@@ -537,8 +529,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                     r[4 * j] = __float_as_uint(v.x); r[4 * j + 1] = __float_as_uint(v.y);
                     r[4 * j + 2] = __float_as_uint(v.z); r[4 * j + 3] = __float_as_uint(v.w);
                 }
-                epi.group(r, ch, Nw_e, pb + cg * 16, P);
-                if (cg + 1 < 4) epi.prefetch(ch, Nw_e, pb + (cg + 1) * 16, P);
+                epi.group(r, ch, Nw, pb + cg * 16, P);
+                if (cg + 1 < 4) epi.prefetch(ch, Nw, pb + (cg + 1) * 16, P);
             }
             buf ^= 1;
         }
@@ -552,7 +544,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         const int chunk = pt & 7;                         // 16-byte chunk (4 channels) inside the 128-byte row
         const int row0 = (pt >> 3) * 4;                   // 4 neighbouring rows row0 + i, i < 4 (one pooling group)
         int stage = 0, phase = 0;
-        if (dbg & 2) P = 0;                               // dbg: nothing is loaded
         // The (tile, k-block) nest is walked as one flat sequence of items so that the raw loads of the item ahead — also
         // when it belongs to the next position tile — are in flight while the current one is being stored.
         struct Cur { int t, kb, p0; };
@@ -568,7 +559,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             if (c.t >= n_ptiles) return;
             const int k = c.kb * TC_K + chunk * 4;
             cf = bl.prep(k, K);
-            if (P > 0) bl.fetch(r, c.p0 + row0, 1, P, k, K);
+            bl.fetch(r, c.p0 + row0, 1, P, k, K);
         };
         Cur c0{(int)blockIdx.x, 0, 0};
         if (c0.t < n_ptiles) c0.p0 = tile_of(c0.t) * TC_N;
@@ -589,7 +580,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             uint8_t* xlo = xhi + TILE_BYTES;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                const float4 v = P > 0 ? bl.finish(r0, f0, i, c0.p0 + row0 + i, P) : make_float4(0.f, 0.f, 0.f, 0.f);
+                const float4 v = bl.finish(r0, f0, i, c0.p0 + row0 + i, P);
                 const uint32_t off = sw128(row0 + i, chunk);
                 *reinterpret_cast<float4*>(xhi + off) = hi_part(v);
                 *reinterpret_cast<float4*>(xlo + off) = lo_part(v);
@@ -611,7 +602,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 // positions x 16 channels (64-byte row segments) so that its transposed stores hit 16 banks (2-way conflicts).
 //   warps 0-3, 4-7  consumers: warpgroup h accumulates rows m0 + h*64 .. of the tile (wgmma m64n128k8, 3xTF32), then writes
 //                   its partial tile: plain stores into the split-K workspace part[split][m][n] (summed in a fixed order by
-//                   wgrad_reduce_kernel: deterministic), or fp32 REDs into dW when no workspace is given
+//                   wgrad_reduce_kernel: deterministic)
 //   warps 8-15      producers: each thread owns 4 channels x 4 positions of both operands per k-block; producer thread 0
 //                   also keeps the L2 prefetch of the slice's rows WG_AHEAD k-blocks ahead of the stores (requesting the whole
 //                   slice up front asks for more than the L2 holds across the grid, and the lines are evicted again before
@@ -641,8 +632,7 @@ __device__ __forceinline__ void store_transposed(const L& ld, const typename L::
 
 template <class XB>
 __global__ void __launch_bounds__(WG_THREADS, 1)
-    pw_wgrad_tc_kernel(TcDy da, XB xb, int P, int M, int N, int chunk, float* __restrict__ dW, int lddw, float* __restrict__ part,
-                       int dbg) {
+    pw_wgrad_tc_kernel(TcDy da, XB xb, int P, int M, int N, int chunk, float* __restrict__ part) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * 4 * TILE_BYTES);
@@ -676,9 +666,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
             const uint32_t ab = sb + h * (TILE_BYTES / 2);                 // dY rows (channels) m0 + h*64 ..
             wgmma_fence_acc(acc);
             wgmma_fence();
-            if (!(dbg & 32))
-                wgmma_3xtf32_kblock<128>(acc, make_desc(ab), make_desc(ab + TILE_BYTES), make_desc(sb + 2 * TILE_BYTES),
-                                         make_desc(sb + 3 * TILE_BYTES), kb == 0);
+            wgmma_3xtf32_kblock<128>(acc, make_desc(ab), make_desc(ab + TILE_BYTES), make_desc(sb + 2 * TILE_BYTES),
+                                     make_desc(sb + 3 * TILE_BYTES), kb == 0);
             wgmma_commit();
             wgmma_wait<0>();
             wgmma_fence_acc(acc);
@@ -686,19 +675,14 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
             if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
         }
         const int Mt = TC_M * (int)gridDim.z, Nt = TC_N * (int)gridDim.y;
-        float* __restrict__ out = part ? part + (size_t)blockIdx.x * Mt * Nt : nullptr;
+        float* __restrict__ out = part + (size_t)blockIdx.x * Mt * Nt;
 #pragma unroll
         for (int i = 0; i < 64; i += 4) {
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 const int m = m0 + h * 64 + 16 * w + (lane >> 2) + 8 * rr, n = n0 + 8 * (i >> 2) + 2 * (lane & 3);
-                const float v0 = acc[i + 2 * rr], v1 = acc[i + 2 * rr + 1];
-                if (out) {
-                    *reinterpret_cast<float2*>(out + (size_t)m * Nt + n) = make_float2(v0, v1);   // zeros when the slice is empty
-                } else if (nkb > 0 && m < M) {
-                    if (n < N) atomicAdd(dW + (size_t)m * lddw + n, v0);
-                    if (n + 1 < N) atomicAdd(dW + (size_t)m * lddw + n + 1, v1);
-                }
+                // zeros when the slice is empty
+                *reinterpret_cast<float2*>(out + (size_t)m * Nt + n) = make_float2(acc[i + 2 * rr], acc[i + 2 * rr + 1]);
             }
         }
     } else {
@@ -709,7 +693,6 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
         TcDy::Batch<4> ra = {};
         typename XB::template Batch<4> rb = {};
         auto fetch = [&](int kb) {
-            if (dbg & 2) return;
             da.fetch(ra, kpos(kb) + prow0, 8, pend, m0 + c4 * 4, M);
             xb.fetch(rb, kpos(kb) + prow0, 8, pend, n0 + c4 * 4, N);
         };
@@ -783,16 +766,11 @@ __global__ void w_pretile_kernel(const float* __restrict__ W, int ld, int rows, 
     }
 }
 
-int g_tc_debug = 0;
-}  // namespace
-extern int o3d_g_fps_wide;
-extern int o3d_g_sa_fused_dbg;
-namespace {
 inline int ilog2_exact(int v) { int l = 0; while ((1 << l) < v) ++l; return l; }
-thread_local int g_tc_rev = 0;   // direction of the next launch (set by the stack sequencer)
 
+// reverse: walk the position tiles from the last to the first (see pw_tc_kernel)
 template <class BLoad, class Epi>
-int launch_tc(BLoad bl, const uint8_t* wtiles, int P, int K, int Nw, Epi epi, cudaStream_t st, const char* name) {
+int launch_tc(BLoad bl, const uint8_t* wtiles, int P, int K, int Nw, Epi epi, bool reverse, cudaStream_t st, const char* name) {
     auto kern = pw_tc_kernel<BLoad, Epi>;
     O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM), name);
     const int gy = (Nw + TC_M - 1) / TC_M;
@@ -801,20 +779,20 @@ int launch_tc(BLoad bl, const uint8_t* wtiles, int P, int K, int Nw, Epi epi, cu
     int gx = o3d_num_sms() / gy;
     if (gx < 1) gx = 1;
     if (gx > n_ptiles) gx = n_ptiles;
-    kern<<<dim3(gx, gy), TC_THREADS, TC_SMEM, st>>>(bl, wtiles, P, K, Nw, nkb, epi, g_tc_debug, g_tc_rev);
+    kern<<<dim3(gx, gy), TC_THREADS, TC_SMEM, st>>>(bl, wtiles, P, K, Nw, nkb, epi, reverse);
     O3D_CHECK_LAUNCH(name);
     return O3D_OK;
 }
 
 template <int LD, class BLoad>
 int launch_fwd(const BLoad& bl, const void* wtiles, const float* bias, int P, int K, int Nw, float* y, int ldy, double* sum,
-               double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp, cudaStream_t st) {
+               double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp, bool reverse, cudaStream_t st) {
     TcFwdEpi<LD> ep{};
     ep.y = y; ep.ldy = ldy; ep.bias = bias; ep.sum = sum; ep.sumsq = sumsq;
     ep.S = S; ep.ymax = ymax; ep.ymin = ymin; ep.arg = arg; ep.ldp = ldp;
     ep.log2S = 0;
     while ((1 << ep.log2S) < S) ++ep.log2S;
-    return launch_tc(bl, (const uint8_t*)wtiles, P, K, Nw, ep, st, "o3d_pw_fwd_tc");
+    return launch_tc(bl, (const uint8_t*)wtiles, P, K, Nw, ep, reverse, st, "o3d_pw_fwd_tc");
 }
 
 template <int LD, bool LIFT = false>
@@ -829,18 +807,10 @@ int launch_dgrad(const TcDy& bl, const void* wtiles_t, int P, int Cout, int Cin,
     ep.out = out; ep.ldo = ldo; ep.yprev = yprev; ep.ldyp = ldyp; ep.scale = pscale; ep.shift = pshift; ep.relu = prelu;
     ep.s1g = s1; ep.s2y = s2y;
     // GEMM: D[pos, cin] = sum_cout dY[pos, cout] * Wt[cin, cout]  ->  "K" = Cout, "Nw" = Cin
-    return launch_tc(bl, (const uint8_t*)wtiles_t, P, Cout, Cin, ep, st, "o3d_pw_dgrad_tc");
+    return launch_tc(bl, (const uint8_t*)wtiles_t, P, Cout, Cin, ep, false, st, "o3d_pw_dgrad_tc");
 }
 
 }  // namespace
-
-extern "C" void o3d_debug_set(int tc_debug) {
-    g_tc_debug = tc_debug;
-    o3d_g_no_skinny = (tc_debug & 128) != 0;
-    o3d_g_fps_wide = (tc_debug & 1024) != 0;
-    o3d_g_sa_fused_dbg = (tc_debug >> 11) & 15;
-}
-extern "C" void o3d_pw_tc_set_reverse(int rev) { g_tc_rev = rev; }
 
 extern "C" long long o3d_pw_tc_wtile_bytes(int rows, int K) {
     const long long mt = (rows + TC_M - 1) / TC_M, nkb = (K + TC_K - 1) / TC_K;
@@ -857,9 +827,9 @@ extern "C" int o3d_pw_tc_pretile(const float* w, int ldw, int rows, int K, void*
     return O3D_OK;
 }
 
-extern "C" int o3d_pw_fwd_tc(const float* x, int ldx, const float* in_scale, const float* in_shift, int in_relu,
-                             const void* wtiles, const float* bias, int P, int K, int N, float* y, int ldy, double* sum,
-                             double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp, void* stream) {
+int o3d_pw_fwd_tc_dir(const float* x, int ldx, const float* in_scale, const float* in_shift, int in_relu, const void* wtiles,
+                      const float* bias, int P, int K, int N, float* y, int ldy, double* sum, double* sumsq, int S, float* ymax,
+                      float* ymin, int32_t* arg, int ldp, void* stream, bool reverse) {
     O3D_REQUIRE(x && wtiles, O3D_ERR_ARG, "o3d_pw_fwd_tc: null pointer");
     O3D_REQUIRE(P >= 0 && K >= 4 && N >= 1 && (K & 3) == 0 && (ldx & 3) == 0, O3D_ERR_ARG, "o3d_pw_fwd_tc: bad sizes");
     O3D_REQUIRE(S == 0 || (P % S == 0 && 64 % S == 0 && ymax && ymin && arg), O3D_ERR_ARG,
@@ -869,12 +839,19 @@ extern "C" int o3d_pw_fwd_tc(const float* x, int ldx, const float* in_scale, con
     TcAct bl{x, ldx, in_scale, in_shift, in_relu};
     // the usual activation widths get a compile-time row stride (immediate store offsets in the epilogue)
     cudaStream_t st = (cudaStream_t)stream;
-#define O3D_FWD_ARGS bl, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, st
+#define O3D_FWD_ARGS bl, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, reverse, st
     if (ldy == 64) return launch_fwd<64>(O3D_FWD_ARGS);
     if (ldy == 128) return launch_fwd<128>(O3D_FWD_ARGS);
     if (ldy == 256) return launch_fwd<256>(O3D_FWD_ARGS);
     return launch_fwd<0>(O3D_FWD_ARGS);
 #undef O3D_FWD_ARGS
+}
+
+extern "C" int o3d_pw_fwd_tc(const float* x, int ldx, const float* in_scale, const float* in_shift, int in_relu,
+                             const void* wtiles, const float* bias, int P, int K, int N, float* y, int ldy, double* sum,
+                             double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp, void* stream) {
+    return o3d_pw_fwd_tc_dir(x, ldx, in_scale, in_shift, in_relu, wtiles, bias, P, K, N, y, ldy, sum, sumsq, S, ymax, ymin, arg,
+                             ldp, stream, false);
 }
 
 namespace {
@@ -885,7 +862,7 @@ int dgrad_tc_impl(const float* g, int ldg, const float* y, int ldy, const float*
     O3D_REQUIRE((g || dpool) && wtiles_t && out, O3D_ERR_ARG, "o3d_pw_dgrad_tc: null pointer");
     O3D_REQUIRE((Cout & 3) == 0 && (Cin & 3) == 0, O3D_ERR_ARG, "o3d_pw_dgrad_tc: channel counts must be multiples of 4");
     if (P == 0) return O3D_OK;
-    TcDy bl{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1), g_tc_debug};
+    TcDy bl{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1)};
     cudaStream_t st = (cudaStream_t)stream;
     const int ld = (!yprev || ldyp == ldo) ? ldo : 0;   // one compile-time stride serves both out and yprev
 #define O3D_DG_ARGS bl, wtiles_t, P, Cout, Cin, out, ldo, yprev, ldyp, pscale, pshift, prelu, s1, s2y, st, lv
@@ -919,56 +896,38 @@ extern "C" int o3d_pw_dgrad_tc_lift(const float* g, int ldg, const float* y, int
 }
 
 namespace {
-// part == nullptr: every split adds its tile into dw with fp32 REDs; otherwise the splits write partial tiles into `part`
-// (part_floats long) and wgrad_reduce_kernel sums them in split order (deterministic)
+// the splits write partial tiles into `part` (part_floats long) and wgrad_reduce_kernel adds their sum into dw in split order
+// (deterministic)
 template <class XB>
 int launch_wgrad(const TcDy& da, const XB& xb, int P, int Cout, int Cin, float* dw, int lddw, float* part, long long part_floats,
                  cudaStream_t st) {
     auto kern = pw_wgrad_tc_kernel<XB>;
-    const char* name = part ? "o3d_pw_wgrad_tc2" : "o3d_pw_wgrad_tc";
-    O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM), name);
+    O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM), "o3d_pw_wgrad_tc2");
     const int mt = (Cout + TC_M - 1) / TC_M, nt = (Cin + TC_N - 1) / TC_N;
     const int Mt = mt * TC_M, Nt = nt * TC_N;
     int splits = o3d_num_sms() / (mt * nt);
     if (splits < 1) splits = 1;
-    if (part) {
-        const long long cap = part_floats / ((long long)Mt * Nt);
-        if (splits > cap) splits = (int)cap;
-        // small problems (the heads: a few thousand positions): every split writes and the reduction re-reads a whole
-        // Mt x Nt partial tile, so at least 128 positions per split
-        const int by_size = (P + 127) / 128;
-        if (splits > by_size) splits = by_size;
-        O3D_REQUIRE(splits >= 1, O3D_ERR_ARG, "o3d_pw_wgrad_tc2: workspace too small");
-    }
+    const long long cap = part_floats / ((long long)Mt * Nt);
+    if (splits > cap) splits = (int)cap;
+    // small problems (the heads: a few thousand positions): every split writes and the reduction re-reads a whole
+    // Mt x Nt partial tile, so at least 128 positions per split
+    const int by_size = (P + 127) / 128;
+    if (splits > by_size) splits = by_size;
+    O3D_REQUIRE(splits >= 1, O3D_ERR_ARG, "o3d_pw_wgrad_tc2: workspace too small");
     int chunk = (P + splits - 1) / splits;
     chunk = ((chunk + TC_K - 1) / TC_K) * TC_K;
     splits = (P + chunk - 1) / chunk;
-    kern<<<dim3(splits, nt, mt), WG_THREADS, WG_SMEM, st>>>(da, xb, P, Cout, Cin, chunk, dw, lddw, part, g_tc_debug);
-    O3D_CHECK_LAUNCH(name);
-    if (part) {
-        dim3 rg((Cin / 4 + 31) / 32, Cout);
-        wgrad_reduce_kernel<<<rg, 256, 0, st>>>(part, splits, Mt, Nt, Cout, Cin, dw, lddw);
-        O3D_CHECK_LAUNCH("o3d_pw_wgrad_tc2: reduce");
-    }
+    kern<<<dim3(splits, nt, mt), WG_THREADS, WG_SMEM, st>>>(da, xb, P, Cout, Cin, chunk, part);
+    O3D_CHECK_LAUNCH("o3d_pw_wgrad_tc2");
+    dim3 rg((Cin / 4 + 31) / 32, Cout);
+    wgrad_reduce_kernel<<<rg, 256, 0, st>>>(part, splits, Mt, Nt, Cout, Cin, dw, lddw);
+    O3D_CHECK_LAUNCH("o3d_pw_wgrad_tc2: reduce");
     return O3D_OK;
 }
 inline TcLift make_tclift(const o3d_lift_t* lf, const int32_t* gidx, const float* scale, const float* shift, int relu) {
     return TcLift{LiftView{lf->z, lf->ldz, lf->z ? gidx : nullptr, lf->s, lf->u}, scale, shift, relu, 0};
 }
 }  // namespace
-
-extern "C" int o3d_pw_wgrad_tc(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b,
-                               const float* cc, const float* dpool, const int32_t* sel, int S, int ldp, const float* x,
-                               int ldx, const float* in_scale, const float* in_shift, int in_relu, int P, int Cout,
-                               int Cin, float* dw, int lddw, void* stream) {
-    O3D_REQUIRE((g || dpool) && x && dw, O3D_ERR_ARG, "o3d_pw_wgrad_tc: null pointer");
-    O3D_REQUIRE((Cout & 3) == 0 && (Cin & 3) == 0 && (ldx & 3) == 0, O3D_ERR_ARG,
-                "o3d_pw_wgrad_tc: channel counts / leading dimensions must be multiples of 4");
-    if (P == 0) return O3D_OK;
-    TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1), g_tc_debug};
-    TcAct xb{x, ldx, in_scale, in_shift, in_relu};
-    return launch_wgrad(da, xb, P, Cout, Cin, dw, lddw, nullptr, 0, (cudaStream_t)stream);
-}
 
 extern "C" long long o3d_pw_wgrad_tc2_workspace_floats(void) {
     return (long long)o3d_num_sms() * TC_M * TC_N;   // splits <= #SMs / tiles of dW, so splits * Mt * Nt <= #SMs * 128 * 128
@@ -982,7 +941,7 @@ extern "C" int o3d_pw_wgrad_tc2(const float* g, int ldg, const float* y, int ldy
     O3D_REQUIRE((Cout & 3) == 0 && (Cin & 3) == 0 && (ldx & 3) == 0 && (lddw & 3) == 0, O3D_ERR_ARG,
                 "o3d_pw_wgrad_tc2: channel counts / leading dimensions must be multiples of 4");
     if (P == 0) return O3D_OK;
-    TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1), g_tc_debug};
+    TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1)};
     TcAct xb{x, ldx, in_scale, in_shift, in_relu};
     return launch_wgrad(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
 }
@@ -993,11 +952,11 @@ extern "C" int o3d_pw_wgrad_tc_lift(const float* g, int ldg, const float* y, int
                                     const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift,
                                     int in_relu, int P, int Cout, int Cin, float* dw, int lddw, float* part,
                                     long long part_floats, void* stream) {
-    O3D_REQUIRE((g || dpool) && lf && (gidx || !lf->z) && dw, O3D_ERR_ARG, "o3d_pw_wgrad_tc_lift: null pointer");
+    O3D_REQUIRE((g || dpool) && lf && (gidx || !lf->z) && dw && part, O3D_ERR_ARG, "o3d_pw_wgrad_tc_lift: null pointer");
     O3D_REQUIRE((Cout & 3) == 0 && (Cin & 3) == 0 && lf->ldz == Cin && (lddw & 3) == 0, O3D_ERR_ARG,
                 "o3d_pw_wgrad_tc_lift: channel counts / leading dimensions");
     if (P == 0) return O3D_OK;
-    TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1), g_tc_debug};
+    TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1)};
     TcLift xb = make_tclift(lf, gidx, in_scale, in_shift, in_relu);
     xb.la = TC_K;      // a producer thread's next fetch lies one k-block of positions further
     return launch_wgrad(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
@@ -1015,7 +974,7 @@ extern "C" int o3d_pw_fwd_tc_lift(const o3d_lift_t* lf, const int32_t* gidx, con
     const int Nw = (N + 3) & ~3;
     const TcLift bl = make_tclift(lf, gidx, in_scale, in_shift, in_relu);
     cudaStream_t st = (cudaStream_t)stream;
-#define O3D_FWD_ARGS bl, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, st
+#define O3D_FWD_ARGS bl, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, false, st
     if (ldy == 64) return launch_fwd<64>(O3D_FWD_ARGS);
     if (ldy == 128) return launch_fwd<128>(O3D_FWD_ARGS);
     if (ldy == 256) return launch_fwd<256>(O3D_FWD_ARGS);

@@ -28,8 +28,6 @@
 #include "tc_ptx.cuh"
 #include "../../include/o3d_b200.h"
 
-int o3d_g_sa_fused_dbg = 0;   // experiments (o3d_debug_set bits 11-14): 1 = every weight tile as 4 bulk copies; wrong results: 2 = no weight copies, 4 = no MMAs, 8 = no epilogue work
-
 namespace {
 
 constexpr int SF_POS = 64;                  // positions per CTA
@@ -47,7 +45,7 @@ struct SfParams {
     int n, Cp, ldf, N, M, S, BM;
     float radius, radius2;
     int normalize;
-    int act_bytes, nslot, dbg;
+    int act_bytes, nslot;
     uint32_t wx_off;       // floats: W0's coordinate columns, [3][n_mt0 * 128]
     uint32_t tiles_off;    // bytes: weight tiles in consumption order (layer, channel tile, k-block)
     SfLayer l[O3D_MAX_LAYERS];
@@ -73,7 +71,7 @@ __device__ __forceinline__ void sf_layer(const SfParams& prm, int l, uint8_t* ac
         for (int mt = 0; mt < L.n_mt; ++mt) {
             for (int kb = 0; kb < L.nkb; ++kb) {
                 o3d_mbar_wait(full + slot, phase);
-                if ((NT == 64 || mt == h) && !(prm.dbg & 4)) {
+                if (NT == 64 || mt == h) {
                     const uint32_t wb = o3d_smem_u32(ring + slot * SF_WTILE) + (NT == 64 ? h * (TILE_BYTES / 2) : 0);
                     const uint32_t ab = o3d_smem_u32(act + kb * SF_ACT_KB);
                     wgmma_fence_acc(acc);
@@ -103,35 +101,33 @@ __device__ __forceinline__ void sf_layer(const SfParams& prm, int l, uint8_t* ac
         rel[0] = s_rel[16 * w + (lane >> 2)];
         rel[1] = s_rel[16 * w + (lane >> 2) + 8];
     }
-    if (!(prm.dbg & 8)) {
 #pragma unroll
-        for (int j = 0; j < NT / 8; ++j) {
-            const int ch = h * NT + 8 * j + 2 * (lane & 3);   // this thread's channels ch, ch + 1
-            if (!last && (ch >> 5) >= next_nkb) continue;     // padding no later layer reads (uniform over the warp)
-            const float2 sc = ld2g(vecs + L.vec_off + ch), sh = ld2g(vecs + L.vec_off + ldv + ch);
-            float2 wx0 = make_float2(0.f, 0.f), wx1 = wx0, wx2 = wx0;
+    for (int j = 0; j < NT / 8; ++j) {
+        const int ch = h * NT + 8 * j + 2 * (lane & 3);   // this thread's channels ch, ch + 1
+        if (!last && (ch >> 5) >= next_nkb) continue;     // padding no later layer reads (uniform over the warp)
+        const float2 sc = ld2g(vecs + L.vec_off + ch), sh = ld2g(vecs + L.vec_off + ldv + ch);
+        float2 wx0 = make_float2(0.f, 0.f), wx1 = wx0, wx2 = wx0;
+        if (first) {
+            wx0 = ld2g(vecs + prm.wx_off + ch);
+            wx1 = ld2g(vecs + prm.wx_off + ldv + ch);
+            wx2 = ld2g(vecs + prm.wx_off + 2 * ldv + ch);
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int pos = 16 * w + (lane >> 2) + 8 * r;
+            float a0 = acc[4 * j + 2 * r], a1 = acc[4 * j + 2 * r + 1];
             if (first) {
-                wx0 = ld2g(vecs + prm.wx_off + ch);
-                wx1 = ld2g(vecs + prm.wx_off + ldv + ch);
-                wx2 = ld2g(vecs + prm.wx_off + 2 * ldv + ch);
+                a0 = fmaf(wx2.x, rel[r].z, fmaf(wx1.x, rel[r].y, fmaf(wx0.x, rel[r].x, a0)));
+                a1 = fmaf(wx2.y, rel[r].z, fmaf(wx1.y, rel[r].y, fmaf(wx0.y, rel[r].x, a1)));
             }
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                const int pos = 16 * w + (lane >> 2) + 8 * r;
-                float a0 = acc[4 * j + 2 * r], a1 = acc[4 * j + 2 * r + 1];
-                if (first) {
-                    a0 = fmaf(wx2.x, rel[r].z, fmaf(wx1.x, rel[r].y, fmaf(wx0.x, rel[r].x, a0)));
-                    a1 = fmaf(wx2.y, rel[r].z, fmaf(wx1.y, rel[r].y, fmaf(wx0.y, rel[r].x, a1)));
-                }
-                const float v0 = fmaxf(fmaf(a0, sc.x, sh.x), floor_v), v1 = fmaxf(fmaf(a1, sc.y, sh.y), floor_v);
-                if (!last) {
-                    uint8_t* dst = act + (ch >> 5) * SF_ACT_KB + sw128(pos, (ch & 31) >> 2) + (ch & 3) * 4;
-                    const float h0 = hi1(v0), h1 = hi1(v1);
-                    *reinterpret_cast<float2*>(dst) = make_float2(h0, h1);
-                    *reinterpret_cast<float2*>(dst + SF_ACT_KB / 2) = make_float2(v0 - h0, v1 - h1);
-                } else {
-                    *reinterpret_cast<float2*>(stg + pos * lds + ch) = make_float2(v0, v1);
-                }
+            const float v0 = fmaxf(fmaf(a0, sc.x, sh.x), floor_v), v1 = fmaxf(fmaf(a1, sc.y, sh.y), floor_v);
+            if (!last) {
+                uint8_t* dst = act + (ch >> 5) * SF_ACT_KB + sw128(pos, (ch & 31) >> 2) + (ch & 3) * 4;
+                const float h0 = hi1(v0), h1 = hi1(v1);
+                *reinterpret_cast<float2*>(dst) = make_float2(h0, h1);
+                *reinterpret_cast<float2*>(dst + SF_ACT_KB / 2) = make_float2(v0 - h0, v1 - h1);
+            } else {
+                *reinterpret_cast<float2*>(stg + pos * lds + ch) = make_float2(v0, v1);
             }
         }
     }
@@ -144,7 +140,7 @@ __device__ __forceinline__ void sf_layer(const SfParams& prm, int l, uint8_t* ac
     // ---- D. max-pool over each centre's nsample positions: thread = channel
     const int ch = threadIdx.x;
     const int S = prm.S;
-    if (prm.dbg & 8 || ch >= ((L.cout + 31) & ~31) || ch >= ldo) return;
+    if (ch >= ((L.cout + 31) & ~31) || ch >= ldo) return;
     const bool real = ch < L.cout;
     for (int g = 0; g < SF_POS / S; ++g) {
         float mx = -INFINITY;
@@ -191,17 +187,8 @@ __global__ void __launch_bounds__(SF_THREADS, 1)
                 if (!L.mma) continue;
                 for (int t = 0; t < L.n_mt * L.nkb; ++t) {
                     o3d_mbar_wait(empty + slot, phase ^ 1);
-                    if (prm.dbg & 2) {
-                        o3d_mbar_arrive(full + slot);
-                    } else if (prm.dbg & 1) {
-                        o3d_mbar_expect_tx(full + slot, SF_WTILE);
-#pragma unroll
-                        for (int c = 0; c < 4; ++c)
-                            o3d_bulk_g2s(ring + slot * SF_WTILE + c * (SF_WTILE / 4), src + c * (SF_WTILE / 4), SF_WTILE / 4, full + slot);
-                    } else {
-                        o3d_mbar_expect_tx(full + slot, SF_WTILE);
-                        o3d_bulk_g2s(ring + slot * SF_WTILE, src, SF_WTILE, full + slot);
-                    }
+                    o3d_mbar_expect_tx(full + slot, SF_WTILE);
+                    o3d_bulk_g2s(ring + slot * SF_WTILE, src, SF_WTILE, full + slot);
                     src += SF_WTILE;
                     if (++slot == nslot) { slot = 0; phase ^= 1; }
                 }
@@ -449,7 +436,6 @@ extern "C" int o3d_sa_fused_forward(const o3d_stack_t* d, const void* block, con
     const int cpc = SF_POS / nsample;
     const int grid = (B * M) / cpc;
     prm.nslot = nslot;
-    prm.dbg = o3d_g_sa_fused_dbg;
     const int smem = 1024 + act + nslot * SF_WTILE + SF_MISC;
     O3D_CUDA(cudaFuncSetAttribute(sa_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "o3d_sa_fused_forward: smem attribute");
     sa_fused_kernel<<<grid, SF_THREADS, smem, (cudaStream_t)stream>>>(prm, (const uint8_t*)block, xyz, new_xyz, feat_cl, out, ldo, idx);

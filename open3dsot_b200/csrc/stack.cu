@@ -128,7 +128,9 @@ struct Plan {
     bool lift, virt;     // layer 0 lifted (o3d_lift_t); virt: Y0 is never stored (the tensor-core kernels gather it)
     size_t gidx;         // [P] int32: global Z row of every position (forward workspace)
     int Nw[O3D_MAX_LAYERS], K[O3D_MAX_LAYERS];
-    bool tc_f[O3D_MAX_LAYERS], tc_b[O3D_MAX_LAYERS];
+    // tensor-core kernels per layer: forward, dgrad, weight gradient (split-K over positions into the `wpart` workspace, partial
+    // tiles summed in a fixed order: deterministic)
+    bool tc_f[O3D_MAX_LAYERS], tc_b[O3D_MAX_LAYERS], tc_w[O3D_MAX_LAYERS];
     // forward (persisted) offsets
     size_t wp[O3D_MAX_LAYERS], wt[O3D_MAX_LAYERS], bias[O3D_MAX_LAYERS], y[O3D_MAX_LAYERS], vec[O3D_MAX_LAYERS],
         stat[O3D_MAX_LAYERS], tiles[O3D_MAX_LAYERS];
@@ -157,12 +159,14 @@ bool make_plan(const o3d_stack_t* d, Plan& p) {
                     d->P >= (d->training ? 128 : 16) &&
                     !(l == d->n_layers - 1 && d->S > 0 && 64 % d->S != 0);
         p.tc_b[l] = (d->use_tc & 1) && p.K[l] >= 64 && p.Nw[l] >= 32 && d->P >= 128;
+        p.tc_w[l] = (d->use_tc & 2) && p.Nw[l] >= 64 && p.K[l] >= 64 && d->P >= 4096;
     }
     if (p.lift) {
-        // Y0 stays virtual when all three GEMMs of layer 1 run on the tensor cores over whole 32-channel k-blocks
-        const bool tcw1 = (d->use_tc & 2) && p.Nw[1] >= 64 && p.K[1] >= 64 && d->P >= 4096;
-        // (inference: no weight-gradient kernel will run, so its size floor P >= 4096 does not apply)
-        p.virt = p.tc_f[1] && p.tc_b[1] && (tcw1 || !d->training) && tc_main(p.K[1]) == p.K[1] && p.K[1] % 32 == 0 && !(d->use_tc & 8);
+        // Y0 stays virtual when all three GEMMs of layer 1 run on the tensor cores over whole 32-channel k-blocks.  In eval mode
+        // the wgrad's size floor (P >= 4096) does not count: a weight gradient is rarely asked for there, and when it is, layer
+        // 1's runs on the tensor cores all the same, since only their operand loader can read a virtual Y0.
+        p.virt = p.tc_f[1] && p.tc_b[1] && (p.tc_w[1] || !d->training) && tc_main(p.K[1]) == p.K[1] && p.K[1] % 32 == 0;
+        if (p.virt) p.tc_w[1] = true;
     }
     // statistics block first (one memset)
     p.stat_all = o;
@@ -206,10 +210,9 @@ bool make_plan(const o3d_stack_t* d, Plan& p) {
     for (int i = 0; i < 2; ++i) { p.gbuf[i] = o; o += al(sizeof(float) * (size_t)p.P * maxk); }
     p.wpart = o;
     p.wpart_floats = 0;
-    if ((d->use_tc & 2) && d->P >= 4096) {
-        p.wpart_floats = o3d_pw_wgrad_tc2_workspace_floats();
-        o += al(sizeof(float) * (size_t)p.wpart_floats);
-    }
+    for (int l = 0; l < p.n; ++l)
+        if (p.tc_w[l]) p.wpart_floats = o3d_pw_wgrad_tc2_workspace_floats();
+    o += al(sizeof(float) * (size_t)p.wpart_floats);
     p.bwd_bytes = o;
     return true;
 }
@@ -327,15 +330,13 @@ extern "C" int o3d_stack_forward(const o3d_stack_t* d, const float* x, void* ws_
             // lifted layer: one gather pass = row indices + batch statistics (+ Y0 itself on the CUDA-core fallback)
             rc = o3d_lift_stats(d->lift, p.P, Nw, at<int32_t>(ws, p.gidx), p.virt ? nullptr : y, sum, sumsq, stream);
         } else if (l == 1 && p.virt) {
-            o3d_pw_tc_set_reverse(0);
             rc = o3d_pw_fwd_tc_lift(d->lift, at<int32_t>(ws, p.gidx), in_scale, in_shift, in_relu, wsp + p.tiles[l], bias, p.P, K,
                                     cout, y, Nw, sum, sumsq, pool ? p.S : 0, ymax, ymin, arg, Nw, stream);
         } else if (p.tc_f[l]) {
             // snake order: layer 0 starts where the grouping kernel finished (the end), layer 1 where layer 0 finished, ...
-            o3d_pw_tc_set_reverse((l & 1) == 0);
             void* tiles = wsp + p.tiles[l];
-            rc = o3d_pw_fwd_tc(cur, cur_ld, in_scale, in_shift, in_relu, tiles, bias, p.P, K, cout, y, Nw, sum, sumsq,
-                               pool ? p.S : 0, ymax, ymin, arg, Nw, stream);
+            rc = o3d_pw_fwd_tc_dir(cur, cur_ld, in_scale, in_shift, in_relu, tiles, bias, p.P, K, cout, y, Nw, sum, sumsq,
+                                   pool ? p.S : 0, ymax, ymin, arg, Nw, stream, (l & 1) == 0);
         } else {
             rc = o3d_pw_fwd(cur, cur_ld, in_scale, in_shift, in_relu, wt, Nw, bias, p.P, K, cout, y, Nw, sum, sumsq,
                             pool ? p.S : 0, ymax, ymin, arg, Nw, stream);
@@ -452,11 +453,9 @@ extern "C" int o3d_stack_backward(const o3d_stack_t* d, const float* x, const vo
             double* ps1 = want ? s1(l - 1) : nullptr;
             double* ps2 = want ? s1(l - 1) + K : nullptr;
             if (l == 1 && p.virt) {
-                o3d_pw_tc_set_reverse(0);
                 rc = o3d_pw_dgrad_tc_lift(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, wf + p.btiles[l], p.P, Nl, K, gout, K, d->lift,
                                           at<int32_t>(wf, p.gidx), psc, psh, prelu, ps1, ps2, stream);
             } else if (p.tc_b[l]) {
-                o3d_pw_tc_set_reverse(0);   // dgrad sweeps forward; the wgrad that follows sweeps the same rows backward
                 // tensor cores on the first floor(K/128)*128 input channels, exact CUDA-core kernel on the ragged tail
                 // (the xyz / box-cloud extras of a first layer)
                 const int Km = tc_main(K);
@@ -480,24 +479,15 @@ extern "C" int o3d_stack_backward(const o3d_stack_t* d, const float* x, const vo
         }
         if (d->d_weight[l]) {
             float* dwp = at<float>(wb, p.dwp[l]);
-            const bool tcw = (d->use_tc & 2) && Nl >= 64 && K >= 64 && p.P >= 4096;
             if (l == 1 && p.virt) {
-                // every tensor-core weight gradient goes through the split-K kernel whose partial tiles are summed by a second
-                // kernel in a fixed order (deterministic; measured 0.7 % faster over the step than the fp32-RED 128x128 kernel,
-                // which use_tc bit 2 still selects)
-                const bool wide = (d->use_tc & 4) == 0;
                 rc = o3d_pw_wgrad_tc_lift(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, d->lift, at<int32_t>(wf, p.gidx), psc, psh, prelu,
-                                          p.P, Nl, K, dwp, K, wide ? at<float>(wb, p.wpart) : nullptr, p.wpart_floats, stream);
-            } else if (tcw) {
+                                          p.P, Nl, K, dwp, K, at<float>(wb, p.wpart), p.wpart_floats, stream);
+            } else if (p.tc_w[l]) {
                 // tensor-core part: the first floor(K/128)*128 input channels; ragged tail (xyz / box-cloud extras)
                 // goes through the exact CUDA-core kernel on the remaining columns
                 const int Kmain = tc_main(K);
-                if ((d->use_tc & 4) == 0)       // deterministic split-K + ordered reduction (see above); bit 2: fp32-RED kernel
-                    rc = o3d_pw_wgrad_tc2(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, xin, K, psc, psh, prelu, p.P, Nl, Kmain, dwp,
-                                          K, at<float>(wb, p.wpart), p.wpart_floats, stream);
-                else
-                    rc = o3d_pw_wgrad_tc(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, xin, K, psc, psh, prelu, p.P, Nl, Kmain, dwp,
-                                         K, stream);
+                rc = o3d_pw_wgrad_tc2(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, xin, K, psc, psh, prelu, p.P, Nl, Kmain, dwp, K,
+                                      at<float>(wb, p.wpart), p.wpart_floats, stream);
                 if (rc) return rc;
                 if (K > Kmain)
                     rc = o3d_pw_wgrad(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, xin + Kmain, K, psc ? psc + Kmain : nullptr,

@@ -114,10 +114,6 @@ def _describe(meta, P, K0, params):
     return d
 
 
-def clear_prepared():
-    """kept for API symmetry: prepared blocks live ON the parameters they were built from and die with them"""
-
-
 def _versions(params):
     return tuple(-1 if t is None else t._version for t in params)
 
@@ -336,9 +332,9 @@ def _pow2_divisor(n, cap=64):
     return g
 
 
-def _liftable(specs, site=None, info=None):
+def _liftable(specs):
     """The first conv can be lifted when another layer follows it, its output width is a multiple of 4, and lifting is on."""
-    return runtime.lift_enabled(site, info) and len(specs) >= 2 and specs[0].weight.shape[0] % 4 == 0
+    return runtime.lift_enabled() and len(specs) >= 2 and specs[0].weight.shape[0] % 4 == 0
 
 
 def mlp_stack(x2d, specs, S=0, training=True, xyz_first=False, c0=0, dx_cols=0):
@@ -476,7 +472,7 @@ def sa_forward(sa, xyz, features, sample_idxs):
             pooled = _sa_fused_forward(specs, xyz_c, new_xyz, feat_cl, C, grouper.radius, S, grouper.normalize_xyz)
             outs.append(from_channels_last(pooled))
             continue
-        if _liftable(specs, "sa", {"N": N, "npoint": npoint, "S": S, "C": C}) and (specs[0].bias is None or feat_cl is not None):
+        if _liftable(specs) and (specs[0].bias is None or feat_cl is not None):
             # Lifted first layer: W0 . [x(idx) - c, f(idx)] = (W0_f . f)[idx] + W0_x . (x(idx) - c) — the feature part of the
             # convolution runs once per SOURCE point (z) and is gathered; the relative coordinates (dx, dy, dz) are applied per
             # position, directly (same difference-then-multiply arithmetic as the reference).  The grouped
@@ -602,7 +598,7 @@ def boxaware_xcorr_forward(xc, template_feature, search_feature, template_xyz, t
     if C % 4:
         tmpl = F.pad(tmpl, (0, _r4(C) - C))
     specs = parse_stack(xc.mlp)
-    if _liftable(specs, "bax") and (N * k) % 4 == 0:
+    if _liftable(specs) and (N * k) % 4 == 0:
         # lifted: the first conv runs on the M template rows; the (B, 268, N, k) grouped tensor is never built (xcorr.py:89-98)
         tm = tmpl.contiguous()
         z = mlp_stack(tm.view(B * M, tm.shape[2]), [_LayerSpec(specs[0].weight, specs[0].bias, None, False)], 0, xc.training)
@@ -626,7 +622,7 @@ def p2b_xcorr_forward(xc, template_feature, search_feature, template_xyz):
     sim_t = _P2BCosine.apply(t_cl.contiguous(), search_feature.transpose(1, 2).contiguous())       # (B,n2,n1), eps 1e-8
     sim = sim_t.transpose(1, 2)                                                                    # (B,n1,n2) as the reference
     specs = parse_stack(xc.mlp)
-    if _liftable(specs, "p2b") and (n1 & (n1 - 1)) == 0:
+    if _liftable(specs) and (n1 & (n1 - 1)) == 0:
         # lifted: the first conv's input [sim(1), xyz(3), feature(f)] (xcorr.py:39-46) is a per-template row plus ONE scalar
         # per (search, template) pair, so Y0[(b,j,i)] = (W[:,1:] . [xyz_i, f_i]) + sim[b,i,j] * W[:,0] and the
         # (B, 260, n1, n2) fusion tensor is never built

@@ -14,15 +14,8 @@ _TC = int(os.environ.get("O3D_TC", "3"))
 _LIFT = os.environ.get("O3D_LIFT", "1") != "0"
 
 
-LIFT_FILTER = None      # diagnostics: callable(site: str, info: dict) -> bool restricting which stacks are lifted
-
-
-def lift_enabled(site=None, info=None) -> bool:
-    if not _LIFT:
-        return False
-    if LIFT_FILTER is not None and site is not None:
-        return bool(LIFT_FILTER(site, info or {}))
-    return True
+def lift_enabled() -> bool:
+    return _LIFT
 
 
 def set_lift(flag: bool) -> None:
@@ -30,10 +23,6 @@ def set_lift(flag: bool) -> None:
     _LIFT = bool(flag)
 
 
-# Inference with static weights (the tracking loop): eval-mode stacks pack their weights and fold their running BatchNorm
-# statistics ONCE (o3d_stack_prepare) instead of per call.  Off by default — a cached block goes stale when the weights change
-# (the engine's fused Adam updates parameters in place without bumping tensor versions): turn it on only around inference,
-# and call fused.clear_prepared() after loading new weights.
 _SA_FUSED = os.environ.get("O3D_SA_FUSED", "1") != "0"
 
 
@@ -60,6 +49,8 @@ def set_branch_overlap(flag: bool) -> None:
     _BRANCH_OVERLAP = bool(flag)
 
 
+# Inference with static weights (the tracking loop): eval-mode stacks pack their weights and fold their running BatchNorm
+# statistics ONCE (o3d_stack_prepare) instead of per call.  Off by default; static_weights_scope() turns it on.
 _STATIC_WEIGHTS = False
 
 
@@ -67,14 +58,12 @@ def static_weights() -> bool:
     return _STATIC_WEIGHTS
 
 
-def set_static_weights(flag: bool) -> None:
-    global _STATIC_WEIGHTS
-    _STATIC_WEIGHTS = bool(flag)
-
-
 @contextlib.contextmanager
 def static_weights_scope():
-    """`with runtime.static_weights_scope():` — inference code whose weights do not change while it runs."""
+    """`with runtime.static_weights_scope():` — inference code whose weights do not change while it runs.
+
+    The cached blocks are keyed by the parameters' tensor versions, and the engine's fused Adam updates parameters in place
+    without bumping them: a scope must not span training steps, or the forward passes after a step run on the old weights."""
     global _STATIC_WEIGHTS
     old = _STATIC_WEIGHTS
     _STATIC_WEIGHTS = True
@@ -104,10 +93,6 @@ def grad_inplace_scope():
         yield
     finally:
         _GRAD_INPLACE = old
-
-
-def tc_enabled() -> bool:
-    return _TC != 0
 
 
 def tc_level() -> int:

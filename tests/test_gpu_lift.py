@@ -30,12 +30,12 @@ def _cloud(B, N, seed, spread=1.2):
     return xyz, g
 
 
-def _run_sa(lift, xyz, feats, mlp, npoint, radius, nsample, use_fps, xyz_grad, seed):
+def _run_sa(lift, xyz, feats, mlp, npoint, radius, nsample, use_fps, xyz_grad, train, seed):
     runtime.set_lift(lift)
     try:
         sa = PointnetSAModule(mlp=list(mlp), radius=radius, nsample=nsample, use_fps=use_fps)
         sa.load_state_dict(det_state_dict(sa.state_dict(), seed=seed))
-        sa = sa.cuda().train()
+        sa = sa.cuda().train(train)
         x = xyz.clone().cuda().requires_grad_(xyz_grad)
         f = None if feats is None else feats.clone().cuda().requires_grad_(True)
         nx, nf, _ = sa(x, f, npoint, True)
@@ -52,23 +52,25 @@ def _run_sa(lift, xyz, feats, mlp, npoint, radius, nsample, use_fps, xyz_grad, s
 
 
 SA_CASES = [
-    # name, B, N, C, mlp, npoint, radius, nsample, use_fps, xyz_grad
-    ("small_fps", 2, 96, 8, [8, 16, 16, 32], 24, 0.35, 16, True, False),            # CUDA-core fallback: Y0 materialised
-    ("small_xyzgrad", 2, 96, 8, [8, 16, 16, 32], 24, 0.35, 16, False, True),
-    ("sa1_nofeat", 8, 512, 0, [0, 64, 64, 128], 256, 0.3, 32, True, False),         # tensor-core path, K1 = 64
-    ("sa2", 8, 256, 128, [128, 128, 128, 256], 128, 0.5, 32, False, False),        # K1 = 128
-    ("sa3", 8, 128, 256, [256, 256, 256, 256], 64, 0.7, 32, False, False),         # K1 = 256, two channel tiles
-    ("rpn_vote", 12, 128, 257, [257, 256, 256, 256], 64, 0.3, 16, False, True),    # nsample 16, ragged channels, d/d xyz
+    # name, B, N, C, mlp, npoint, radius, nsample, use_fps, xyz_grad, train
+    ("small_fps", 2, 96, 8, [8, 16, 16, 32], 24, 0.35, 16, True, False, True),            # CUDA-core fallback: Y0 materialised
+    ("small_xyzgrad", 2, 96, 8, [8, 16, 16, 32], 24, 0.35, 16, False, True, True),
+    ("sa1_nofeat", 8, 512, 0, [0, 64, 64, 128], 256, 0.3, 32, True, False, True),         # tensor-core path, K1 = 64
+    ("sa2", 8, 256, 128, [128, 128, 128, 256], 128, 0.5, 32, False, False, True),        # K1 = 128
+    ("sa3", 8, 128, 256, [256, 256, 256, 256], 64, 0.7, 32, False, False, True),         # K1 = 256, two channel tiles
+    ("rpn_vote", 12, 128, 257, [257, 256, 256, 256], 64, 0.3, 16, False, True, True),    # nsample 16, ragged channels, d/d xyz
+    # eval mode keeps Y0 virtual below the wgrad's P >= 4096 floor (P = 2048): layer 1's weight gradient on the tensor cores
+    ("sa2_eval", 1, 256, 128, [128, 128, 128, 256], 64, 0.5, 32, False, False, False),
 ]
 
 
 @pytest.mark.parametrize("case", SA_CASES, ids=[c[0] for c in SA_CASES])
 def test_lifted_sa_matches_materialised_path(case):
-    name, B, N, C, mlp, npoint, radius, nsample, use_fps, xyz_grad = case
+    name, B, N, C, mlp, npoint, radius, nsample, use_fps, xyz_grad, train = case
     xyz, g = _cloud(B, N, seed=3)
     feats = torch.randn(B, C, N, generator=g) if C else None
-    o_l, g_l, s_l = _run_sa(True, xyz, feats, mlp, npoint, radius, nsample, use_fps, xyz_grad, seed=5)
-    o_m, g_m, s_m = _run_sa(False, xyz, feats, mlp, npoint, radius, nsample, use_fps, xyz_grad, seed=5)
+    o_l, g_l, s_l = _run_sa(True, xyz, feats, mlp, npoint, radius, nsample, use_fps, xyz_grad, train, seed=5)
+    o_m, g_m, s_m = _run_sa(False, xyz, feats, mlp, npoint, radius, nsample, use_fps, xyz_grad, train, seed=5)
     assert rel(o_l, o_m) < RTOL
     for a, b in zip(s_l, s_m):
         assert rel(a, b) < RTOL

@@ -38,18 +38,9 @@ dev = {k: v.cuda() for k, v in batch.items()}
 inject = {("ball_query", 6): taps["rpn.vote_aggregation:bq_idx"][0]}
 if name == "bat":
     inject[("boxaware_topk", 0)] = taps["xcorr:topk"][0]
-MODES = [("fused lift tc3", True, True, 3, None), ("fused lift tc0", True, True, 0, None), ("fused nolift tc3", True, False, 3, None),
-         ("fused nolift tc0", True, False, 0, None), ("composed (torch ops)", False, False, 0, None)]
-if len(sys.argv) > 6:     # bisect: lift only one class of stacks at a time
-    MODES = [("nolift tc3", True, False, 3, None),
-             ("lift bax only", True, True, 3, lambda s, i: s == "bax"),
-             ("lift rpn-sa only", True, True, 3, lambda s, i: s == "sa" and i["S"] == 16),
-             ("lift SA1 only", True, True, 3, lambda s, i: s == "sa" and i["C"] == 0),
-             ("lift SA2 only", True, True, 3, lambda s, i: s == "sa" and i["C"] == 128),
-             ("lift SA3 only", True, True, 3, lambda s, i: s == "sa" and i["C"] == 256 and i["S"] == 32),
-             ("lift all", True, True, 3, None)]
-for tag, fused_on, lift, tc, flt in MODES:
-    runtime.LIFT_FILTER = flt
+MODES = [("fused lift tc3", True, True, 3), ("fused lift tc0", True, True, 0), ("fused nolift tc3", True, False, 3),
+         ("fused nolift tc0", True, False, 0), ("composed (torch ops)", False, False, 0)]
+for tag, fused_on, lift, tc in MODES:
     net.load_state_dict(base)
     net.zero_grad(set_to_none=True)
     runtime.set_fused(fused_on); runtime.set_lift(lift); runtime.set_tc(tc)
