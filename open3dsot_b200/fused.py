@@ -75,8 +75,13 @@ def parse_stack(module):
 
 
 # ---------------------------------------------------------------------------------------------- the autograd op
+def _tracks_stats(bn):
+    return bn is not None and bn.track_running_stats and bn.running_mean is not None
+
+
 class _Meta:
-    """Static description of one stack invocation (python objects only)."""
+    """Static description of one stack invocation (python objects only), with the stack's flat parameter list
+    ([weight, bias, gamma, beta] per layer, None where a layer has no such tensor) and the running BatchNorm statistics."""
 
     def __init__(self, specs, S, training, xyz_first=False, c0=0, dx_cols=0):
         if len(specs) > _lib.MAX_LAYERS:
@@ -93,9 +98,14 @@ class _Meta:
         # a spec without weight is the lifted first layer (BatchNorm / ReLU only; `lift_c0` output channels)
         self.cout = [s.weight.shape[0] if s.weight is not None else s.lift_c0 for s in specs]
         self.cin = [s.weight.numel() // s.weight.shape[0] if s.weight is not None else 0 for s in specs]
+        self.params = []
+        for s in specs:
+            self.params += [s.weight, s.bias, s.bn.weight if s.bn is not None else None, s.bn.bias if s.bn is not None else None]
+        self.stats = [t for bn in self.bns if _tracks_stats(bn) for t in (bn.running_mean, bn.running_var)]
 
 
 def _describe(meta, P, K0, params):
+    """the StackDesc of `meta` over `params` (meta.params, or the same tensors as received by the autograd function)"""
     d = _lib.StackDesc()
     d.n_layers, d.P, d.K0, d.S = meta.n, P, K0, meta.S
     d.training, d.use_tc = int(meta.training), int(runtime.tc_level())
@@ -108,221 +118,158 @@ def _describe(meta, P, K0, params):
         if bn is not None:
             d.momentum[l] = 0.1 if bn.momentum is None else bn.momentum
             d.eps[l] = bn.eps
-            if bn.track_running_stats and bn.running_mean is not None:
+            if _tracks_stats(bn):
                 d.running_mean[l], d.running_var[l] = bn.running_mean.data_ptr(), bn.running_var.data_ptr()
                 d.num_batches_tracked[l] = bn.num_batches_tracked.data_ptr()
     return d
 
 
-def _versions(params):
-    return tuple(-1 if t is None else t._version for t in params)
+def _static_cached(tag, extra, deps, make):
+    """`make()` -- a tensor computed from the tensors `deps` (None entries allowed) -- cached for inference with static weights
+    (runtime.static_weights_scope).  The entry is stored on the first tensor of `deps`, keyed by `tag`, `extra` and the identity
+    of every dep, and is valid while every dep's version is unchanged (`load_state_dict` / in-place edits invalidate it).  It
+    keeps its deps alive, so their ids stay unique.
 
-
-def _cacheable():
-    """A cached tensor may be read from another stream (the template / search branches run side by side, fused.run_ahead) with no
-    ordering against the stream that built it.  Outside graph capture the builder therefore finishes before the entry becomes
-    visible (`_publish`); during capture nothing is cached — whatever is missing is built privately, as part of the graph."""
-    return not torch.cuda.is_current_stream_capturing()
-
-
-def _publish():
-    torch.cuda.current_stream().synchronize()
+    A cached tensor may be read from another stream (the template / search branches run side by side, run_ahead) with no
+    ordering against the stream that built it, so the builder finishes before the entry becomes visible.  During graph capture
+    nothing is cached: a missing value is built privately, as part of the graph.  Either way the caller keeps the returned
+    tensor referenced until the kernel that reads it is enqueued."""
+    owner = next(t for t in deps if t is not None)
+    cache = owner.__dict__.setdefault("_o3d_static", {})
+    key = (tag, extra, tuple(id(t) for t in deps))
+    versions = tuple(-1 if t is None else t._version for t in deps)
+    hit = cache.get(key)
+    if hit is not None and hit[0] == versions:
+        return hit[1]
+    value = make()
+    if not torch.cuda.is_current_stream_capturing():
+        torch.cuda.current_stream().synchronize()
+        cache[key] = (versions, value, deps)
+    return value
 
 
 def _derived(weight, tag, make):
     """A tensor computed from `weight` (e.g. a contiguous column slice).  With static weights and no autograd it is built once
-    and stored ON the weight (keyed by the weight's version counter: `load_state_dict` / in-place edits invalidate it), which
-    also keeps its address stable for the prepared-block cache."""
+    and cached on the weight, which also keeps its address stable for the prepared-block cache."""
     if not runtime.static_weights() or torch.is_grad_enabled():
         return make()
-    cache = weight.__dict__.setdefault("_o3d_derived", {})
-    hit = cache.get(tag)
-    if hit is None or hit[0] != weight._version:
-        if not _cacheable():
-            return make().detach()
-        hit = cache[tag] = (weight._version, make().detach())
-        _publish()
-    return hit[1]
+    return _static_cached(tag, None, [weight], lambda: make().detach())
 
 
-def _attach_prepared(d, meta, params, P, K0, lifted, need_grad, device):
-    """Inference with static weights: point the descriptor at the stack's prepared block (built on first use).  The block is
-    stored on the stack's first parameter tensor, keyed by the shape class and by every parameter's identity + version."""
-    if need_grad or meta.training or not runtime.static_weights():
-        return None
-    owner = next(t for t in params if t is not None)
-    cache = owner.__dict__.setdefault("_o3d_prepared", {})
-    key = (tuple(id(t) for t in params), P, K0, meta.S, lifted, runtime.tc_level(), meta.xyz_first, meta.c0)
-    ver = _versions(params)
-    hit = cache.get(key)
-    if hit is None or hit[0] != ver:
-        L = _lib.lib()
-        nbytes = L.o3d_stack_prepared_bytes(ctypes.byref(d))
-        if nbytes < 0:
-            raise RuntimeError("fused MLP stack: invalid stack description")
-        block = torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
-        _lib.check(L.o3d_stack_prepare(ctypes.byref(d), block.data_ptr(), _stream()), "o3d_stack_prepare")
-        hit = (ver, block, params)                        # params kept alive with the block: their ids stay unique
-        if _cacheable():
-            cache[key] = hit
-            _publish()
-    d.prepared = hit[1].data_ptr()
-    return hit[1]
+def _prepare_stack(d, device):
+    """the stack's prepared block: packed weights and folded running statistics (o3d_stack_prepare)"""
+    L = _lib.lib()
+    nbytes = L.o3d_stack_prepared_bytes(ctypes.byref(d))
+    if nbytes < 0:
+        raise RuntimeError("fused MLP stack: invalid stack description")
+    block = torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
+    _lib.check(L.o3d_stack_prepare(ctypes.byref(d), block.data_ptr(), _stream()), "o3d_stack_prepare")
+    return block
 
 
-def _param_grad_targets(ctx_needs, params, d, meta, first_param_index):
-    """Where a stack's backward writes its parameter gradients.  Default: fresh tensors returned to autograd.  Inside
-    `runtime.grad_inplace_scope()` and when EVERY parameter that needs a gradient is a leaf with a pre-allocated contiguous `.grad`
-    (the engine's flat bucket): the kernels add into those buffers directly and autograd gets None for them."""
-    need = [(l, j) for l in range(meta.n) for j in range(4)
-            if params[4 * l + j] is not None and ctx_needs[first_param_index + 4 * l + j]]
+def _param_grad_targets(needs, d, meta):
+    """Where a stack's backward writes its parameter gradients (`needs`: needs_input_grad of meta.params).  Default: fresh
+    tensors returned to autograd.  Inside `runtime.grad_inplace_scope()` and when EVERY parameter that needs a gradient is a leaf
+    with a pre-allocated contiguous `.grad` (the engine's flat bucket): the kernels add into those buffers directly and autograd
+    gets None for them."""
+    params = meta.params
+    need = [i for i, t in enumerate(params) if t is not None and needs[i]]
     inplace = runtime.grad_inplace() and bool(need) and all(
-        params[4 * l + j].is_leaf and params[4 * l + j].grad is not None and params[4 * l + j].grad.is_contiguous()
-        and params[4 * l + j].grad.dtype == torch.float32 for l, j in need)
-    grads = [None] * (4 * meta.n)
-    fields = (d.d_weight, d.d_bias, d.d_gamma, d.d_beta)
-    for l in range(meta.n):
-        for j in range(4):
-            fields[j][l] = None
-    for l, j in need:
-        t = params[4 * l + j]
-        if inplace:
-            fields[j][l] = t.grad.data_ptr()
-        else:
-            gt = torch.empty_like(t)
-            grads[4 * l + j] = gt
-            fields[j][l] = gt.data_ptr()
+        params[i].is_leaf and params[i].grad is not None and params[i].grad.is_contiguous() and params[i].grad.dtype == torch.float32
+        for i in need)
+    grads = [None] * len(params)
+    fields = (d.d_weight, d.d_bias, d.d_gamma, d.d_beta)           # params[i] is field i % 4 of layer i // 4
+    for i in range(len(params)):
+        fields[i % 4][i // 4] = None
+    for i in need:
+        if not inplace:
+            grads[i] = torch.empty_like(params[i])
+        fields[i % 4][i // 4] = (params[i].grad if inplace else grads[i]).data_ptr()
     d.accumulate = int(inplace)
     return grads
 
 
-class _MLPStackFn(torch.autograd.Function):
-    """x (P, K0) channels-last fp32; per layer: weight (checkpoint layout), bias|None, gamma|None, beta|None."""
+class _LiftGeom:
+    """Static geometry of a lifted stack: Y0[p] = Z[cloud(p) * rows_per_cloud + (ridx[p] | p % ridx_mod)] + s[p] . u, with c0
+    channels."""
+    __slots__ = ("P", "ridx_mod", "rows_per_cloud", "pos_per_cloud", "grp", "c0")
+
+    def __init__(self, P, ridx_mod, rows_per_cloud, pos_per_cloud, grp, c0):
+        self.P, self.ridx_mod, self.rows_per_cloud, self.pos_per_cloud, self.grp = P, ridx_mod, rows_per_cloud, pos_per_cloud, grp
+        self.c0 = c0
+
+
+class _StackFn(torch.autograd.Function):
+    """One stack; params = meta.params.  Plain (lift None): x (P, K0) channels-last fp32.  Lifted (lift a _LiftGeom, x None): the
+    first 1x1 convolution has been split (include/o3d_b200.h `o3d_lift_t`) into its feature part applied to the SOURCE points
+    (z = W0_f . rows, an ordinary one-layer stack) and gathered, plus up to four per-position scalars s with weight rows u:
+    z (rows, c0) | None, ridx (P,) int32 | None, s (P, 4) | None, u (4, c0) | None; layer 0 = (None, None, gamma0, beta0)."""
 
     @staticmethod
-    def forward(ctx, meta, x, *params):
-        P, K0 = x.shape
-        for t in params:
+    def forward(ctx, meta, lift, x, z, ridx, s, u, *params):
+        for t in (x, z, ridx, s, u) + params:
             if t is not None and not t.is_contiguous():
-                raise RuntimeError("fused MLP stack: parameters must be contiguous")
+                raise RuntimeError("fused MLP stack: tensors must be contiguous")
+        P, K0 = x.shape if lift is None else (lift.P, lift.c0)
+        dev = next(t for t in (x, z, s) if t is not None).device
         d = _describe(meta, P, K0, params)
+        lf = None
+        if lift is not None:
+            lf = _lib.LiftDesc()
+            lf.z, lf.ldz, lf.ridx, lf.ridx_mod = _ptr(z), lift.c0, _ptr(ridx), lift.ridx_mod
+            lf.rows_per_cloud, lf.pos_per_cloud, lf.grp = lift.rows_per_cloud, lift.pos_per_cloud, lift.grp
+            lf.s, lf.u = _ptr(s), _ptr(u)
+            d.lift = ctypes.pointer(lf)
         L = _lib.lib()
         need_grad = meta.grad_mode and any(ctx.needs_input_grad)   # (needs_input_grad mirrors requires_grad even under no_grad)
-        _attach_prepared(d, meta, params, P, K0, False, need_grad, x.device)
+        block = None            # inference with static weights: the prepared block, referenced here until the forward is enqueued
+        if not need_grad and not meta.training and runtime.static_weights():
+            lifted = False if lift is None else (z is not None, s is not None)
+            shape = (P, K0, meta.S, lifted, runtime.tc_level(), meta.xyz_first, meta.c0)
+            block = _static_cached("stack", shape, meta.params + meta.stats, lambda: _prepare_stack(d, dev))
+            d.prepared = block.data_ptr()
         nbytes = L.o3d_stack_workspace_bytes(ctypes.byref(d), 0)
         if nbytes < 0:
             raise RuntimeError("fused MLP stack: invalid stack description")
-        ws = torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=x.device)
-        rows = P // meta.S if meta.S > 0 else P
-        Nw, Cout = _r4(meta.cout[-1]), meta.cout[-1]
-        out = torch.empty(rows, Nw, dtype=torch.float32, device=x.device)
-        ops.LAUNCHES += 3 * meta.n + 1
-        _lib.check(L.o3d_stack_forward(ctypes.byref(d), x.data_ptr(), ws.data_ptr(), out.data_ptr(), int(need_grad),
-                                       _stream()), "o3d_stack_forward")
-        if need_grad:
-            ctx.meta, ctx.desc, ctx.params = meta, d, params
-            ctx.save_for_backward(x, ws, out)
-        return out if Nw == Cout else out[:, :Cout]
-
-    @staticmethod
-    def backward(ctx, dout):
-        meta, d, params = ctx.meta, ctx.desc, ctx.params
-        x, ws, out = ctx.saved_tensors
-        P, K0 = x.shape
-        Nw = out.shape[1]
-        if dout.shape[1] != Nw or not dout.is_contiguous():
-            dpad = torch.zeros(out.shape, dtype=torch.float32, device=x.device)
-            dpad[:, :dout.shape[1]] = dout
-            dout = dpad
-        grads = _param_grad_targets(ctx.needs_input_grad, params, d, meta, 2)
-        dx = torch.empty(P, K0, dtype=torch.float32, device=x.device) if ctx.needs_input_grad[1] else None
-        L = _lib.lib()
-        nbytes = L.o3d_stack_workspace_bytes(ctypes.byref(d), 1)
-        wb = torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=x.device)
-        ops.LAUNCHES += 5 * meta.n + 1
-        _lib.check(L.o3d_stack_backward(ctypes.byref(d), x.data_ptr(), ws.data_ptr(), wb.data_ptr(), out.data_ptr(),
-                                        dout.data_ptr(), _ptr(dx), _stream()), "o3d_stack_backward")
-        return (None, dx, *grads)
-
-
-# ---------------------------------------------------------------------------------------------- lifted first layer
-class _LiftGeom:
-    """Static geometry of a lifted stack: Y0[p] = Z[cloud(p) * rows_per_cloud + (ridx[p] | p % ridx_mod)] + s[p] . u."""
-    __slots__ = ("P", "ridx_mod", "rows_per_cloud", "pos_per_cloud", "grp")
-
-    def __init__(self, P, ridx_mod, rows_per_cloud, pos_per_cloud, grp):
-        self.P, self.ridx_mod, self.rows_per_cloud, self.pos_per_cloud, self.grp = P, ridx_mod, rows_per_cloud, pos_per_cloud, grp
-
-
-class _LiftedStackFn(torch.autograd.Function):
-    """A stack whose first 1x1 convolution has been split (include/o3d_b200.h `o3d_lift_t`): its feature part applied to the
-    SOURCE points (z = W0_f . rows, an ordinary one-layer stack) and gathered, plus up to four per-position scalars s with
-    weight rows u.  Inputs: z (rows, C0) | None, ridx (P,) int32 | None, s (P, 4) | None, u (4, C0) | None; params as in
-    _MLPStackFn with layer 0 = (None, None, gamma0, beta0)."""
-
-    @staticmethod
-    def forward(ctx, meta, geom, c0, z, ridx, s, u, *params):
-        P, C0 = geom.P, c0
-        for t in (z, ridx, s, u) + tuple(params):
-            if t is not None and not t.is_contiguous():
-                raise RuntimeError("lifted MLP stack: tensors must be contiguous")
-        dev = (z if z is not None else s).device
-        d = _describe(meta, P, C0, params)
-        lf = _lib.LiftDesc()
-        lf.z, lf.ldz, lf.ridx, lf.ridx_mod = _ptr(z), C0, _ptr(ridx), geom.ridx_mod
-        lf.rows_per_cloud, lf.pos_per_cloud, lf.grp = geom.rows_per_cloud, geom.pos_per_cloud, geom.grp
-        lf.s, lf.u = _ptr(s), _ptr(u)
-        d.lift = ctypes.pointer(lf)
-        L = _lib.lib()
-        need_grad = meta.grad_mode and any(ctx.needs_input_grad)   # (needs_input_grad mirrors requires_grad even under no_grad)
-        _attach_prepared(d, meta, params, P, C0, (z is not None, s is not None), need_grad, dev)
-        nbytes = L.o3d_stack_workspace_bytes(ctypes.byref(d), 0)
-        if nbytes < 0:
-            raise RuntimeError("lifted MLP stack: invalid stack description")
         ws = torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=dev)
         rows = P // meta.S if meta.S > 0 else P
         Nw, Cout = _r4(meta.cout[-1]), meta.cout[-1]
         out = torch.empty(rows, Nw, dtype=torch.float32, device=dev)
         ops.LAUNCHES += 3 * meta.n + 1
-        _lib.check(L.o3d_stack_forward(ctypes.byref(d), None, ws.data_ptr(), out.data_ptr(), int(need_grad), _stream()),
-                   "o3d_stack_forward (lifted)")
+        _lib.check(L.o3d_stack_forward(ctypes.byref(d), _ptr(x), ws.data_ptr(), out.data_ptr(), int(need_grad), _stream()),
+                   "o3d_stack_forward")
         if need_grad:
-            ctx.meta, ctx.geom, ctx.desc, ctx.lf, ctx.params = meta, geom, d, lf, params
-            ctx.save_for_backward(z, ridx, s, u, ws, out)
+            ctx.meta, ctx.desc, ctx.lf = meta, d, lf     # the backward writes d_z / d_s / d_u into lf
+            ctx.save_for_backward(x, z, ridx, s, u, ws, out)
         return out if Nw == Cout else out[:, :Cout]
 
     @staticmethod
     def backward(ctx, dout):
-        meta, geom, d, lf, params = ctx.meta, ctx.geom, ctx.desc, ctx.lf, ctx.params
-        z, ridx, s, u, ws, out = ctx.saved_tensors
-        Nw = out.shape[1]
-        if dout.shape[1] != Nw or not dout.is_contiguous():
+        meta, d, lf = ctx.meta, ctx.desc, ctx.lf
+        x, z, ridx, s, u, ws, out = ctx.saved_tensors
+        if dout.shape[1] != out.shape[1] or not dout.is_contiguous():
             dpad = torch.zeros(out.shape, dtype=torch.float32, device=out.device)
             dpad[:, :dout.shape[1]] = dout
             dout = dpad
-        grads = _param_grad_targets(ctx.needs_input_grad, params, d, meta, 7)
-        need = ctx.needs_input_grad
-        dz = torch.zeros_like(z) if (z is not None and need[3]) else None
-        ds = torch.zeros_like(s) if (s is not None and need[5]) else None
-        du = torch.zeros_like(u) if (u is not None and need[6]) else None
-        lf.d_z, lf.d_s, lf.d_u = _ptr(dz), _ptr(ds), _ptr(du)
+        need = ctx.needs_input_grad                     # False for inputs that are None
+        grads = _param_grad_targets(need[7:], d, meta)
+        dx = torch.empty_like(x) if need[2] else None
+        dz, ds, du = (torch.zeros_like(t) if need[i] else None for i, t in ((3, z), (5, s), (6, u)))
+        if lf is not None:
+            lf.d_z, lf.d_s, lf.d_u = _ptr(dz), _ptr(ds), _ptr(du)
         L = _lib.lib()
         nbytes = L.o3d_stack_workspace_bytes(ctypes.byref(d), 1)
         wb = torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=out.device)
         ops.LAUNCHES += 5 * meta.n + 1
-        _lib.check(L.o3d_stack_backward(ctypes.byref(d), None, ws.data_ptr(), wb.data_ptr(), out.data_ptr(), dout.data_ptr(),
-                                        None, _stream()), "o3d_stack_backward (lifted)")
-        return (None, None, None, dz, None, ds, du, *grads)
+        _lib.check(L.o3d_stack_backward(ctypes.byref(d), _ptr(x), ws.data_ptr(), wb.data_ptr(), out.data_ptr(), dout.data_ptr(),
+                                        _ptr(dx), _stream()), "o3d_stack_backward")
+        return (None, None, dx, dz, None, ds, du, *grads)
 
 
-def lifted_stack(specs, geom, c0, z=None, ridx=None, s=None, u=None, S=0, training=True):
+def lifted_stack(specs, geom, z=None, ridx=None, s=None, u=None, S=0, training=True):
     """specs[0] is the lifted layer: its conv has ALREADY been applied (z, s.u); only its BatchNorm / ReLU remain."""
-    first = _LayerSpec(None, None, specs[0].bn, specs[0].relu, lift_c0=c0)
-    meta = _Meta([first] + list(specs[1:]), S, training)
-    params = [None, None, first.bn.weight if first.bn is not None else None, first.bn.bias if first.bn is not None else None]
-    for sp in specs[1:]:
-        params += [sp.weight, sp.bias, sp.bn.weight if sp.bn is not None else None, sp.bn.bias if sp.bn is not None else None]
-    return _LiftedStackFn.apply(meta, geom, c0, z, ridx, s, u, *params)
+    meta = _Meta([_LayerSpec(None, None, specs[0].bn, specs[0].relu, lift_c0=geom.c0)] + list(specs[1:]), S, training)
+    return _StackFn.apply(meta, geom, None, z, ridx, s, u, *meta.params)
 
 
 def _pow2_divisor(n, cap=64):
@@ -351,10 +298,7 @@ def mlp_stack(x2d, specs, S=0, training=True, xyz_first=False, c0=0, dx_cols=0):
         raise RuntimeError("open3dsot_b200.fused: CUDA tensors required (there is no CPU path)")
     assert x2d.dim() == 2 and x2d.is_contiguous() and x2d.dtype == torch.float32 and x2d.shape[1] % 4 == 0
     meta = _Meta(specs, S, training, xyz_first, c0, dx_cols)
-    params = []
-    for s in specs:
-        params += [s.weight, s.bias, s.bn.weight if s.bn is not None else None, s.bn.bias if s.bn is not None else None]
-    return _MLPStackFn.apply(meta, x2d, *params)
+    return _StackFn.apply(meta, None, x2d, None, None, None, None, *meta.params)
 
 
 # ---------------------------------------------------------------------------------------------- layout helpers
@@ -383,38 +327,20 @@ def _sa_fused_ok(specs, S, npoint, N, C):
     for s in specs:
         if s.weight is None or s.weight.shape[0] > 256:
             return False
-        if s.bn is not None and (not s.bn.track_running_stats or s.bn.running_mean is None):
+        if s.bn is not None and not _tracks_stats(s.bn):
             return False
     return specs[0].weight.numel() // specs[0].weight.shape[0] == C + 3
 
 
-def _sa_fused_block(d, params, bns, device):
-    """the layer's parameter block (pre-tiled weight images, folded BatchNorm): built per call, or — static weights — once,
-    stored on the first weight and keyed by every parameter's / running statistic's identity and version"""
+def _sa_fused_prepare(d, device):
+    """the layer's parameter block: pre-tiled weight images, folded BatchNorm"""
     L = _lib.lib()
-
-    def make():
-        nbytes = L.o3d_sa_fused_prepared_bytes(ctypes.byref(d))
-        if nbytes < 0:
-            raise RuntimeError("fused SA layer: SharedMLP outside the kernel's range")
-        block = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
-        _lib.check(L.o3d_sa_fused_prepare(ctypes.byref(d), block.data_ptr(), _stream()), "o3d_sa_fused_prepare")
-        return block
-
-    if not runtime.static_weights():
-        return make()
-    stats = [t for bn in bns if bn is not None for t in (bn.running_mean, bn.running_var)]
-    owner = params[0]
-    cache = owner.__dict__.setdefault("_o3d_sa_fused", {})
-    key = tuple(id(t) for t in params) + tuple(id(t) for t in stats)
-    ver = _versions(params) + _versions(stats)
-    hit = cache.get(key)
-    if hit is None or hit[0] != ver:
-        if not _cacheable():
-            return make()                                 # during graph capture: built privately, as part of the graph
-        hit = cache[key] = (ver, make(), params, stats)
-        _publish()
-    return hit[1]
+    nbytes = L.o3d_sa_fused_prepared_bytes(ctypes.byref(d))
+    if nbytes < 0:
+        raise RuntimeError("fused SA layer: SharedMLP outside the kernel's range")
+    block = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
+    _lib.check(L.o3d_sa_fused_prepare(ctypes.byref(d), block.data_ptr(), _stream()), "o3d_sa_fused_prepare")
+    return block
 
 
 def _sa_fused_forward(specs, xyz, new_xyz, feat_cl, C, radius, S, normalize):
@@ -422,11 +348,11 @@ def _sa_fused_forward(specs, xyz, new_xyz, feat_cl, C, radius, S, normalize):
     B, N, _ = xyz.shape
     npoint = new_xyz.shape[1]
     meta = _Meta(specs, S, False, xyz_first=True, c0=C)
-    params = []
-    for s in specs:
-        params += [s.weight, s.bias, s.bn.weight if s.bn is not None else None, s.bn.bias if s.bn is not None else None]
-    d = _describe(meta, B * npoint * S, _r4(C) + 4, params)
-    block = _sa_fused_block(d, params, meta.bns, xyz.device)
+    d = _describe(meta, B * npoint * S, _r4(C) + 4, meta.params)
+    if runtime.static_weights():
+        block = _static_cached("sa_fused", None, meta.params + meta.stats, lambda: _sa_fused_prepare(d, xyz.device))
+    else:
+        block = _sa_fused_prepare(d, xyz.device)
     ldo = _r4(meta.cout[-1])
     out = torch.empty(B, npoint, ldo, dtype=torch.float32, device=xyz.device)
     _lib.check(_lib.lib().o3d_sa_fused_forward(ctypes.byref(d), block.data_ptr(), xyz.data_ptr(), new_xyz.data_ptr(), _ptr(feat_cl),
@@ -496,8 +422,8 @@ def sa_forward(sa, xyz, features, sample_idxs):
             if feat_cl is not None:
                 Wf = _derived(W0, "w_feat", lambda: W2[:, 3:].contiguous())
                 z = mlp_stack(feat_cl.view(B * N, Cp), [_LayerSpec(Wf, specs[0].bias, None, False)], 0, sa.training)
-            geom = _LiftGeom(B * npoint * S, 0, N, npoint * S, S)
-            pooled = lifted_stack(specs, geom, C0, z=z, ridx=idx.view(-1) if z is not None else None,
+            geom = _LiftGeom(B * npoint * S, 0, N, npoint * S, S, C0)
+            pooled = lifted_stack(specs, geom, z=z, ridx=idx.view(-1) if z is not None else None,
                                   s=rel.view(B * npoint * S, 4), u=u, S=S, training=sa.training)
         else:
             grouped, _idx = pointnet2_utils.query_and_group_cl(xyz, new_xyz, feat_cl, grouper.radius, S,
@@ -602,8 +528,8 @@ def boxaware_xcorr_forward(xc, template_feature, search_feature, template_xyz, t
         # lifted: the first conv runs on the M template rows; the (B, 268, N, k) grouped tensor is never built (xcorr.py:89-98)
         tm = tmpl.contiguous()
         z = mlp_stack(tm.view(B * M, tm.shape[2]), [_LayerSpec(specs[0].weight, specs[0].bias, None, False)], 0, xc.training)
-        geom = _LiftGeom(B * N * k, 0, M, N * k, _pow2_divisor(N * k))
-        pooled = lifted_stack(specs, geom, z.shape[1], z=z, ridx=topk.view(-1), S=k, training=xc.training)
+        geom = _LiftGeom(B * N * k, 0, M, N * k, _pow2_divisor(N * k), z.shape[1])
+        pooled = lifted_stack(specs, geom, z=z, ridx=topk.view(-1), S=k, training=xc.training)
     else:
         rows = _GroupRowsCL.apply(tmpl.contiguous(), topk.view(B, N * k))                 # (B, N*k, Cp)
         pooled = mlp_stack(rows.view(B * N * k, rows.shape[2]), specs, k, xc.training)
@@ -633,8 +559,8 @@ def p2b_xcorr_forward(xc, template_feature, search_feature, template_xyz):
             rows = F.pad(rows, (0, _r4(C) - C))
         Wr = _derived(specs[0].weight, "w_rest", lambda: W0[:, 1:].contiguous())
         z = mlp_stack(rows.reshape(B * n1, rows.shape[2]), [_LayerSpec(Wr, specs[0].bias, None, False)], 0, xc.training)
-        geom = _LiftGeom(B * n2 * n1, n1, n1, n2 * n1, n1)
-        pooled = lifted_stack(specs, geom, z.shape[1], z=z, s=F.pad(sim_t.reshape(-1, 1), (0, 3)),
+        geom = _LiftGeom(B * n2 * n1, n1, n1, n2 * n1, n1, z.shape[1])
+        pooled = lifted_stack(specs, geom, z=z, s=F.pad(sim_t.reshape(-1, 1), (0, 3)),
                               u=_derived(specs[0].weight, "u_sim", lambda: F.pad(W0[:, :1].t(), (0, 0, 0, 3)).contiguous()), S=n1,
                               training=xc.training)
     else:
@@ -719,15 +645,19 @@ def segpointnet_forward(net, x):
 _SIDE_STREAMS = {}
 
 
+def _side_stream(device):
+    side = _SIDE_STREAMS.get(device.index)
+    if side is None:
+        side = _SIDE_STREAMS[device.index] = torch.cuda.Stream(device=device)
+    return side
+
+
 def fps_ahead(points, npoint):
     """Launch furthest-point sampling of `points` (B,N,3+) on a side stream and return (idx, join).  FPS is a serial chain
     of npoint steps that occupies one CTA per cloud (48 of 132 SMs at config 2); started before the template branch it
     runs underneath that branch's GEMMs.  `join()` makes the current stream wait for it (graph-capture safe fork/join)."""
     cur = torch.cuda.current_stream()
-    dev = points.device.index
-    side = _SIDE_STREAMS.get(dev)
-    if side is None:
-        side = _SIDE_STREAMS[dev] = torch.cuda.Stream(device=points.device)
+    side = _side_stream(points.device)
     xyz = points[..., 0:3].contiguous()
     side.wait_stream(cur)
     with torch.cuda.stream(side):
@@ -756,10 +686,7 @@ def run_ahead(fn):
     cross-correlation — run side by side; inside a captured CUDA graph the fork / join becomes two parallel branches."""
     assert not torch.is_grad_enabled(), "run_ahead is for inference (autograd does not see the stream switch)"
     cur = torch.cuda.current_stream()
-    dev = cur.device
-    side = _SIDE_STREAMS.get(dev.index)
-    if side is None:
-        side = _SIDE_STREAMS[dev.index] = torch.cuda.Stream(device=dev)
+    side = _side_stream(cur.device)
     side.wait_stream(cur)
     with torch.cuda.stream(side):
         result = fn()

@@ -62,8 +62,10 @@ def static_weights() -> bool:
 def static_weights_scope():
     """`with runtime.static_weights_scope():` — inference code whose weights do not change while it runs.
 
-    The cached blocks are keyed by the parameters' tensor versions, and the engine's fused Adam updates parameters in place
-    without bumping them: a scope must not span training steps, or the forward passes after a step run on the old weights."""
+    The cached blocks are keyed by the identity and tensor version of every tensor they are computed from: the parameters and
+    the running mean and variance of every BatchNorm that tracks them, so `load_state_dict` and other in-place updates rebuild
+    them.  The engine's fused Adam updates parameters in place without bumping them: a scope must not span training steps, or
+    the forward passes after a step run on the old weights."""
     global _STATIC_WEIGHTS
     old = _STATIC_WEIGHTS
     _STATIC_WEIGHTS = True

@@ -117,10 +117,7 @@ def test_fused_sa_layer_index_output_is_the_ball_query():
     sa = _module([C, 32, 64], radius, S, seed=5)
     specs = fused.parse_stack(sa.mlps[0])
     meta = fused._Meta(specs, S, False, xyz_first=True, c0=C)
-    params = []
-    for s in specs:
-        params += [s.weight, s.bias, s.bn.weight, s.bn.bias]
-    d = fused._describe(meta, B * npoint * S, C + 4, params)
+    d = fused._describe(meta, B * npoint * S, C + 4, meta.params)
     L = _lib.lib()
     block = torch.empty(int(L.o3d_sa_fused_prepared_bytes(ctypes.byref(d))), dtype=torch.uint8, device="cuda")
     _lib.check(L.o3d_sa_fused_prepare(ctypes.byref(d), block.data_ptr(), None), "prepare")
