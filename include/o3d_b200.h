@@ -340,6 +340,15 @@ int o3d_adam_step(float* param, const float* grad, float* exp_avg, float* exp_av
 int o3d_crop_box_frame(const float* scans, const long long* count, const long long* frame, const float* center,
                        const float* rot, const float* half, int B, int N, float* local, unsigned char* keep, void* stream);
 
+/* The crop of o3d_crop_box_frame appended to a per-slot history (the template of shape_aggregation 'all'): for every slot b
+ * with frame[b] >= 0, the points i < count[frame[b]] of scan frame[b] strictly inside half[b] in the frame of box b (the same
+ * local coordinates as o3d_crop_box_frame, bit for bit) are written in scan order to hist[b, hist_count[b] + j] with
+ * hist_keep set there, for positions < H only; hist_count[b] then grows by the number kept, including those that did not fit.
+ * frame[b] < 0 leaves slot b untouched.  hist [B,H,3], hist_keep [B,H] bytes, hist_count [B] int64; count nullable. */
+int o3d_crop_append(const float* scans, const long long* count, const long long* frame, const float* center, const float* rot,
+                    const float* half, int B, int N, int H, float* hist, unsigned char* hist_keep, long long* hist_count,
+                    void* stream);
+
 /* Fixed-shape resampling of a masked candidate set (datasets/points_utils.py:24-40 regularize_pc, device form): per cloud,
  * n = #keep;  n >= size: the `size` kept candidates with the smallest keys u_perm, in ascending key order (a uniform draw
  * without replacement);  2 < n < size: draw i = the floor(u_pick[i] * n)-th kept candidate;  n <= 2: zeros.

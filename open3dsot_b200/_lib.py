@@ -58,6 +58,7 @@ PROTOTYPES = {
                          ctypes.c_longlong, _p],
     "o3d_adam_step": [_p, _p, _p, _p, ctypes.c_longlong, _p, _f, _f, _f, _f, _p],
     "o3d_crop_box_frame": [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p],
+    "o3d_crop_append": [_p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p],
     "o3d_resample": [_p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p],
     "o3d_lift_stats": [_p, _i, _i, _p, _p, _p, _p, _p],
     "o3d_lift_scatter": [_p, _i, _i, _p, _p, _p, _i, _p, _p, _p, _p],

@@ -128,6 +128,37 @@ __device__ __forceinline__ void o3d_prefetch_l2(const void* gptr, size_t bytes) 
         n -= c;
     }
 }
+// Exclusive block scan of one value per thread in a block of exactly 1024 threads (32 warps); `total` receives the
+// block sum, s_warp is 32 words of shared memory.  Two barriers.
+__device__ __forceinline__ uint32_t o3d_block_exscan1024(uint32_t v, uint32_t* s_warp, uint32_t& total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, inc, o);
+        if (lane >= o) inc += t;
+    }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    uint32_t w = s_warp[lane];
+    uint32_t winc = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, winc, o);
+        if (lane >= o) winc += t;
+    }
+    total = __shfl_sync(0xFFFFFFFFu, winc, 31);
+    const uint32_t wbase = __shfl_sync(0xFFFFFFFFu, winc - w, warp);
+    __syncthreads();                      // s_warp may be rewritten by the next call
+    return wbase + inc - v;
+}
+// Points in the frame of a box: the row vector (p - c) times R, whose columns are the box axes.  The one formula of every
+// box-frame crop kernel, so that they produce bit-identical local coordinates.
+__device__ __forceinline__ void o3d_to_box_frame(float dx, float dy, float dz, const float (&R)[9], float& x, float& y, float& z) {
+    x = fmaf(dz, R[6], fmaf(dy, R[3], dx * R[0]));
+    y = fmaf(dz, R[7], fmaf(dy, R[4], dx * R[1]));
+    z = fmaf(dz, R[8], fmaf(dy, R[5], dx * R[2]));
+}
 __device__ __forceinline__ uint32_t o3d_lanemask_lt() {
     uint32_t m;
     asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));

@@ -21,30 +21,7 @@ namespace {
 
 constexpr int RS_THREADS = 1024;
 constexpr int RS_MAX_SIZE = 2048;
-
-// exclusive block scan of one value per thread (RS_THREADS threads); `total` receives the block sum.  Two barriers.
-__device__ __forceinline__ uint32_t block_exscan(uint32_t v, uint32_t* s_warp, uint32_t& total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, inc, o);
-        if (lane >= o) inc += t;
-    }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    uint32_t w = s_warp[lane];            // RS_THREADS / 32 == 32 warps
-    uint32_t winc = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, winc, o);
-        if (lane >= o) winc += t;
-    }
-    total = __shfl_sync(0xFFFFFFFFu, winc, 31);
-    const uint32_t wbase = __shfl_sync(0xFFFFFFFFu, winc - w, warp);
-    __syncthreads();                      // s_warp may be rewritten by the next call
-    return wbase + inc - v;
-}
+static_assert(RS_THREADS == 1024, "o3d_block_exscan1024 scans exactly 32 warps");
 
 __global__ void __launch_bounds__(RS_THREADS)
     resample_kernel(const float* __restrict__ points, const uint8_t* __restrict__ keep, const float* __restrict__ u_perm,
@@ -85,7 +62,7 @@ __global__ void __launch_bounds__(RS_THREADS)
     uint32_t cnt = 0;
     for (int i = beg; i < end; i += 4) cnt += __popc(flags4(i));
     uint32_t n;
-    uint32_t pos = block_exscan(cnt, s_warp, n);
+    uint32_t pos = o3d_block_exscan1024(cnt, s_warp, n);
     for (int i = beg; i < end; i += 4) {
         const uint32_t f = flags4(i);
 #pragma unroll
@@ -131,7 +108,7 @@ __global__ void __launch_bounds__(RS_THREADS)
             __syncthreads();
             const uint32_t h0 = s_hist[2 * tid], h1 = s_hist[2 * tid + 1];
             uint32_t total;
-            const uint32_t ex = block_exscan(h0 + h1, s_warp, total);
+            const uint32_t ex = o3d_block_exscan1024(h0 + h1, s_warp, total);
             if (ex < krem && krem <= ex + h0) {
                 s_digit = 2 * tid; s_krem = krem - ex; s_eq = h0;
             } else if (ex + h0 < krem && krem <= ex + h0 + h1) {
@@ -178,7 +155,7 @@ __global__ void __launch_bounds__(RS_THREADS)
                     hit = __float_as_uint(U[idx]) == prefix;
                 }
                 uint32_t total;
-                const uint32_t r = taken + block_exscan(hit, s_warp, total);
+                const uint32_t r = taken + o3d_block_exscan1024(hit, s_warp, total);
                 if (hit && r < krem) s_sel[n_less + r] = ((unsigned long long)prefix << 32) | idx;
                 taken += total;
             }

@@ -250,6 +250,24 @@ def crop_box_frame(scans, center, rot, half, frame=None, count=None):
     return local, keep
 
 
+def crop_append(scans, center, rot, half, frame, count, hist, hist_keep, hist_count):
+    """o3d_crop_box_frame's crop appended in place to per-slot histories (csrc/geometry.cu): scans (F, N, 3) fp32 CUDA; center
+    (B, 3), rot (B, 3, 3), half (B, 3); frame (B,) int64, < 0 = slot untouched; count (F,) int64 or None; hist (B, H, 3) fp32,
+    hist_keep (B, H) bool, hist_count (B,) int64.  Kept points go, in scan order, to positions hist_count[b] + j < H, and
+    hist_count[b] grows by the full number kept."""
+    _chk_f(scans, "scans"); _chk_f(hist, "hist")
+    F, N, _ = scans.shape
+    B, H, _ = hist.shape
+    for t, name in ((frame, "frame"), (hist_count, "hist_count")) + (() if count is None else ((count, "count"),)):
+        if not t.is_cuda or t.dtype != torch.int64 or not t.is_contiguous():
+            raise RuntimeError(f"{name} must be a contiguous int64 CUDA tensor")
+    assert frame.shape == (B,) and hist_count.shape == (B,) and hist_keep.shape == (B, H)
+    assert hist_keep.dtype == torch.bool and hist_keep.is_contiguous()
+    center, rot, half = (t.contiguous().float() for t in (center, rot, half))
+    _call("o3d_crop_append", scans.data_ptr(), None if count is None else count.data_ptr(), frame.data_ptr(), center.data_ptr(),
+          rot.data_ptr(), half.data_ptr(), B, N, H, hist.data_ptr(), hist_keep.data_ptr(), hist_count.data_ptr(), _stream())
+
+
 # ------------------------------------------------------------------ split evaluation, K tracklets in flight (tracking/batched_tracker.py)
 def keyed_uniform(tracklet, frame, seed, stream, n, out=None):
     """Counter-based uniform [0, 1) draws (csrc/track_eval.cu): tracklet (K,) / frame (K,) int64 CUDA -> out (K, n) fp32, row k a pure

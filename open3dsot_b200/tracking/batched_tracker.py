@@ -3,15 +3,19 @@
 `DeviceTracker` runs one B=1 frame per replay, which leaves most of the GPU idle (FPS and resampling run one CTA per
 cloud).  Here a chunk of tracklets sits on the device as a `DeviceTracklets` pool (padded scans, per-frame first /
 previous indices, fp32 boxes) plus fp64 copies of the ground-truth boxes, and K slots each track one tracklet of it:
-  * one fixed-shape step advances every slot by one frame — search crop of the current frame and template crop of the
-    previous one in the slot's box frame, template = first-frame crop + previous crop, resampling, BoxCloud, the network
-    in eval mode, best proposal, box update, and the overlap / centre distance of the new box against the ground truth
-    (csrc/track_eval.cu) written into a record indexed by the pool frame — and is captured once in a CUDA graph;
+  * one fixed-shape step advances every slot by one frame — search crop of the current frame in the reference box's frame
+    (the slot's result box, or the pool's ground truth of the previous / current frame for reference_BB 'previous_gt' /
+    'current_gt'), template crop of the previous frame in the result box's frame, template = first-frame crop + previous crop
+    (or, for shape_aggregation 'all', the slot's history: the crops of every past frame, appended once per step by
+    csrc/geometry.cu's o3d_crop_append), resampling, BoxCloud, the network in eval mode, best proposal, box update of the
+    reference box, and the overlap / centre distance of the new box against the ground truth (csrc/track_eval.cu) written
+    into a record indexed by the pool frame — and is captured once in a CUDA graph;
   * the random draws of a slot (resampling, limit_box) are keyed by (seed, tracklet id, frame within the tracklet), so a
     tracklet's result does not depend on the slot it runs in or on K;
   * between replays, a slot whose tracklet has ended is re-filled with the next one (`DeviceTracker.reset`'s computation for
     that tracklet, issued without a host sync); the host plans that schedule from the tracklet lengths, longest first;
-  * the host synchronises once per chunk, to copy the records back.
+  * the host synchronises once per chunk, to copy the records back (and, in 'all' mode, the slots' peak history counts: a
+    chunk whose history overflowed its capacity runs again with the capacity raised, so nothing is truncated).
 Idle slots run on a valid dummy frame and record nothing."""
 import heapq
 
@@ -21,6 +25,7 @@ import torch
 from .. import ops, runtime
 from ..datasets.device_sampler import DeviceTracklets
 from . import boxes as bx
+from .device_tracker import HISTORY_POINTS, is_motion, tracking_modes
 from .sampling import resample_batched
 
 # keyed-draw streams of one frame, in DeviceTracker's buffer layout: u_s (perm, pick), u_t (perm, pick), limit_box's two draws
@@ -56,14 +61,23 @@ def pool_frame_bytes(max_points):
     return 12 * int(max_points) + 512
 
 
-def plan_chunks(lengths, frame_bytes, max_resident_bytes):
-    """Consecutive groups of tracklets (input order) whose frames fit `max_resident_bytes`; a tracklet is never split."""
+def history_bytes(slots, capacity):
+    """Device bytes of the 'all' template history of `slots` slots: points (12 B) and keep mask (1 B) per position, plus the
+    template's permutation draw (4 B) and the resampling's compaction scratch (4 B) over the same positions."""
+    return int(slots) * int(capacity) * (12 + 1 + 4 + 4)
+
+
+def plan_chunks(lengths, frame_bytes, max_resident_bytes, fixed_bytes=0):
+    """Consecutive groups of tracklets (input order) whose frames fit `max_resident_bytes` beside `fixed_bytes` of per-chunk
+    state (the 'all' history); a tracklet is never split."""
+    budget = max_resident_bytes - fixed_bytes
     chunks, cur, used = [], [], 0
     for j, n in enumerate(lengths):
         need = int(n) * frame_bytes
-        if need > max_resident_bytes:
-            raise ValueError(f"tracklet {j} needs {need} bytes on the device, more than max_resident_bytes={max_resident_bytes}")
-        if cur and used + need > max_resident_bytes:
+        if need > budget:
+            raise ValueError(f"tracklet {j} needs {need} bytes on the device beside {fixed_bytes} bytes of slot state, more than "
+                             f"max_resident_bytes={max_resident_bytes}")
+        if cur and used + need > budget:
             chunks.append(cur)
             cur, used = [], 0
         cur.append(j)
@@ -75,18 +89,18 @@ def plan_chunks(lengths, frame_bytes, max_resident_bytes):
 
 class BatchedDeviceTracker:
     """K slots tracking the tracklets of one chunk.  `tracklets`: lists of {"pc", "3d_bbox"}; `ids`: their tracklet ids
-    (the key of their random draws; default 0..n-1); `max_points`: padded scan size (default: the largest scan)."""
+    (the key of their random draws; default 0..n-1); `max_points`: padded scan size (default: the largest scan);
+    `history`: starting capacity (points per slot) of the 'all' template history, raised by `run()` when a slot needs more."""
 
-    def __init__(self, model, tracklets, slots, seed=0, ids=None, max_points=None, use_graph=True):
+    def __init__(self, model, tracklets, slots, seed=0, ids=None, max_points=None, use_graph=True, history=HISTORY_POINTS):
         self.model = model.eval()
         self.cfg = cfg = model.config
         self.dev = dev = next(model.parameters()).device
-        if cfg.get("shape_aggregation", "firstandprevious").upper() == "ALL":
-            raise NotImplementedError("shape_aggregation 'all' needs every past frame of every slot on the device")
         self.use_graph = bool(use_graph) and dev.type == "cuda"
         self.seed = int(seed)
         self.needs_bc = hasattr(model, "mlp_bc")
-        self.motion = "point_sample_size" in cfg and not hasattr(model, "backbone")
+        self.motion = is_motion(model)
+        self.mode, self.ref_mode = tracking_modes(model)
         lengths = [len(t) for t in tracklets]
         self.ids = list(range(len(tracklets))) if ids is None else [int(i) for i in ids]
         self.plan = plan_schedule(lengths, slots)
@@ -106,8 +120,9 @@ class BatchedDeviceTracker:
         self.box_c = torch.zeros(K, 3, **f)
         self.box_s = torch.ones(K, 3, **f)
         self.box_r = torch.eye(3, **f).repeat(K, 1, 1)
-        self.first_local = torch.zeros(K, N, 3, **f)
-        self.first_keep = torch.zeros(K, N, dtype=torch.bool, device=dev)
+        if self.mode != "all":
+            self.first_local = torch.zeros(K, N, 3, **f)
+            self.first_keep = torch.zeros(K, N, dtype=torch.bool, device=dev)
         self.first_flag = torch.zeros(K, **f)
         self.frame = torch.full((K,), -1, dtype=torch.int64, device=dev)       # pool frame being tracked, -1 = idle
         self.tracklet = torch.zeros(K, dtype=torch.int64, device=dev)
@@ -122,6 +137,19 @@ class BatchedDeviceTracker:
         self.rec_r = torch.zeros(F + 1, 3, 3, **f)
         self.overlap = torch.zeros(F, **f64)
         self.distance = torch.zeros(F, **f64)
+        if self.mode == "all":
+            self.hist_count = torch.zeros(K, dtype=torch.int64, device=dev)
+            self.hist_peak = torch.zeros(K, dtype=torch.int64, device=dev)  # largest count of each slot over the chunk
+            self._alloc_history(int(history))
+        self.graph = None
+
+    def _alloc_history(self, H):
+        """History buffers for H points per slot (contents undefined until admission); drops the captured graph."""
+        K = self.K
+        self.hist = torch.zeros(K, H, 3, device=self.dev)
+        self.hist_keep = torch.zeros(K, H, dtype=torch.bool, device=self.dev)
+        self.u_t = (torch.zeros(K, H, device=self.dev), self.u_t[1])          # the template draw is over the history
+        self.H = H
         self.graph = None
 
     # ------------------------------------------------------------------ one step for all slots, fixed shapes
@@ -151,23 +179,28 @@ class BatchedDeviceTracker:
     def _canon(self, box):
         return bx.Box(torch.zeros_like(box.center), box.wlh, torch.eye(3, device=self.dev).expand_as(box.rot))
 
-    def _inputs(self, f, box):
-        """DeviceTracker._inputs with a slot dimension."""
+    def _inputs(self, f, box, ref, active):
+        """DeviceTracker._inputs with a slot dimension: `box` the slots' result boxes, `ref` their reference boxes."""
         if self.motion:
             return self._inputs_motion(f, box)
-        cfg, P = self.cfg, self.pool
-        s_local, s_keep = bx.crop_in_box_frame(P.scans, box, cfg.search_bb_scale, cfg.search_bb_offset, f, P.count)
+        cfg, P, mode = self.cfg, self.pool, self.mode
+        s_local, s_keep = bx.crop_in_box_frame(P.scans, ref, cfg.search_bb_scale, cfg.search_bb_offset, f, P.count)
         search, _, _ = resample_batched(s_local, s_keep, cfg.search_size, *self.u_s)
-        mode = cfg.shape_aggregation.upper()
-        p_local, p_keep = bx.crop_in_box_frame(P.scans, box, cfg.model_bb_scale, cfg.model_bb_offset, P.prev[f], P.count)
-        if "FIRSTANDPREVIOUS" in mode:
-            cand, keep = torch.cat([self.first_local, p_local], 1), torch.cat([self.first_keep, p_keep], 1)
-        elif "FIRST" in mode:
+        if mode == "all":
+            # append the previous frame's crop in the current result box; the history then holds frames 0 .. t-1
+            prev = torch.where(active, P.prev[f], torch.full_like(f, -1))
+            bx.crop_append(P.scans, box, cfg.model_bb_scale, cfg.model_bb_offset, prev, P.count, self.hist, self.hist_keep,
+                           self.hist_count)
+            torch.maximum(self.hist_peak, self.hist_count, out=self.hist_peak)
+            cand, keep = self.hist, self.hist_keep
+        elif mode == "first":
             cand, keep = self.first_local, self.first_keep
-        elif "PREVIOUS" in mode:
-            cand, keep = p_local, p_keep
         else:
-            raise NotImplementedError(f"shape_aggregation '{cfg.shape_aggregation}'")
+            p_local, p_keep = bx.crop_in_box_frame(P.scans, box, cfg.model_bb_scale, cfg.model_bb_offset, P.prev[f], P.count)
+            if mode == "firstandprevious":
+                cand, keep = torch.cat([self.first_local, p_local], 1), torch.cat([self.first_keep, p_keep], 1)
+            else:
+                cand, keep = p_local, p_keep
         template, _, _ = resample_batched(cand, keep, cfg.template_size, self.u_t[0][:, : cand.shape[1]], self.u_t[1])
         data = {"template_points": template, "search_points": search}
         if self.needs_bc:
@@ -181,13 +214,19 @@ class BatchedDeviceTracker:
             f = self.frame.clamp(min=0)                                        # idle slots track pool frame 0, unrecorded
             self._draw(f - P.first[f])
             box = bx.Box(self.box_c, self.box_s, self.box_r)
-            est = self.model(self._inputs(f, box))["estimation_boxes"]         # (K, num_proposal, 5) or (K, 4)
+            if self.ref_mode == "previous_result":
+                ref = box
+            else:
+                ref = P.box(P.prev[f] if self.ref_mode == "previous_gt" else f)
+            est = self.model(self._inputs(f, box, ref, active))["estimation_boxes"]   # (K, num_proposal, 5) or (K, 4)
             if est.dim() == 3:
                 best = est[:, :, 4].argmax(1)
                 est = est.gather(1, best[:, None, None].expand(-1, 1, est.shape[-1]))[:, 0, :4]
-            new = bx.offset_box(box, est, degrees=cfg.degrees, use_z=cfg.use_z, limit_box=cfg.limit_box, rand=self.u_lim * 2 - 1)
+            new = bx.offset_box(ref, est, degrees=cfg.degrees, use_z=cfg.use_z, limit_box=cfg.limit_box, rand=self.u_lim * 2 - 1)
             self.box_c.copy_(new.center)
             self.box_r.copy_(new.rot)
+            if ref is not box:
+                self.box_s.copy_(new.wlh)                                      # the result takes the reference box's size
             row = f.masked_fill(~active, self.F)
             self.rec_c.index_copy_(0, row, self.box_c)
             self.rec_r.index_copy_(0, row, self.box_r)
@@ -216,7 +255,10 @@ class BatchedDeviceTracker:
         self.box_c[k].copy_(P.center[f0])
         self.box_s[k].copy_(P.wlh[f0])
         self.box_r[k].copy_(P.rot[f0])
-        if not self.motion:
+        if self.mode == "all":
+            self.hist_count[k] = 0
+            self.hist_keep[k].zero_()
+        elif not self.motion:
             box = bx.Box(P.center[f0], P.wlh[f0], P.rot[f0])
             local, keep, _ = bx.crop_and_center(P.scans[f0], box, offset=cfg.model_bb_offset, scale=cfg.model_bb_scale)
             self.first_local[k].copy_(local)
@@ -244,8 +286,18 @@ class BatchedDeviceTracker:
 
     def run(self):
         """Track every tracklet of the chunk; returns host copies of the records after the chunk's one synchronisation:
-        (overlap (F,), distance (F,), result centre (F, 3), result rotation (F, 3, 3)); frame-0 entries are left at 0."""
+        (overlap (F,), distance (F,), result centre (F, 3), result rotation (F, 3, 3)); frame-0 entries are left at 0.
+        In 'all' mode, a chunk in which some slot's history outgrew its capacity runs again with the capacity raised to
+        cover it, so the result is that of an unbounded history."""
         self.track()
+        while self.mode == "all":
+            peak = int(self.hist_peak.max())
+            if peak <= self.H:
+                break
+            self._alloc_history(-(-peak * 5 // 4 // 4096) * 4096)               # headroom: the rerun's trajectory may differ
+            self.hist_peak.zero_()
+            self.hist_count.zero_()
+            self.track()
         F = self.F
         return (self.overlap.cpu().numpy(), self.distance.cpu().numpy(), self.rec_c[:F].cpu().double().numpy(),
                 self.rec_r[:F].cpu().double().numpy())

@@ -107,6 +107,27 @@ def crop_in_box_frame(scans, box: Box, scale, offset, frame=None, count=None):
     return local, keep
 
 
+def crop_append(scans, box: Box, scale, offset, frame, count, hist, hist_keep, hist_count):
+    """`crop_in_box_frame`'s kept points appended in place to per-slot histories, in scan order — getModel's concatenation
+    (:88-100) one frame at a time.  scans (F, N, 3), one box per slot, frame (B,) (< 0: the slot is untouched), count (F,) or
+    None; hist (B, H, 3), hist_keep (B, H) bool, hist_count (B,) int64.  Slot b's kept points go to positions
+    hist_count[b] + j, those at H or beyond are dropped, and hist_count[b] grows by the full number kept, so an overflow shows
+    as hist_count > H.  CUDA fp32 inputs go through one kernel (csrc/geometry.cu); other tensors through the tensor formulation."""
+    half = torch.stack([box.wlh[..., 1], box.wlh[..., 0], box.wlh[..., 2]], -1) * (scale / 2) + offset
+    if scans.is_cuda and scans.dtype == torch.float32:
+        from .. import ops
+        ops.crop_append(scans.contiguous(), box.center, box.rot, half, frame, count, hist, hist_keep, hist_count)
+        return
+    H = hist_keep.shape[1]
+    local, keep = crop_in_box_frame(scans, box, scale, offset, frame.clamp(min=0), count)
+    keep = keep & (frame >= 0)[:, None]
+    pos = hist_count[:, None] + torch.cumsum(keep, 1) - 1
+    b, i = torch.nonzero(keep & (pos < H), as_tuple=True)
+    hist[b, pos[b, i]] = local[b, i].to(hist.dtype)
+    hist_keep[b, pos[b, i]] = True
+    hist_count += keep.sum(1)
+
+
 def point_to_box_distance(points, box: Box, wlh_factor=1.0):
     """get_point_to_box_distance (:127-144): (..., N, 9) distances to the centre and the eight corners."""
     ref = torch.cat([box.center[..., None, :], corners(box, wlh_factor)], -2)                  # (..., 9, 3)

@@ -3,26 +3,68 @@
 The reference's frame loop (models/base_model.py:44-117, :166-247) crops and resamples on the host with numpy /
 pyquaternion, uploads two small clouds, runs the network, downloads the proposals (`.cpu().numpy()`, :48) and updates the
 box on the host.  Here a frame is: scan already on the device -> search-area crop in the previous box's frame
-(generate_search_area :197-218) -> template = first-frame crop + previous-frame crop (generate_template :166-195,
-shape_aggregation 'firstandprevious' / 'first' / 'previous') -> fixed-shape resampling (sampling.py) -> BoxCloud of the
-template (bat.py:41-55) -> network in eval mode on the fused kernels -> best proposal -> box update (getOffsetBB).
+(generate_search_area :197-218; reference_BB 'previous_gt' / 'current_gt': the ground-truth box the caller passes) ->
+template = first-frame crop + previous-frame crop (generate_template :166-195, shape_aggregation 'firstandprevious' /
+'first' / 'previous'), or for 'all' the crops of every past frame, each in its own result box, appended to a history buffer
+-> fixed-shape resampling (sampling.py) -> BoxCloud of the template (bat.py:41-55) -> network in eval mode on the fused
+kernels -> best proposal -> box update (getOffsetBB) of the reference box.
 Every tensor has a static shape, nothing is read back, so the frame is captured once in a CUDA graph and replayed."""
 import torch
 
 from . import boxes as bx
 from .sampling import resample
 
+HISTORY_POINTS = 1 << 18        # starting capacity of the 'all' template history, points per tracklet (it grows on demand)
+
+
+def template_mode(cfg):
+    """shape_aggregation the way generate_template reads it (substring tests, in its order): 'firstandprevious', 'first',
+    'previous' or 'all'; anything else is a ValueError."""
+    raw = cfg.get("shape_aggregation", "firstandprevious")
+    for mode in ("FIRSTANDPREVIOUS", "FIRST", "PREVIOUS", "ALL"):
+        if mode in str(raw).upper():
+            return mode.lower()
+    raise ValueError(f"unknown shape_aggregation '{raw}'")
+
+
+def reference_mode(cfg):
+    """reference_BB the way generate_search_area reads it: 'previous_result', 'previous_gt' or 'current_gt'."""
+    raw = cfg.get("reference_BB", "previous_result")
+    for mode in ("PREVIOUS_RESULT", "PREVIOUS_GT", "CURRENT_GT"):
+        if mode in str(raw).upper():
+            return mode.lower()
+    raise ValueError(f"unknown reference_BB '{raw}'")
+
+
+def is_motion(model):
+    """Motion-centric models (M2-Track): a two-frame input instead of template + search area."""
+    return "point_sample_size" in model.config and not hasattr(model, "backbone")
+
+
+def tracking_modes(model):
+    """(template mode, reference mode) of a model's config; motion models ignore both settings, as the reference's
+    MotionBaseModel.build_input_dict does: (None, 'previous_result')."""
+    if is_motion(model):
+        return None, "previous_result"
+    return template_mode(model.config), reference_mode(model.config)
+
 
 class DeviceTracker:
-    def __init__(self, model, max_points, use_graph=True, seed=1):
+    """`reset(points, box)` on a tracklet's first frame, then `step(points, n_valid, ref_box)` per frame.  `seed` keys the
+    random draws; `history`: starting capacity (points) of the 'all' template history.  Motion models (M2-Track) ignore
+    shape_aggregation and reference_BB, as the reference's MotionBaseModel does."""
+
+    def __init__(self, model, max_points, use_graph=True, seed=1, history=HISTORY_POINTS):
         self.model = model.eval()
         self.cfg = model.config
         self.dev = next(model.parameters()).device
         self.max_points = int(max_points)
         self.use_graph = bool(use_graph) and self.dev.type == "cuda"
+        self.seed = int(seed)
         self.gen = torch.Generator(device=self.dev).manual_seed(seed)
         self.needs_bc = hasattr(model, "mlp_bc")            # BAT consumes the template BoxCloud
-        self.motion = "point_sample_size" in self.cfg and not hasattr(model, "backbone")   # M2-Track style two-frame input
+        self.motion = is_motion(model)                      # M2-Track style two-frame input
+        self.mode, self.ref_mode = tracking_modes(model)
         f = dict(device=self.dev, dtype=torch.float32)
         n = self.max_points
         # static buffers (graph inputs / state)
@@ -41,12 +83,47 @@ class DeviceTracker:
         self.u_s = (torch.zeros(n, **f), torch.zeros(size_s, **f))
         self.u_t = (torch.zeros(2 * n, **f), torch.zeros(size_t, **f))
         self.first_flag = torch.ones((), **f)               # 1 on the first tracked frame (prior box = ground truth), then 0
+        # reference box of the search area and of the box update in the ground-truth modes (step's ref_box)
+        self.ref_c, self.ref_s, self.ref_r = torch.zeros(3, **f), torch.ones(3, **f), torch.eye(3, **f)
+        if self.mode == "all":
+            # history of the 'all' template: the crops of frames 0 .. t-1, each in its result box, in frame and scan order
+            i64 = dict(device=self.dev, dtype=torch.int64)
+            self.scan_count, self.prev_count = torch.zeros(1, **i64), torch.zeros(1, **i64)
+            self.slot0 = torch.zeros(1, **i64)              # the one slot's scan index and tracklet id
+            self.frame_id = torch.zeros(1, **i64)
+            self.hist_count = torch.zeros(1, **i64)
+            self.hist_bound = 0                             # host upper bound of hist_count
+            self.prev_n = 0                                 # valid points of the previous scan: what the next append can add
+            self._alloc_history(int(history))
         self.graph = None
         self.frames = 0
+
+    def _alloc_history(self, H, keep_count=0):
+        """(Re)allocate the history for H points, keeping its first `keep_count` entries; the captured graph is dropped."""
+        f = dict(device=self.dev, dtype=torch.float32)
+        hist, keep = torch.zeros(1, H, 3, **f), torch.zeros(1, H, dtype=torch.bool, device=self.dev)
+        if keep_count:
+            hist[:, :keep_count].copy_(self.hist[:, :keep_count])
+            keep[:, :keep_count].copy_(self.hist_keep[:, :keep_count])
+        self.hist, self.hist_keep, self.H = hist, keep, H
+        self.u_t = (torch.zeros(H, **f), self.u_t[1])      # the template draw is over the history
+        self.graph = None
 
     # ------------------------------------------------------------------ state helpers
     def _box(self):
         return bx.Box(self.box_c, self.box_s, self.box_r)
+
+    def _ref_box(self):
+        """The box the search area is cropped in and the offset is applied to (generate_search_area's ref_bb)."""
+        return self._box() if self.ref_mode == "previous_result" else bx.Box(self.ref_c, self.ref_s, self.ref_r)
+
+    def _set_ref(self, ref_box):
+        if self.ref_mode == "previous_result":
+            return
+        if ref_box is None:
+            raise ValueError(f"reference_BB '{self.ref_mode}' needs the ground-truth reference box: step(..., ref_box=...)")
+        rb = ref_box.to(self.dev)
+        self.ref_c.copy_(rb.center); self.ref_s.copy_(rb.wlh); self.ref_r.copy_(rb.rot)
 
     def _load_scan(self, points, n_valid=None):
         n = points.shape[0]
@@ -54,15 +131,25 @@ class DeviceTracker:
             raise ValueError(f"scan has {n} points, tracker was built for {self.max_points}")
         self.scan.zero_()
         self.scan[:n].copy_(points)
+        n_valid = n if n_valid is None else int(n_valid)
         self.scan_valid.zero_()
-        self.scan_valid[: (n if n_valid is None else int(n_valid))] = True
+        self.scan_valid[:n_valid] = True
+        if self.mode == "all":
+            self.scan_count.fill_(n_valid)
+        return n_valid
 
     def reset(self, points, box: bx.Box):
-        """First frame: remember the object crop (cropAndCenterPC of the first box) and the box itself."""
-        self._load_scan(points)
+        """First frame: remember the object crop (cropAndCenterPC of the first box) and the box itself; in 'all' mode empty
+        the history (the first step appends this frame's crop)."""
+        n = self._load_scan(points)
         box = box.to(self.dev)
         self.box_c.copy_(box.center); self.box_s.copy_(box.wlh); self.box_r.copy_(box.rot)
-        if not self.motion:
+        if self.mode == "all":
+            self.hist_count.zero_()
+            self.hist_keep.zero_()
+            self.prev_count.copy_(self.scan_count)
+            self.hist_bound, self.prev_n = 0, n
+        elif not self.motion:
             local, keep, _ = bx.crop_and_center(self.scan, box, offset=self.cfg.model_bb_offset, scale=self.cfg.model_bb_scale)
             self.first_local.copy_(local)
             self.first_keep.copy_(keep & self.scan_valid)
@@ -97,22 +184,26 @@ class DeviceTracker:
     def _inputs(self):
         if self.motion:
             return self._inputs_motion()
-        cfg, box = self.cfg, self._box()
+        cfg, box, ref = self.cfg, self._box(), self._ref_box()
         b1 = bx.Box(box.center[None], box.wlh[None], box.rot[None])
+        r1 = bx.Box(ref.center[None], ref.wlh[None], ref.rot[None])
 
         def build_template():
-            # template: first-frame crop (+ previous-frame crop around the previous result)
-            mode = cfg.shape_aggregation.upper()
-            p_local, p_keep = bx.crop_in_box_frame(self.prev_scan[None], b1, cfg.model_bb_scale, cfg.model_bb_offset)
-            p_local, p_keep = p_local[0], p_keep[0] & self.prev_valid
-            if "FIRSTANDPREVIOUS" in mode:
-                cand, keep = torch.cat([self.first_local, p_local]), torch.cat([self.first_keep, p_keep])
-            elif "FIRST" in mode:
+            # template: first-frame crop (+ previous-frame crop around the previous result), or every past frame's crop
+            mode = self.mode
+            if mode == "all":
+                bx.crop_append(self.prev_scan[None], b1, cfg.model_bb_scale, cfg.model_bb_offset, self.slot0, self.prev_count,
+                               self.hist, self.hist_keep, self.hist_count)
+                cand, keep = self.hist[0], self.hist_keep[0]
+            elif mode == "first":
                 cand, keep = self.first_local, self.first_keep
-            elif "PREVIOUS" in mode:
-                cand, keep = p_local, p_keep
             else:
-                raise NotImplementedError(f"shape_aggregation '{cfg.shape_aggregation}' needs every past frame on the device")
+                p_local, p_keep = bx.crop_in_box_frame(self.prev_scan[None], b1, cfg.model_bb_scale, cfg.model_bb_offset)
+                p_local, p_keep = p_local[0], p_keep[0] & self.prev_valid
+                if mode == "firstandprevious":
+                    cand, keep = torch.cat([self.first_local, p_local]), torch.cat([self.first_keep, p_keep])
+                else:
+                    cand, keep = p_local, p_keep
             template, _ = resample(cand, keep, cfg.template_size, u_perm=self.u_t[0][: cand.shape[0]], u_pick=self.u_t[1])
             bc = None
             if self.needs_bc:
@@ -124,8 +215,8 @@ class DeviceTracker:
         # the two crops + draws are independent: the template's run on the side stream (a parallel branch of the frame's graph)
         overlap = fused.branch_overlap(self.scan)
         join = fused.run_ahead(build_template) if overlap else None
-        # search area: current scan in the frame of the reference box (= previous result)
-        s_local, s_keep = bx.crop_in_box_frame(self.scan[None], b1, cfg.search_bb_scale, cfg.search_bb_offset)
+        # search area: current scan in the frame of the reference box (previous result, or the caller's ground truth)
+        s_local, s_keep = bx.crop_in_box_frame(self.scan[None], r1, cfg.search_bb_scale, cfg.search_bb_offset)
         s_local, s_keep = s_local[0], s_keep[0]
         search, _ = resample(s_local, s_keep & self.scan_valid, cfg.search_size, u_perm=self.u_s[0], u_pick=self.u_s[1])
         template, bc = join() if overlap else build_template()
@@ -143,22 +234,61 @@ class DeviceTracker:
             est = out["estimation_boxes"][0]                                   # (num_proposal, 5) or (4,)
             if est.dim() == 2:
                 est = est.index_select(0, est[:, 4].argmax().reshape(1))[0, :4]    # (indexing by a 0-d tensor would sync)
-            new = bx.offset_box(self._box(), est, degrees=cfg.degrees, use_z=cfg.use_z, limit_box=cfg.limit_box)
+            new = bx.offset_box(self._ref_box(), est, degrees=cfg.degrees, use_z=cfg.use_z, limit_box=cfg.limit_box)
             self.box_c.copy_(new.center); self.box_r.copy_(new.rot)
+            if self.ref_mode != "previous_result":
+                self.box_s.copy_(new.wlh)                                       # the result takes the reference box's size
             self.prev_scan.copy_(self.scan); self.prev_valid.copy_(self.scan_valid)
+            if self.mode == "all":
+                self.prev_count.copy_(self.scan_count)
             self.first_flag.zero_()
 
-    def step(self, points, n_valid=None):
-        """Next frame: `points` (n, 3) device tensor.  Returns the tracked box (views of the tracker's state buffers)."""
+    def _reserve_history(self):
+        """Make room for this step's append, which adds at most the previous scan's valid points.  The host bound on the count
+        is exact only after a read-back, so the count is read (one synchronisation) only when the bound could pass H, and
+        the history grows (copied, graph captured again) only when the exact count could."""
+        need = self.hist_bound + self.prev_n
+        if need > self.H:
+            self.hist_bound = int(self.hist_count[0])
+            need = self.hist_bound + self.prev_n
+            if need > self.H:
+                self._alloc_history(max(need, 2 * self.H), keep_count=min(self.hist_bound, self.H))
+        self.hist_bound = need
+
+    def _draw(self):
+        """Per-frame uniform draws, outside the graph.  The 'all' history's permutation draw is keyed by (seed, tracklet 0,
+        frame) on the device, so it does not depend on the history's capacity; the others come from the tracker's generator."""
+        if self.mode != "all":
+            for u in self.u_s + self.u_t:
+                u.uniform_(generator=self.gen)
+            return
+        for u in self.u_s + self.u_t[1:]:
+            u.uniform_(generator=self.gen)
+        if self.dev.type == "cuda":
+            from .. import ops
+            from .batched_tracker import STREAM_TEMPLATE_PERM
+            self.frame_id.fill_(self.frames)
+            ops.keyed_uniform(self.slot0, self.frame_id, self.seed, STREAM_TEMPLATE_PERM, self.H, out=self.u_t[0].view(1, -1))
+        else:
+            self.u_t[0].uniform_(generator=self.gen)
+
+    def step(self, points, n_valid=None, ref_box=None):
+        """Next frame: `points` (n, 3) device tensor, the first `n_valid` valid.  `ref_box`: this frame's reference box,
+        required in the reference_BB modes 'previous_gt' (the previous frame's ground truth) and 'current_gt' (this frame's).
+        Returns the tracked box (views of the tracker's state buffers)."""
         if self.frames == 0:
             raise RuntimeError("call reset() with the first frame and its box before step()")
-        self._load_scan(points, n_valid)
-        for u in self.u_s + self.u_t:
-            u.uniform_(generator=self.gen)
+        self._set_ref(ref_box)
+        if self.mode == "all":
+            self._reserve_history()
+        n = self._load_scan(points, n_valid)
+        self._draw()
         if not self.use_graph:
             self._frame()
         elif self.graph is None:
-            state = (self.box_c, self.box_r, self.prev_scan, self.prev_valid, self.first_flag)
+            state = (self.box_c, self.box_s, self.box_r, self.prev_scan, self.prev_valid, self.first_flag)
+            if self.mode == "all":
+                state += (self.hist_keep, self.hist_count, self.prev_count)
             snap = [t.clone() for t in state]
             s = torch.cuda.Stream()
             s.wait_stream(torch.cuda.current_stream())
@@ -176,4 +306,6 @@ class DeviceTracker:
         else:
             self.graph.replay()
         self.frames += 1
+        if self.mode == "all":
+            self.prev_n = n
         return self._box()

@@ -25,18 +25,24 @@ def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 <
     (seed, its index in `sequences`, frame), so its result does not depend on `slots`.
     Returns the keys of `evaluate()` ("results": a data_classes.Box list per tracklet, in input order) plus the per-frame
     "overlaps" / "distances" (lists per tracklet).  Frame 0 of every tracklet is scored on the host, as the reference does:
-    its ground truth against itself sits exactly on Success's top threshold."""
+    its ground truth against itself sits exactly on Success's top threshold.
+    The model's shape_aggregation (including 'all': every past frame's crop, kept in a per-slot history whose bytes count
+    against `max_resident_bytes`) and reference_BB ('previous_gt' / 'current_gt': the search area and the box update use the
+    ground truth of the previous / current frame, and the result box takes its size) are honoured as the host loop does."""
     import numpy as np
 
     from ..datasets import data_classes
     from ..utils.metrics import estimateAccuracy, estimateOverlap
-    from .batched_tracker import BatchedDeviceTracker, plan_chunks, pool_frame_bytes
+    from .batched_tracker import BatchedDeviceTracker, history_bytes, plan_chunks, pool_frame_bytes
+    from .device_tracker import HISTORY_POINTS, tracking_modes
 
     sequences = list(sequences)
     cfg = model.config
     dim, up = cfg.IoU_space, cfg.up_axis
     n = len(sequences)
     lengths = [len(s) for s in sequences]
+    mode, ref_mode = tracking_modes(model)
+    size_from = {"previous_result": lambda t: 0, "previous_gt": lambda t: t - 1, "current_gt": lambda t: t}[ref_mode]
     overlaps, distances, results = [[] for _ in range(n)], [[] for _ in range(n)], [[] for _ in range(n)]
     for j, seq in enumerate(sequences):
         if lengths[j]:
@@ -46,7 +52,8 @@ def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 <
             results[j].append(gt0)
     if any(n_ > 1 for n_ in lengths):
         npts = max(f["pc"].points.shape[1] for s in sequences for f in s)
-        for chunk in plan_chunks(lengths, pool_frame_bytes(npts), max_resident_bytes):
+        fixed = history_bytes(min(slots, n), HISTORY_POINTS) if mode == "all" else 0
+        for chunk in plan_chunks(lengths, pool_frame_bytes(npts), max_resident_bytes, fixed):
             if all(lengths[j] < 2 for j in chunk):
                 continue
             trk = BatchedDeviceTracker(model, [sequences[j] for j in chunk], slots, seed=seed, ids=chunk, max_points=npts,
@@ -56,10 +63,11 @@ def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 <
             del trk
             for i, j in enumerate(chunk):
                 o, L = int(offsets[i]), lengths[j]
-                wlh = np.asarray(sequences[j][0]["3d_bbox"].wlh, dtype=np.float32).astype(np.float64)   # the fp32 state's size
+                # the fp32 state's size: the first box's, or in the ground-truth modes the reference box's
+                wlh = [np.asarray(f["3d_bbox"].wlh, dtype=np.float32).astype(np.float64) for f in sequences[j]]
                 overlaps[j] += ov[o + 1: o + L].tolist()
                 distances[j] += di[o + 1: o + L].tolist()
-                results[j] += [data_classes.Box(cen[o + t], wlh, rot[o + t]) for t in range(1, L)]
+                results[j] += [data_classes.Box(cen[o + t], wlh[size_from(t)], rot[o + t]) for t in range(1, L)]
     succ, prec = Success(), Precision()
     for j in range(n):
         succ(overlaps[j])
