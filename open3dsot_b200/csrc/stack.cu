@@ -117,9 +117,11 @@ __global__ void unpack_wgrad_kernel(const UnpackArgs args) {
     }
 }
 
-__global__ void d2f_kernel(const double* __restrict__ src, int n, float* __restrict__ dst, int accumulate) {
+// bias gradient dst (+)= src * scale from the fp64 column sums `src` of the gradient entering the layer (scale nullable = 1)
+__global__ void d2f_kernel(const double* __restrict__ src, const float* __restrict__ scale, int n, float* __restrict__ dst,
+                           int accumulate) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) dst[i] = (accumulate ? dst[i] : 0.f) + (float)src[i];
+    if (i < n) dst[i] = (accumulate ? dst[i] : 0.f) + (float)(scale ? src[i] * (double)scale[i] : src[i]);
 }
 
 // ---- workspace plan -------------------------------------------------------------------------------------------
@@ -417,10 +419,14 @@ extern "C" int o3d_stack_backward(const o3d_stack_t* d, const float* x, const vo
                                      cout, coef, coef + Nl, coef + 2 * Nl, d->d_gamma[l], d->d_beta[l], stream);
             if (rc) return rc;
             a = coef; b = coef + Nl; cc = coef + 2 * Nl;
-            if (d->d_bias[l] && !d->accumulate)      // BN removes the mean: the bias gradient is zero (nothing to add when accumulating)
-                O3D_CUDA(cudaMemsetAsync(d->d_bias[l], 0, sizeof(float) * cout, st), "d_bias");
+            if (d->d_bias[l] && d->training) {
+                if (!d->accumulate)      // BN removes the mean: the bias gradient is zero (nothing to add when accumulating)
+                    O3D_CUDA(cudaMemsetAsync(d->d_bias[l], 0, sizeof(float) * cout, st), "d_bias");
+            } else if (d->d_bias[l]) {   // running statistics: BN is the affine map a*y + const, so d_bias = a * sum g
+                d2f_kernel<<<(cout + 127) / 128, 128, 0, st>>>(s1(l), a, cout, d->d_bias[l], d->accumulate);
+            }
         } else if (d->d_bias[l]) {
-            d2f_kernel<<<(cout + 127) / 128, 128, 0, st>>>(s1(l), cout, d->d_bias[l], d->accumulate);
+            d2f_kernel<<<(cout + 127) / 128, 128, 0, st>>>(s1(l), nullptr, cout, d->d_bias[l], d->accumulate);
         }
         if (l == 0 && p.lift) {
             // the lifted layer has no GEMM: dY0 = a*g + b + cc*Y0 is scattered into dZ / dcc / ds / du

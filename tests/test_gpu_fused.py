@@ -20,8 +20,10 @@ def rel(a, b):
     return float((a - b).norm() / (b.norm() + 1e-30))
 
 
-def reference_stack(x, specs, S, training):
-    """fp64 statement of the stack on a (P, K) matrix; returns output and leaves grads to autograd."""
+def reference_stack(x, specs, S, training, batch_stats=None):
+    """fp64 statement of the stack on a (P, K) matrix; returns output and leaves grads to autograd.  The max over a pooling
+    group sends its gradient to the FIRST position holding the maximum (as F.max_pool2d does), whatever max(dim) would pick
+    among exact ties.  `batch_stats`, a list, receives (mean, unbiased variance) of every training-mode BatchNorm."""
     h = x.double()
     for s in specs:
         W = s.weight.reshape(s.weight.shape[0], -1).double()
@@ -31,22 +33,28 @@ def reference_stack(x, specs, S, training):
         if s.bn is not None:
             if training:
                 mu, var = h.mean(0), h.var(0, unbiased=False)
+                if batch_stats is not None:
+                    batch_stats.append((mu.detach(), h.var(0, unbiased=True).detach()))
             else:
                 mu, var = s.bn.running_mean.double(), s.bn.running_var.double()
             h = (h - mu) / torch.sqrt(var + s.bn.eps) * s.bn.weight.double() + s.bn.bias.double()
         if s.relu:
             h = F.relu(h)
     if S > 0:
-        h = h.view(-1, S, h.shape[1]).max(dim=1)[0]
+        g = h.view(-1, S, h.shape[1])
+        mx = g.detach().max(dim=1, keepdim=True)[0]
+        first = (g.detach() == mx).to(torch.uint8).argmax(dim=1, keepdim=True)   # argmax returns the first maximal index
+        h = g.gather(1, first).squeeze(1)
     return h
 
 
-def check_grads(g_out, g_ref, S, xshape):
+def check_grads(g_out, g_ref, S, xshape, max_flips=3):
     """Gradients must agree to 2e-4 relative.  One bounded exception: a discrete decision that sits within fp32
     round-off of its threshold — two positions of a pooling group with (almost) equal values, or a pre-activation within
     ~1e-6 of zero — can fall the other way in the fp32 kernels than in the fp64 reference.  That moves ONE element's
     gradient, i.e. it shows up as an error confined to a few rows of the input gradient (and an O(1e-3) ripple in the
-    parameter gradients).  At most three such rows / pooling groups are accepted."""
+    parameter gradients).  At most `max_flips` such rows / pooling groups are accepted (0 where the inputs hold exact ties,
+    which both sides must break the same way)."""
     scale = max(float(g.double().norm()) for g in g_ref if g is not None)
     tol = 2e-4
     if g_ref[0] is not None:
@@ -54,7 +62,7 @@ def check_grads(g_out, g_ref, S, xshape):
         e = (g_out[0].double() - g_ref[0].double()).reshape(-1, rows, xshape[1]).norm(dim=(1, 2))
         thr = 2e-4 * float(g_ref[0].double().norm()) / max(e.numel(), 1) ** 0.5
         flipped = int((e > 50 * thr).sum())
-        assert flipped <= 3, f"{flipped} rows / pooling groups disagree with the reference"
+        assert flipped <= max_flips, f"{flipped} rows / pooling groups disagree with the reference"
         if flipped:
             tol = 1e-2
     for gn, gr in zip(g_out, g_ref):
