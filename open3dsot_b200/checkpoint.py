@@ -80,7 +80,24 @@ def load_reference_weights(model, path, strict=True, map_location="cpu"):
     return ckpt
 
 
-def save_lightning_checkpoint(model, path, epoch=0, global_step=0, optimizer_states=None, lr_schedulers=None, extra_state_dict=None):
+class ModelCheckpoint:
+    """Stand-in for the class Lightning keys ModelCheckpoint's state by in `callbacks`; `save_lightning_checkpoint` pickles it
+    under the global name `pytorch_lightning.callbacks.model_checkpoint.ModelCheckpoint`.  Never instantiated."""
+
+
+_PICKLED_AS = {"ModelCheckpoint": "pytorch_lightning.callbacks.model_checkpoint"}
+
+
+def model_checkpoint_state(ckpt):
+    """The ModelCheckpoint entry of a checkpoint's `callbacks` (ours or Lightning's), or None."""
+    for key, value in (ckpt.get("callbacks") or {}).items():
+        if getattr(key, "__name__", key) == "ModelCheckpoint":
+            return value
+    return None
+
+
+def save_lightning_checkpoint(model, path, epoch=0, global_step=0, optimizer_states=None, lr_schedulers=None, extra_state_dict=None,
+                              callbacks=None):
     """Write `model` in the layout of the reference's Lightning-1.3.8 checkpoints (SURVEY.md §8b), so that the reference's
     own `Model.load_from_checkpoint(path, config=cfg)` / `--checkpoint` (main.py:67-70,78-79) reads it back:
 
@@ -90,7 +107,8 @@ def save_lightning_checkpoint(model, path, epoch=0, global_step=0, optimizer_sta
 
     `extra_state_dict`: entries of the reference's parameter-free metric modules (`prec.*`, `success.*`: torchmetrics buffers)
     to carry over from a loaded checkpoint; they hold no weights and are absent by default (Lightning loads non-strictly
-    only if asked, so pass them through when the file must load with `strict=True` in the reference)."""
+    only if asked, so pass them through when the file must load with `strict=True` in the reference).
+    `callbacks`: {ModelCheckpoint: state dict} as trainer.Trainer writes it (default: empty)."""
     import sys
     import types
     from .compat import easydict as _ed
@@ -102,23 +120,31 @@ def save_lightning_checkpoint(model, path, epoch=0, global_step=0, optimizer_sta
     if cfg is not None:
         hp["config"] = _ed.EasyDict(dict(cfg))
     ckpt = {"epoch": int(epoch), "global_step": int(global_step), "pytorch-lightning_version": "1.3.8", "state_dict": sd,
-            "hyper_parameters": hp, "optimizer_states": optimizer_states or [], "lr_schedulers": lr_schedulers or [], "callbacks": {}}
-    # the stand-in EasyDict must be written under the name the reference environment resolves: easydict.EasyDict
-    cls = _ed.EasyDict
-    shim = None
-    if cls.__module__ != "easydict":
-        shim = types.ModuleType("easydict")
-        shim.EasyDict = cls
-        old = (cls.__module__, cls.__qualname__, sys.modules.get("easydict"))
-        cls.__module__, cls.__qualname__ = "easydict", "EasyDict"
-        sys.modules["easydict"] = shim
+            "hyper_parameters": hp, "optimizer_states": optimizer_states or [], "lr_schedulers": lr_schedulers or [],
+            "callbacks": callbacks or {}}
+    # the stand-ins must be written under the names the reference environment resolves: easydict.EasyDict and Lightning's
+    # ModelCheckpoint; pickle checks a global name by importing its module, so each module and its parents are stubbed
+    renamed, stubbed = [], {}
+    for cls, module in ((_ed.EasyDict, "easydict"), (ModelCheckpoint, _PICKLED_AS["ModelCheckpoint"])):
+        if cls.__module__ == module:
+            continue
+        renamed.append((cls, cls.__module__, cls.__qualname__))
+        cls.__module__, cls.__qualname__ = module, cls.__name__
+        parts = module.split(".")
+        for i in range(1, len(parts) + 1):
+            name = ".".join(parts[:i])
+            if name not in stubbed:
+                stubbed[name] = sys.modules.get(name)
+                sys.modules[name] = types.ModuleType(name)
+        setattr(sys.modules[module], cls.__name__, cls)
     try:
         torch.save(ckpt, path, _use_new_zipfile_serialization=False)      # the legacy (non-zip) format Lightning 1.3.8 wrote
     finally:
-        if shim is not None:
-            cls.__module__, cls.__qualname__ = old[0], old[1]
-            if old[2] is None:
-                sys.modules.pop("easydict", None)
+        for cls, module, qualname in renamed:
+            cls.__module__, cls.__qualname__ = module, qualname
+        for name, old in stubbed.items():
+            if old is None:
+                sys.modules.pop(name, None)
             else:
-                sys.modules["easydict"] = old[2]
+                sys.modules[name] = old
     return path

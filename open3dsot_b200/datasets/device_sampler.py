@@ -252,10 +252,17 @@ class DeviceSiameseSampler:
         self.num_candidates = cfg.get("num_candidates", 1)
         self._graphs = {}
 
-    def _build(self, B):
+    def __len__(self):
+        """Samples per epoch, as the reference's PointTrackingSampler counts them: every frame once per candidate."""
+        return self.data.num_frames * self.num_candidates
+
+    def _build(self, B, indices=None):
         pool = int(B * self.oversample) + 1
         dev = self.data.scans.device
-        index = torch.randint(0, self.data.num_frames * self.num_candidates, (pool,), device=dev, generator=self.gen)
+        if indices is None:
+            index = torch.randint(0, len(self), (pool,), device=dev, generator=self.gen)
+        else:       # the epoch's samples first; the random rest of the pool stands in for the ones that are rejected
+            index = torch.cat([indices, torch.randint(0, len(self), (pool - B,), device=dev, generator=self.gen)])
         batch, valid = self.processing(self.data, self.cfg, index // self.num_candidates, index % self.num_candidates,
                                        generator=self.gen)
         order = torch.argsort((~valid).to(torch.int8), stable=True)           # valid samples first, original order kept
@@ -266,21 +273,30 @@ class DeviceSiameseSampler:
         order = order[torch.arange(B, device=dev) % nvalid]
         return {k: v[order] for k, v in batch.items() if not k.startswith("_")}, valid[order]
 
-    def next_batch(self, batch_size=None):
+    def next_batch(self, batch_size=None, indices=None):
+        """`indices`: optional (B,) int64 device tensor of sample indices in [0, len(self)) (frame * num_candidates +
+        candidate), the reference's epoch order; by default every sample is drawn at random.  Sample i of the batch is
+        indices[i] unless the reference would reject it; then valid samples move up and random valid draws fill the end."""
         B = batch_size or self.cfg.batch_size
+        if indices is not None and tuple(indices.shape) != (B,):
+            raise ValueError(f"next_batch: indices of shape {tuple(indices.shape)} for a batch of {B}")
         if not self.use_graph:
-            return self._build(B)
-        if B not in self._graphs:
+            return self._build(B, indices)
+        key = (B, indices is not None)
+        if key not in self._graphs:
+            static = None if indices is None else torch.zeros(B, dtype=torch.int64, device=self.data.scans.device)
             s = torch.cuda.Stream()
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
-                self._build(B)                                   # warm-up: allocator, lazy initialisations
+                self._build(B, static)                           # warm-up: allocator, lazy initialisations
             torch.cuda.current_stream().wait_stream(s)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                out = self._build(B)
-            self._graphs[B] = (g, out)
-        g, out = self._graphs[B]
+                out = self._build(B, static)
+            self._graphs[key] = (g, out, static)
+        g, out, static = self._graphs[key]
+        if static is not None:
+            static.copy_(indices, non_blocking=True)
         g.replay()
         return out
 

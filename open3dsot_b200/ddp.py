@@ -81,8 +81,18 @@ def broadcast_parameters(flat: FlatParams, module: torch.nn.Module):
     if not dist.is_initialized() or dist.get_world_size() == 1:
         return
     dist.broadcast(flat.flat, src=0)
+    broadcast_buffers(module)
+
+
+def broadcast_buffers(module: torch.nn.Module):
+    """Rank 0's buffers (BatchNorm running statistics) become everyone's; no-op on a single rank.  The collective writes
+    bump no tensor version, so the weights generation advances for the static-weight caches."""
+    if not dist.is_initialized() or dist.get_world_size() == 1:
+        return
+    from . import runtime
     for b in module.buffers():
         dist.broadcast(b, src=0)
+    runtime.advance_weights_generation()
 
 
 def allreduce_gradients(flat: FlatParams, async_op=False):

@@ -9,7 +9,7 @@ not reproduced).
 """
 import torch
 
-from . import _lib, ddp, ops
+from . import _lib, ddp, ops, runtime
 
 
 class BatchSlab:
@@ -62,6 +62,60 @@ class FlatAdam:
         ops._call("o3d_adam_step", self.flat.flat.data_ptr(), self.flat.grad.data_ptr(), self.exp_avg.data_ptr(),
                   self.exp_avg_sq.data_ptr(), self.flat.numel, self.state.data_ptr(), self.betas[0], self.betas[1],
                   self.eps, self.wd, ops._stream())
+        runtime.advance_weights_generation()
+
+    def _slices(self):
+        off = 0
+        for p in self.flat.params:
+            yield off, p
+            off += p.numel()
+
+    def state_dict(self, initial_lr=None):
+        """`torch.optim.Adam.state_dict()` of one param group over `flat.params` (the model's trainable parameters, in order;
+        the indices match an Adam over all of `model.parameters()`, the reference's, only when none is frozen, which
+        `trainer.Trainer` requires): `state`
+        keyed by parameter index with `step`, `exp_avg` and `exp_avg_sq` (CPU copies of slices of the flat buffers), or empty
+        before the first step, as Adam's is."""
+        step, lr = (float(v) for v in self.state.cpu())
+        state = {}
+        if step > 0:
+            for i, (off, p) in enumerate(self._slices()):
+                n = p.numel()
+                state[i] = {"step": torch.tensor(step), "exp_avg": self.exp_avg[off:off + n].view_as(p).cpu().clone(),
+                            "exp_avg_sq": self.exp_avg_sq[off:off + n].view_as(p).cpu().clone()}
+        group = {"lr": lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.wd, "amsgrad": False,
+                 "initial_lr": lr if initial_lr is None else initial_lr, "params": list(range(len(self.flat.params)))}
+        return {"state": state, "param_groups": [group]}
+
+    def load_state_dict(self, sd):
+        """Moments and step from an Adam state dict (ours or a Lightning checkpoint's `optimizer_states[0]`).  An empty `state`
+        means zero moments and step 0.  The learning rate is left to the caller's schedule."""
+        params = self.flat.params
+        groups = sd["param_groups"]
+        n = sum(len(g["params"]) for g in groups)
+        if len(groups) != 1 or n != len(params):
+            raise ValueError(f"Adam state: {len(groups)} param group(s) over {n} parameters; the model has one group of "
+                             f"{len(params)}")
+        state = sd["state"]
+        exp_avg, exp_avg_sq = torch.zeros_like(self.exp_avg), torch.zeros_like(self.exp_avg_sq)
+        steps = set()
+        for i, (off, p) in enumerate(self._slices()):
+            s = state.get(groups[0]["params"][i])
+            if s is None:
+                if state:
+                    raise ValueError(f"Adam state: parameter {i} has no state while others have")
+                continue
+            for key, dst in (("exp_avg", exp_avg), ("exp_avg_sq", exp_avg_sq)):
+                if tuple(s[key].shape) != tuple(p.shape):
+                    raise ValueError(f"Adam state: parameter {i} {key} has shape {tuple(s[key].shape)}, the model's is "
+                                     f"{tuple(p.shape)}")
+                dst[off:off + p.numel()].copy_(s[key].reshape(-1))
+            steps.add(float(s["step"]))
+        if len(steps) > 1:
+            raise ValueError(f"Adam state: the parameters' steps differ ({sorted(steps)}); the flat optimizer keeps one")
+        self.exp_avg.copy_(exp_avg)
+        self.exp_avg_sq.copy_(exp_avg_sq)
+        self.state[0] = steps.pop() if steps else 0.0
 
 
 class TrainStep:
@@ -158,4 +212,5 @@ class TrainStep:
         self.graph.replay()
         if not self.graph_has_update:
             self._finish()
+        runtime.advance_weights_generation()        # the replayed Adam and BatchNorm writes bump no tensor version
         return self.static_loss

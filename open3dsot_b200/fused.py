@@ -127,8 +127,9 @@ def _describe(meta, P, K0, params):
 def _static_cached(tag, extra, deps, make):
     """`make()` -- a tensor computed from the tensors `deps` (None entries allowed) -- cached for inference with static weights
     (runtime.static_weights_scope).  The entry is stored on the first tensor of `deps`, keyed by `tag`, `extra` and the identity
-    of every dep, and is valid while every dep's version is unchanged (`load_state_dict` / in-place edits invalidate it).  It
-    keeps its deps alive, so their ids stay unique.
+    of every dep, and is valid while every dep's version and the weights generation (advanced by every training step, whose
+    writes bump no version) are unchanged (`load_state_dict` / in-place edits / training invalidate it).  It keeps its deps
+    alive, so their ids stay unique.
 
     A cached tensor may be read from another stream (the template / search branches run side by side, run_ahead) with no
     ordering against the stream that built it, so the builder finishes before the entry becomes visible.  During graph capture
@@ -137,7 +138,7 @@ def _static_cached(tag, extra, deps, make):
     owner = next(t for t in deps if t is not None)
     cache = owner.__dict__.setdefault("_o3d_static", {})
     key = (tag, extra, tuple(id(t) for t in deps))
-    versions = tuple(-1 if t is None else t._version for t in deps)
+    versions = (runtime.weights_generation(),) + tuple(-1 if t is None else t._version for t in deps)
     hit = cache.get(key)
     if hit is not None and hit[0] == versions:
         return hit[1]

@@ -53,6 +53,20 @@ def set_branch_overlap(flag: bool) -> None:
 # statistics ONCE (o3d_stack_prepare) instead of per call.  Off by default; static_weights_scope() turns it on.
 _STATIC_WEIGHTS = False
 
+# Advanced by the engine once per training step.  Its Adam writes the parameters through a raw pointer, a graph replay bumps no
+# tensor version, and the fused training forward writes the BatchNorm running statistics through pointers: none of these is
+# visible in `Tensor._version`, so every static-weight cache entry also records the generation it was built in.
+_WEIGHTS_GENERATION = 0
+
+
+def weights_generation() -> int:
+    return _WEIGHTS_GENERATION
+
+
+def advance_weights_generation() -> None:
+    global _WEIGHTS_GENERATION
+    _WEIGHTS_GENERATION += 1
+
 
 def static_weights() -> bool:
     return _STATIC_WEIGHTS
@@ -64,8 +78,8 @@ def static_weights_scope():
 
     The cached blocks are keyed by the identity and tensor version of every tensor they are computed from: the parameters and
     the running mean and variance of every BatchNorm that tracks them, so `load_state_dict` and other in-place updates rebuild
-    them.  The engine's fused Adam updates parameters in place without bumping them: a scope must not span training steps, or
-    the forward passes after a step run on the old weights."""
+    them.  They also record the weights generation, which every `engine.TrainStep.step` / `FlatAdam.step` advances, so the
+    first forward after a training step rebuilds them, whether or not a scope was open across the step."""
     global _STATIC_WEIGHTS
     old = _STATIC_WEIGHTS
     _STATIC_WEIGHTS = True

@@ -18,11 +18,12 @@ def evaluate(model, sequences, progress=None):
     return {"success": succ.compute(), "precision": prec.compute(), "frames": frames, "results": results}
 
 
-def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 << 30, use_graph=True):
+def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 << 30, use_graph=True, ids=None):
     """`evaluate()` with `slots` tracklets in flight on the device (tracking/batched_tracker.py): one graph replay per frame
     step for all of them, overlap and centre distance computed on the device, one device-to-host copy per chunk of tracklets
     whose padded frames fit `max_resident_bytes` (a tracklet is never split).  The random draws of a tracklet are keyed by
-    (seed, its index in `sequences`, frame), so its result does not depend on `slots`.
+    (seed, its id, frame), so its result does not depend on `slots`.  `ids`: the tracklets' ids (default: their indices in
+    `sequences`); a shard of a split passes the tracklets' indices in the whole split (`evaluate_sharded`).
     Returns the keys of `evaluate()` ("results": a data_classes.Box list per tracklet, in input order) plus the per-frame
     "overlaps" / "distances" (lists per tracklet).  Frame 0 of every tracklet is scored on the host, as the reference does:
     its ground truth against itself sits exactly on Success's top threshold.
@@ -40,6 +41,9 @@ def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 <
     cfg = model.config
     dim, up = cfg.IoU_space, cfg.up_axis
     n = len(sequences)
+    ids = list(range(n)) if ids is None else [int(i) for i in ids]
+    if len(ids) != n:
+        raise ValueError(f"evaluate_batched: {len(ids)} ids for {n} tracklets")
     lengths = [len(s) for s in sequences]
     mode, ref_mode = tracking_modes(model)
     size_from = {"previous_result": lambda t: 0, "previous_gt": lambda t: t - 1, "current_gt": lambda t: t}[ref_mode]
@@ -56,8 +60,8 @@ def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 <
         for chunk in plan_chunks(lengths, pool_frame_bytes(npts), max_resident_bytes, fixed):
             if all(lengths[j] < 2 for j in chunk):
                 continue
-            trk = BatchedDeviceTracker(model, [sequences[j] for j in chunk], slots, seed=seed, ids=chunk, max_points=npts,
-                                       use_graph=use_graph)
+            trk = BatchedDeviceTracker(model, [sequences[j] for j in chunk], slots, seed=seed, ids=[ids[j] for j in chunk],
+                                       max_points=npts, use_graph=use_graph)
             ov, di, cen, rot = trk.run()
             offsets = trk.plan["offsets"]
             del trk
@@ -74,3 +78,52 @@ def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 <
         prec(distances[j])
     return {"success": succ.compute(), "precision": prec.compute(), "frames": sum(lengths), "results": results,
             "overlaps": overlaps, "distances": distances}
+
+
+def shard_plan(lengths, world):
+    """The tracklets each of `world` ranks evaluates: longest first, each to the rank with the fewest frames so far (ties to
+    the lowest rank), so every tracklet is evaluated exactly once and the ranks' frame counts stay balanced.  Each shard is
+    in ascending index order."""
+    shards, load = [[] for _ in range(world)], [0] * world
+    for j in sorted(range(len(lengths)), key=lambda j: (-lengths[j], j)):
+        r = min(range(world), key=lambda r: (load[r], r))
+        shards[r].append(j)
+        load[r] += lengths[j]
+    return [sorted(s) for s in shards]
+
+
+def gather_shards(n, ids, local):
+    """All ranks' shard results (`local`: evaluate_batched's output over the tracklets `ids`) reassembled in global order on
+    every rank, with Success / Precision over all `n` tracklets accumulated in that order."""
+    import torch.distributed as dist
+    parts = [None] * dist.get_world_size()
+    dist.all_gather_object(parts, (list(ids), local["overlaps"], local["distances"], local["results"]))
+    overlaps, distances, results = [None] * n, [None] * n, [None] * n
+    for ids_r, ov, di, res in parts:
+        for i, j in enumerate(ids_r):
+            if overlaps[j] is not None:
+                raise RuntimeError(f"gather_shards: tracklet {j} was evaluated by two ranks")
+            overlaps[j], distances[j], results[j] = ov[i], di[i], res[i]
+    missing = [j for j in range(n) if overlaps[j] is None]
+    if missing:
+        raise RuntimeError(f"gather_shards: tracklets {missing[:8]} were evaluated by no rank")
+    succ, prec = Success(), Precision()
+    for j in range(n):
+        succ(overlaps[j])
+        prec(distances[j])
+    return {"success": succ.compute(), "precision": prec.compute(), "frames": sum(len(o) for o in overlaps),
+            "results": results, "overlaps": overlaps, "distances": distances}
+
+
+def evaluate_sharded(model, sequences, slots=64, seed=0, **kw):
+    """`evaluate_batched` split across the ranks of a process group (shard_plan): each rank tracks its tracklets with their
+    draws keyed by their index in `sequences`, and every rank returns the whole split's result.  With one rank it is
+    `evaluate_batched`."""
+    from .. import ddp
+    sequences = list(sequences)
+    if not ddp.is_distributed():
+        return evaluate_batched(model, sequences, slots=slots, seed=seed, **kw)
+    import torch.distributed as dist
+    mine = shard_plan([len(s) for s in sequences], dist.get_world_size())[dist.get_rank()]
+    local = evaluate_batched(model, [sequences[j] for j in mine], slots=slots, seed=seed, ids=mine, **kw)
+    return gather_shards(len(sequences), mine, local)
