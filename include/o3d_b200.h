@@ -358,6 +358,22 @@ int o3d_crop_append(const float* scans, const long long* count, const long long*
 int o3d_resample(const float* points, const unsigned char* keep, const float* u_perm, const float* u_pick, int B, int N, int size,
                  int32_t* scratch, float* out, long long* src, long long* n_out, void* stream);
 
+/* Crop + resample of a shared scan for K targets in one kernel (one CTA per target; the live multi-target tracker's crops).
+ * Target k's candidates are [prefix[k, 0 .. Np-1], crop of scans[frame[k]]]: element e < Np is prefix point e (already in the
+ * box frame) when prefix_keep[k, e] != 0; element Np + i is point i of the scan in the frame of box k, kept when
+ * i < count[frame[k]] and |local| < half[k] per axis (o3d_crop_box_frame's test and coordinates, bit for bit).  The result is
+ * o3d_resample of those candidates with the keyed draws of o3d_keyed_uniform: u_perm = stream perm_stream over Np + N elements,
+ * u_pick = stream pick_stream over size elements, both for (seed, key[k], key_frame[k]) — bitwise the same output and survivor
+ * count as crop_box_frame -> keyed_uniform -> resample on the concatenation, without its (K, Np + N) intermediates.
+ * scans [S, N, 3], count [S] int64 or NULL, frame [K] int64, center [K, 3], rot [K, 9], half [K, 3] (all may be NULL when N = 0:
+ * prefix only); prefix [K, Np, 3], prefix_keep [K, Np] bytes (NULL when Np = 0); key / key_frame [K] int64;
+ * scratch [K, 2, Np + N] int32 (written for survivors only); out [K, size, 3]; n_out (nullable) [K] int64.
+ * K <= 65535, 1 <= size <= 2048. */
+int o3d_crop_resample(const float* scans, const long long* count, const long long* frame, const float* center, const float* rot,
+                      const float* half, int N, const float* prefix, const unsigned char* prefix_keep, int Np, unsigned int seed,
+                      const long long* key, const long long* key_frame, int perm_stream, int pick_stream, int K, int size,
+                      int32_t* scratch, float* out, long long* n_out, void* stream);
+
 /* Block 6 — split evaluation with K tracklets in flight (tracking/batched_tracker.py).
  *
  * o3d_keyed_uniform: out [K, n] uniform [0, 1) draws of one stream.  Slot k's element e is a pure function of

@@ -14,23 +14,19 @@
 //   B. 3-pass radix select (11 / 11 / 10 bits, shared-memory histograms) of the size-th smallest key over the survivors,
 //   C. collection of the keys below the threshold (+ ties in index order), bitonic sort of the <= 2048 (key, index) pairs,
 //   D. gather of the selected points.
-#include "common.cuh"
+#include "resample_core.cuh"
 #include "../../include/o3d_b200.h"
 
 namespace {
 
-constexpr int RS_THREADS = 1024;
-constexpr int RS_MAX_SIZE = 2048;
-static_assert(RS_THREADS == 1024, "o3d_block_exscan1024 scans exactly 32 warps");
+constexpr int RS_THREADS = O3D_RS_THREADS;
+constexpr int RS_MAX_SIZE = O3D_RS_MAX_SIZE;
 
 __global__ void __launch_bounds__(RS_THREADS)
     resample_kernel(const float* __restrict__ points, const uint8_t* __restrict__ keep, const float* __restrict__ u_perm,
                     const float* __restrict__ u_pick, int N, int size, int32_t* __restrict__ scratch, float* __restrict__ out,
                     long long* __restrict__ src, long long* __restrict__ n_out) {
-    __shared__ unsigned long long s_sel[RS_MAX_SIZE];
-    __shared__ uint32_t s_hist[2048];
-    __shared__ uint32_t s_warp[32];
-    __shared__ uint32_t s_digit, s_krem, s_eq, s_cnt;
+    __shared__ O3dResampleSmem sm;
 
     const int b = blockIdx.x, tid = threadIdx.x;
     const float* __restrict__ P = points + (size_t)b * N * 3;
@@ -62,7 +58,7 @@ __global__ void __launch_bounds__(RS_THREADS)
     uint32_t cnt = 0;
     for (int i = beg; i < end; i += 4) cnt += __popc(flags4(i));
     uint32_t n;
-    uint32_t pos = o3d_block_exscan1024(cnt, s_warp, n);
+    uint32_t pos = o3d_block_exscan1024(cnt, sm.warp, n);
     for (int i = beg; i < end; i += 4) {
         const uint32_t f = flags4(i);
 #pragma unroll
@@ -75,15 +71,7 @@ __global__ void __launch_bounds__(RS_THREADS)
     if ((int)n < size || n <= 2) {
         // ---- with replacement (2 < n < size) / placeholder (n <= 2)
         for (int i = tid; i < size; i += RS_THREADS) {
-            long long w;
-            if (n == 0) {
-                w = N - 1;
-            } else {
-                long long r = (long long)(UP[i] * (float)n);
-                if (r > (long long)n - 1) r = (long long)n - 1;
-                if (r < 0) r = 0;
-                w = S[r];
-            }
+            const long long w = n == 0 ? N - 1 : S[o3d_pick_rank(UP[i], n)];
             SRC[i] = w;
             const bool zero = n <= 2;
             O[i * 3 + 0] = zero ? 0.f : P[w * 3 + 0];
@@ -92,101 +80,16 @@ __global__ void __launch_bounds__(RS_THREADS)
         }
         return;
     }
-
-    // ---- B. radix select: the size-th smallest key among the n survivors (keys are floats in [0, 1): bit patterns are monotone)
-    uint32_t prefix = 0, krem = (uint32_t)size, eq_total = 0;
-    if ((int)n > size) {
-        const int shifts[3] = {21, 10, 0}, bits[3] = {11, 11, 10};
-        for (int pass = 0; pass < 3; ++pass) {
-            const int sh = shifts[pass], nb = bits[pass];
-            for (int i = tid; i < 2048; i += RS_THREADS) s_hist[i] = 0;
-            __syncthreads();
-            for (uint32_t s = tid; s < n; s += RS_THREADS) {
-                const uint32_t key = __float_as_uint(U[S[s]]);
-                if (pass == 0 || (key >> (sh + nb)) == prefix) atomicAdd(&s_hist[(key >> sh) & ((1u << nb) - 1u)], 1u);
-            }
-            __syncthreads();
-            const uint32_t h0 = s_hist[2 * tid], h1 = s_hist[2 * tid + 1];
-            uint32_t total;
-            const uint32_t ex = o3d_block_exscan1024(h0 + h1, s_warp, total);
-            if (ex < krem && krem <= ex + h0) {
-                s_digit = 2 * tid; s_krem = krem - ex; s_eq = h0;
-            } else if (ex + h0 < krem && krem <= ex + h0 + h1) {
-                s_digit = 2 * tid + 1; s_krem = krem - ex - h0; s_eq = h1;
-            }
-            __syncthreads();
-            prefix = (prefix << nb) | s_digit;
-            krem = s_krem;
-            eq_total = s_eq;
-            __syncthreads();
-        }
-    }
-    // ---- C. collect: keys below the threshold, then `krem` of the keys equal to it (index order when there are more)
-    const bool all = (int)n == size;
-    if (tid == 0) s_cnt = 0;
-    __syncthreads();
-    const uint32_t n_less = all ? n : (uint32_t)size - krem;
-    for (uint32_t s = tid; s < n; s += RS_THREADS) {
-        const uint32_t idx = (uint32_t)S[s];
-        const uint32_t key = __float_as_uint(U[idx]);
-        if (all || key < prefix) {
-            const uint32_t p = atomicAdd(&s_cnt, 1u);
-            s_sel[p] = ((unsigned long long)key << 32) | idx;
-        }
-    }
-    if (!all) {
-        if (eq_total == krem) {
-            for (uint32_t s = tid; s < n; s += RS_THREADS) {
-                const uint32_t idx = (uint32_t)S[s];
-                const uint32_t key = __float_as_uint(U[idx]);
-                if (key == prefix) {
-                    const uint32_t p = atomicAdd(&s_cnt, 1u);
-                    s_sel[p] = ((unsigned long long)key << 32) | idx;
-                }
-            }
-        } else {
-            // more equal keys than places: the first `krem` in index order (ordered block scan over the survivors)
-            uint32_t taken = 0;
-            for (uint32_t s0 = 0; s0 < n && taken < krem; s0 += RS_THREADS) {
-                const uint32_t s = s0 + tid;
-                uint32_t idx = 0, hit = 0;
-                if (s < n) {
-                    idx = (uint32_t)S[s];
-                    hit = __float_as_uint(U[idx]) == prefix;
-                }
-                uint32_t total;
-                const uint32_t r = taken + o3d_block_exscan1024(hit, s_warp, total);
-                if (hit && r < krem) s_sel[n_less + r] = ((unsigned long long)prefix << 32) | idx;
-                taken += total;
-            }
-        }
-    }
-    int P2 = 1;
-    while (P2 < size) P2 <<= 1;
-    for (int i = size + tid; i < P2; i += RS_THREADS) s_sel[i] = ~0ull;
-    __syncthreads();
-    // bitonic sort, ascending (key, index)
-    for (int k = 2; k <= P2; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = tid; i < P2; i += RS_THREADS) {
-                const int x = i ^ j;
-                if (x > i) {
-                    const unsigned long long a = s_sel[i], c = s_sel[x];
-                    const bool up = (i & k) == 0;
-                    if ((a > c) == up) { s_sel[i] = c; s_sel[x] = a; }
-                }
-            }
-            __syncthreads();
-        }
-    }
-    // ---- D. gather
-    for (int i = tid; i < size; i += RS_THREADS) {
-        const uint32_t idx = (uint32_t)(s_sel[i] & 0xFFFFFFFFull);
-        SRC[i] = idx;
-        O[i * 3 + 0] = P[(size_t)idx * 3 + 0];
-        O[i * 3 + 1] = P[(size_t)idx * 3 + 1];
-        O[i * 3 + 2] = P[(size_t)idx * 3 + 2];
-    }
+    // ---- B-D. select the `size` smallest keys, sort them, gather (resample_core.cuh)
+    o3d_resample_select(
+        n, size, S, [&](uint32_t s) { return __float_as_uint(U[S[s]]); },
+        [&](int i, uint32_t idx) {
+            SRC[i] = idx;
+            O[i * 3 + 0] = P[(size_t)idx * 3 + 0];
+            O[i * 3 + 1] = P[(size_t)idx * 3 + 1];
+            O[i * 3 + 2] = P[(size_t)idx * 3 + 2];
+        },
+        sm);
 }
 
 }  // namespace

@@ -8,29 +8,10 @@
 // o3d_track_metrics  — utils/metrics.py estimateOverlap / estimateAccuracy (reference utils/metrics.py:27-60) in fp64 for
 //                      one (result box, ground truth) pair per slot.  Every operation is an explicit round-to-nearest
 //                      intrinsic: the build contracts a*b+c into FMAs by default, and the host restatement does not.
-#include "common.cuh"
+#include "resample_core.cuh"          // o3d_philox4x32_10, o3d_word_to_uniform
 #include "../../include/o3d_b200.h"
 
 namespace {
-
-constexpr uint32_t kPhiloxM0 = 0xD2511F53u, kPhiloxM1 = 0xCD9E8D57u;
-constexpr uint32_t kPhiloxW0 = 0x9E3779B9u, kPhiloxW1 = 0xBB67AE85u;
-
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        if (r) {
-            k0 += kPhiloxW0;
-            k1 += kPhiloxW1;
-        }
-        const uint32_t hi0 = __umulhi(kPhiloxM0, c.x), lo0 = kPhiloxM0 * c.x;
-        const uint32_t hi1 = __umulhi(kPhiloxM1, c.z), lo1 = kPhiloxM1 * c.z;
-        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-    }
-    return c;
-}
-
-__device__ __forceinline__ float word_to_uniform(uint32_t w) { return (float)(w >> 8) * 5.9604644775390625e-8f; }  // 2^-24
 
 // thread = one Philox block = four consecutive elements of one slot's stream
 __global__ void __launch_bounds__(256)
@@ -42,16 +23,16 @@ __global__ void __launch_bounds__(256)
     float* __restrict__ row = out + (size_t)k * n;
     const int blocks = (n + 3) >> 2;
     for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < blocks; b += gridDim.x * blockDim.x) {
-        const uint4 w = philox4x32_10(make_uint4((uint32_t)b, fr, stream, 0u), seed, key1);
+        const uint4 w = o3d_philox4x32_10(make_uint4((uint32_t)b, fr, stream, 0u), seed, key1);
         const int e = b << 2;
         if (e + 3 < n) {
-            row[e + 0] = word_to_uniform(w.x);
-            row[e + 1] = word_to_uniform(w.y);
-            row[e + 2] = word_to_uniform(w.z);
-            row[e + 3] = word_to_uniform(w.w);
+            row[e + 0] = o3d_word_to_uniform(w.x);
+            row[e + 1] = o3d_word_to_uniform(w.y);
+            row[e + 2] = o3d_word_to_uniform(w.z);
+            row[e + 3] = o3d_word_to_uniform(w.w);
         } else {
             const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
-            for (int j = 0; e + j < n; ++j) row[e + j] = word_to_uniform(ws[j]);
+            for (int j = 0; e + j < n; ++j) row[e + j] = o3d_word_to_uniform(ws[j]);
         }
     }
 }

@@ -136,26 +136,10 @@ class kittiDataset(BaseDataset):
     def _get_frame_from_anno(self, anno):
         """kitti.py:144-188."""
         scene_id, frame_id = anno['scene'], anno['frame']
-        if scene_id not in self.calibs:
-            self.calibs[scene_id] = self._read_calib_file(os.path.join(self.KITTI_calib, scene_id + ".txt"))
-        velo_to_cam = np.vstack((self.calibs[scene_id]["Tr_velo_cam"], np.array([0, 0, 0, 1])))
-        size = [anno["width"], anno["length"], anno["height"]]
-        if self.coordinate_mode == 'velodyne':
-            center_cam = np.array([anno["x"], anno["y"] - anno["height"] / 2, anno["z"], 1])
-            center = (np.linalg.inv(velo_to_cam) @ center_cam)[:3]
-            rot = _rotz(-anno["rotation_y"]) @ _rotz(-np.pi / 2)
-        else:
-            center = [anno["x"], anno["y"] - anno["height"] / 2, anno["z"]]
-            rot = _rot([0, 1, 0], anno["rotation_y"]) @ _rot([1, 0, 0], np.pi / 2)
-        bb = Box(center, size, rot)
+        bb = self.box_from_anno(anno)
         try:
             if frame_id not in self.velos[scene_id]:
-                path = os.path.join(self.KITTI_velo, scene_id, '{:06}.bin'.format(frame_id))
-                pts = np.fromfile(path, dtype=np.float32).reshape(-1, 4).T
-                pc = PointCloud(pts)
-                if self.coordinate_mode == "camera":
-                    pc.points = (velo_to_cam @ np.vstack((pc.points[:3], np.ones(pc.points.shape[1]))))[:3]
-                self.velos[scene_id][frame_id] = pc
+                self.velos[scene_id][frame_id] = self._read_scan(scene_id, frame_id)
             pc = self.velos[scene_id][frame_id]
             if self.preload_offset > 0:                       # crop_pc_axis_aligned(pc, bb, offset=preload_offset)
                 c = bb.corners()
@@ -165,6 +149,42 @@ class kittiDataset(BaseDataset):
         except (OSError, ValueError):
             pc = PointCloud(np.array([[0, 0, 0]], dtype=np.float32).T)
         return {"pc": pc, "3d_bbox": bb, 'meta': anno}
+
+    def _velo_to_cam(self, scene_id):
+        if scene_id not in self.calibs:
+            self.calibs[scene_id] = self._read_calib_file(os.path.join(self.KITTI_calib, scene_id + ".txt"))
+        return np.vstack((self.calibs[scene_id]["Tr_velo_cam"], np.array([0, 0, 0, 1])))
+
+    def box_from_anno(self, anno):
+        """The label's box in the reader's coordinate_mode (kitti.py:150-163), without loading the scan."""
+        velo_to_cam = self._velo_to_cam(anno['scene'])
+        size = [anno["width"], anno["length"], anno["height"]]
+        if self.coordinate_mode == 'velodyne':
+            center_cam = np.array([anno["x"], anno["y"] - anno["height"] / 2, anno["z"], 1])
+            center = (np.linalg.inv(velo_to_cam) @ center_cam)[:3]
+            rot = _rotz(-anno["rotation_y"]) @ _rotz(-np.pi / 2)
+        else:
+            center = [anno["x"], anno["y"] - anno["height"] / 2, anno["z"]]
+            rot = _rot([0, 1, 0], anno["rotation_y"]) @ _rot([1, 0, 0], np.pi / 2)
+        return Box(center, size, rot)
+
+    def _read_scan(self, scene_id, frame_id):
+        pts = np.fromfile(self.scan_path(scene_id, frame_id), dtype=np.float32).reshape(-1, 4).T
+        pc = PointCloud(pts)
+        if self.coordinate_mode == "camera":
+            pc.points = (self._velo_to_cam(scene_id) @ np.vstack((pc.points[:3], np.ones(pc.points.shape[1]))))[:3]
+        return pc
+
+    def scan_path(self, scene_id, frame_id):
+        return os.path.join(self.KITTI_velo, scene_id, '{:06}.bin'.format(frame_id))
+
+    def read_scan(self, scene_id, frame_id):
+        """The whole scan of a frame in the reader's coordinate_mode, not cached and not cropped (a missing or unreadable
+        file gives the reader's one-point placeholder)."""
+        try:
+            return self._read_scan(scene_id, frame_id)
+        except (OSError, ValueError):
+            return PointCloud(np.array([[0, 0, 0]], dtype=np.float32).T)
 
     @staticmethod
     def _read_calib_file(filepath):

@@ -195,3 +195,34 @@ def synthetic_sequence(n_frames=8, n_points=20000, seed=20260924, wlh=CAR_WLH, s
         center = center + speed * np.array([c, s, 0.0])
         yaw = yaw + np.deg2rad(yaw_rate)
     return frames
+
+
+def synthetic_scene(n_frames=8, n_points=60000, n_objects=8, seed=20260924, wlh=CAR_WLH, n_object=300, extent=60.0):
+    """A scan stream with several moving boxes: {"scans": [(n_points, 3) float32 per frame], "boxes": [[Box per frame] per
+    object]}.  Objects start on a grid over [-extent, extent]^2, each with its own heading, speed and turn rate; every scan has
+    `n_object` surface points per object over ground + clutter returns (points inside any box removed), `n_points` in all."""
+    from .data_classes import Box
+    rng = np.random.default_rng(seed)
+    side = int(np.ceil(np.sqrt(n_objects)))
+    cells = np.linspace(-extent * 0.8, extent * 0.8, side) if side > 1 else np.zeros(1)
+    z0 = -0.8 + wlh[2] / 2
+    state = [(np.array([cells[i % side] + rng.uniform(-2, 2), cells[i // side] + rng.uniform(-2, 2), z0]),
+              rng.uniform(-np.pi, np.pi), rng.uniform(0.2, 0.8), np.deg2rad(rng.uniform(-3, 3))) for i in range(n_objects)]
+    n_bg = max(n_points - n_objects * n_object, 0)
+    ground = np.stack([rng.uniform(-extent, extent, n_bg), rng.uniform(-extent, extent, n_bg), np.full(n_bg, -0.8)], 1)
+    clutter = rng.uniform([-extent, -extent, -0.8], [extent, extent, 2.0], size=(n_bg // 10, 3))
+    scans, boxes = [], [[] for _ in range(n_objects)]
+    for _ in range(n_frames):
+        objs, bg = [], np.concatenate([ground + rng.normal(0, 0.01, ground.shape), clutter])
+        for i, (center, yaw, speed, turn) in enumerate(state):
+            c, s = np.cos(yaw), np.sin(yaw)
+            rot = np.array([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]])
+            objs.append(_surface_points(rng, n_object, wlh) @ rot.T + center[None])
+            bg = bg[~_in_box(bg, center, np.asarray(wlh) * 1.05, yaw)]
+            boxes[i].append(Box(center.copy(), wlh, rot.copy()))
+            state[i] = (center + speed * np.array([c, s, 0.0]), yaw + turn, speed, turn)
+        pts = np.concatenate(objs + [bg])[:n_points]
+        if pts.shape[0] < n_points:
+            pts = np.concatenate([pts, bg[rng.integers(0, len(bg), n_points - pts.shape[0])]])
+        scans.append(pts.astype(np.float32))
+    return {"scans": scans, "boxes": boxes}

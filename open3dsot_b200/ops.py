@@ -268,6 +268,44 @@ def crop_append(scans, center, rot, half, frame, count, hist, hist_keep, hist_co
           rot.data_ptr(), half.data_ptr(), B, N, H, hist.data_ptr(), hist_keep.data_ptr(), hist_count.data_ptr(), _stream())
 
 
+def _chk_i64(t, name):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.int64 or not t.is_contiguous():
+        raise RuntimeError(f"{name} must be a contiguous int64 CUDA tensor")
+
+
+def crop_resample(scans, count, frame, center, rot, half, size, seed, key, key_frame, perm_stream, pick_stream, prefix=None,
+                  prefix_keep=None):
+    """Crop of a shared scan per target, resampled to `size` points, in one kernel (csrc/crop_resample.cu): scans (S, N, 3) fp32
+    CUDA, count (S,) int64 or None, frame (K,) int64 picks each target's scan; center (K, 3), rot (K, 3, 3), half (K, 3) as
+    `crop_box_frame` takes them; prefix (K, Np, 3) fp32 / prefix_keep (K, Np) bool: candidates already in the box frame that come
+    before the crop; key / key_frame (K,) int64 and the perm / pick stream ids key the draws as `keyed_uniform` does.
+    Returns out (K, size, 3) and the survivor counts (K,) int64, bitwise equal to `crop_box_frame` -> `keyed_uniform` ->
+    `resample` on the concatenation [prefix, crop]."""
+    _chk_f(scans, "scans")
+    _, N, _ = scans.shape
+    K = key.shape[0]
+    for t, name in ((key, "key"), (key_frame, "key_frame")) + ((frame, "frame"),) + (() if count is None else ((count, "count"),)):
+        _chk_i64(t, name)
+    assert key_frame.shape == (K,) and frame.shape == (K,)
+    center, rot, half = (t.contiguous().float() for t in (center, rot, half))
+    assert center.shape == (K, 3) and rot.shape == (K, 3, 3) and half.shape == (K, 3)
+    Np = 0
+    if prefix is not None:
+        _chk_f(prefix, "prefix")
+        Np = prefix.shape[1]
+        assert prefix.shape == (K, Np, 3) and prefix_keep.shape == (K, Np) and prefix_keep.dtype == torch.bool
+        assert prefix_keep.is_contiguous()
+    dev = scans.device
+    scratch = torch.empty(K, 2, Np + N, dtype=torch.int32, device=dev)
+    out = torch.empty(K, int(size), 3, device=dev)
+    n = torch.empty(K, dtype=torch.int64, device=dev)
+    _call("o3d_crop_resample", scans.data_ptr(), None if count is None else count.data_ptr(), frame.data_ptr(), center.data_ptr(),
+          rot.data_ptr(), half.data_ptr(), N, None if prefix is None else prefix.data_ptr(),
+          None if prefix is None else prefix_keep.data_ptr(), Np, int(seed) & 0xFFFFFFFF, key.data_ptr(), key_frame.data_ptr(),
+          int(perm_stream), int(pick_stream), K, int(size), scratch.data_ptr(), out.data_ptr(), n.data_ptr(), _stream())
+    return out, n
+
+
 # ------------------------------------------------------------------ split evaluation, K tracklets in flight (tracking/batched_tracker.py)
 def keyed_uniform(tracklet, frame, seed, stream, n, out=None):
     """Counter-based uniform [0, 1) draws (csrc/track_eval.cu): tracklet (K,) / frame (K,) int64 CUDA -> out (K, n) fp32, row k a pure

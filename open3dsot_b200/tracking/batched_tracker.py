@@ -32,6 +32,34 @@ from .sampling import resample_batched
 STREAM_SEARCH_PERM, STREAM_SEARCH_PICK, STREAM_TEMPLATE_PERM, STREAM_TEMPLATE_PICK, STREAM_LIMIT_BOX = range(5)
 
 
+def canonical(box):
+    """The slots' boxes moved to the origin, axis-aligned (the frame the template / previous points are expressed in)."""
+    return bx.Box(torch.zeros_like(box.center), box.wlh, torch.eye(3, device=box.center.device).expand_as(box.rot))
+
+
+def motion_data(cfg, box, prev_pts, this_pts, first_flag):
+    """DeviceTracker._inputs_motion's input dict with a slot dimension, from the resampled previous / current crops (K, n, 3):
+    the previous points masked 1 / 0 by the box on the first frame (first_flag (K,) = 1), 0.8 / 0.2 afterwards."""
+    half = torch.stack([box.wlh[:, 1], box.wlh[:, 0], box.wlh[:, 2]], -1) * (1.25 / 2)
+    inside = (prev_pts.abs() <= half[:, None, :]).all(-1).float()
+    first = first_flag[:, None]
+    mask_prev = inside * (0.6 + 0.4 * first) + 0.2 * (1 - first)             # 1 / 0 on the first frame, 0.8 / 0.2 afterwards
+    col = lambda pts, t, m: torch.cat([pts, torch.full_like(pts[..., :1], t), m[..., None]], -1)
+    data = {"points": torch.cat([col(prev_pts, 0.0, mask_prev), col(this_pts, 0.1, torch.full_like(mask_prev, 0.5))], 1)}
+    if getattr(cfg, "box_aware", False):
+        bc = bx.point_to_box_distance(prev_pts, canonical(box))
+        data["candidate_bc"] = torch.cat([bc, torch.zeros_like(bc)], 1)
+    return data
+
+
+def best_proposal(est):
+    """(K, num_proposal, 5) proposals -> (K, 4) offsets of the highest-scoring one per slot; (K, 4) passes through."""
+    if est.dim() == 3:
+        best = est[:, :, 4].argmax(1)
+        est = est.gather(1, best[:, None, None].expand(-1, 1, est.shape[-1]))[:, 0, :4]
+    return est
+
+
 def plan_schedule(lengths, slots):
     """Slot schedule of one chunk.  `lengths`: frames per tracklet, in pool order.  Tracklets are admitted longest first
     (ties in input order), each into the slot that frees first (lowest slot on ties); a tracklet of n frames holds its slot
@@ -165,19 +193,10 @@ class BatchedDeviceTracker:
         t_local, t_keep = bx.crop_in_box_frame(P.scans, box, cfg.bb_scale, cfg.bb_offset, f, P.count)
         prev_pts, _, _ = resample_batched(p_local, p_keep, n, self.u_t[0][:, :N], self.u_t[1])
         this_pts, _, _ = resample_batched(t_local, t_keep, n, self.u_s[0], self.u_s[1])
-        half = torch.stack([box.wlh[:, 1], box.wlh[:, 0], box.wlh[:, 2]], -1) * (1.25 / 2)
-        inside = (prev_pts.abs() <= half[:, None, :]).all(-1).float()
-        first = self.first_flag[:, None]
-        mask_prev = inside * (0.6 + 0.4 * first) + 0.2 * (1 - first)         # 1 / 0 on the first frame, 0.8 / 0.2 afterwards
-        col = lambda pts, t, m: torch.cat([pts, torch.full_like(pts[..., :1], t), m[..., None]], -1)
-        data = {"points": torch.cat([col(prev_pts, 0.0, mask_prev), col(this_pts, 0.1, torch.full_like(mask_prev, 0.5))], 1)}
-        if getattr(cfg, "box_aware", False):
-            bc = bx.point_to_box_distance(prev_pts, self._canon(box))
-            data["candidate_bc"] = torch.cat([bc, torch.zeros_like(bc)], 1)
-        return data
+        return motion_data(cfg, box, prev_pts, this_pts, self.first_flag)
 
     def _canon(self, box):
-        return bx.Box(torch.zeros_like(box.center), box.wlh, torch.eye(3, device=self.dev).expand_as(box.rot))
+        return canonical(box)
 
     def _inputs(self, f, box, ref, active):
         """DeviceTracker._inputs with a slot dimension: `box` the slots' result boxes, `ref` their reference boxes."""
@@ -218,10 +237,7 @@ class BatchedDeviceTracker:
                 ref = box
             else:
                 ref = P.box(P.prev[f] if self.ref_mode == "previous_gt" else f)
-            est = self.model(self._inputs(f, box, ref, active))["estimation_boxes"]   # (K, num_proposal, 5) or (K, 4)
-            if est.dim() == 3:
-                best = est[:, :, 4].argmax(1)
-                est = est.gather(1, best[:, None, None].expand(-1, 1, est.shape[-1]))[:, 0, :4]
+            est = best_proposal(self.model(self._inputs(f, box, ref, active))["estimation_boxes"])
             new = bx.offset_box(ref, est, degrees=cfg.degrees, use_z=cfg.use_z, limit_box=cfg.limit_box, rand=self.u_lim * 2 - 1)
             self.box_c.copy_(new.center)
             self.box_r.copy_(new.rot)
