@@ -374,6 +374,28 @@ int o3d_crop_resample(const float* scans, const long long* count, const long lon
                       const long long* key, const long long* key_frame, int perm_stream, int pick_stream, int K, int size,
                       int32_t* scratch, float* out, long long* n_out, void* stream);
 
+/* Scan ingest for the live tracker's feeds (one sensor or recorded scene each): every feed that gets a new scan this step hands
+ * its raw point rows, as stored, and the reader's affine transforms; one launch writes them all as float32 xyz.
+ * Descriptor i: rows [rows, stride] of float32 (is_f64 = 0) or float64 (is_f64 = 1) at byte `offset` of the slab, x y z first;
+ * each row is moved through xf[0], then xf[1] (the first n_xf of them; row-major 3x4 [R | t]: p <- R p + t) in float64 and written
+ * to scans[feed, half, 0 .. rows-1] as float32; count[feed, half] = rows.
+ * desc_host: the descriptors in host memory, checked before the launch; desc: the same n_desc descriptors in device memory (the
+ * kernel reads these).  scans [feeds, 2, max_points, 3] fp32, count [feeds, 2] int64.  Checks: feed in [0, feeds), half 0 / 1,
+ * stride in [3, 16], n_xf in [0, 2], rows in [0, max_points], the rows inside [0, slab_bytes) at an element-aligned offset, no two
+ * descriptors with the same (feed, half), n_desc <= 2 * feeds.  n_desc = 0: nothing is launched. */
+typedef struct {
+    long long offset;  /* byte offset of the first row in the slab */
+    int rows;          /* number of rows (points) */
+    int stride;        /* values per row */
+    int is_f64;        /* 0: float32 rows, 1: float64 rows */
+    int feed;          /* destination feed */
+    int half;          /* destination half of the feed's ping-pong pair */
+    int n_xf;          /* transforms applied, in order */
+    double xf[2][12];  /* row-major 3x4 [R | t] */
+} o3d_scan_desc_t;
+int o3d_scan_ingest(const o3d_scan_desc_t* desc_host, const o3d_scan_desc_t* desc, int n_desc, const void* slab, long long slab_bytes,
+                    int feeds, int max_points, float* scans, long long* count, void* stream);
+
 /* Block 6 — split evaluation with K tracklets in flight (tracking/batched_tracker.py).
  *
  * o3d_keyed_uniform: out [K, n] uniform [0, 1) draws of one stream.  Slot k's element e is a pure function of

@@ -178,6 +178,36 @@ class kittiDataset(BaseDataset):
     def scan_path(self, scene_id, frame_id):
         return os.path.join(self.KITTI_velo, scene_id, '{:06}.bin'.format(frame_id))
 
+    # ---- the per-reader interface of the live tracking command line (track.py): scenes, their scans, their raw point rows
+    def scene_frames(self, scene_id):
+        """The frame numbers of a scene's scans, in order: 0 .. its last velodyne file or labelled frame."""
+        d = os.path.join(self.KITTI_velo, scene_id)
+        names = os.listdir(d) if os.path.isdir(d) else []
+        last = max((int(n[:-4]) for n in names if n.endswith(".bin") and n[:-4].isdigit()), default=-1)
+        for annos in self.tracklet_anno_list:
+            if annos[0]["scene"] == scene_id:
+                last = max(last, annos[-1]["frame"])
+        return list(range(last + 1))
+
+    @staticmethod
+    def anno_frame(anno):
+        """(scene, frame) of an annotation."""
+        return anno["scene"], anno["frame"]
+
+    def scan_size(self, scene_id, frame_id):
+        """Points in a frame's scan, from the file size (16 bytes per point; 1 for the placeholder of a missing file)."""
+        path = self.scan_path(scene_id, frame_id)
+        return max(os.path.getsize(path) // 16, 1) if os.path.isfile(path) else 1
+
+    def raw_scan(self, scene_id, frame_id):
+        """The scan's rows as stored ((n, 4) float32: x, y, z, reflectance) and the transforms `read_scan` applies to them:
+        none in velodyne mode, Tr_velo_cam (3x4) in camera mode.  A missing or unreadable file gives the placeholder point."""
+        try:
+            rows = np.fromfile(self.scan_path(scene_id, frame_id), dtype=np.float32).reshape(-1, 4)
+            return rows, ([self._velo_to_cam(scene_id)[:3]] if self.coordinate_mode == "camera" else [])
+        except (OSError, ValueError):
+            return np.zeros((1, 3), np.float32), []
+
     def read_scan(self, scene_id, frame_id):
         """The whole scan of a frame in the reader's coordinate_mode, not cached and not cropped (a missing or unreadable
         file gives the reader's one-point placeholder)."""

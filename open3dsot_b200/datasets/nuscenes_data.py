@@ -155,16 +155,72 @@ class NuScenesDataset(BaseDataset):
 
     def _get_frame_from_anno_data(self, anno):
         """nuscenes_data.py:152-173."""
-        sd, box_anno = anno['sample_data_lidar'], anno['box_anno']
-        bb = Box(box_anno['translation'], box_anno['size'], quat_to_rot(box_anno['rotation']))
-        scan = np.fromfile(os.path.join(self.path, sd['filename']), dtype=np.float32).reshape(-1, 5)[:, :3].T.astype(np.float64)
-        cs = self.nusc.get('calibrated_sensor', sd['calibrated_sensor_token'])
-        scan = quat_to_rot(cs['rotation']) @ scan + np.array(cs['translation'])[:, None]                 # sensor -> ego
-        pose = self.nusc.get('ego_pose', sd['ego_pose_token'])
-        scan = quat_to_rot(pose['rotation']) @ scan + np.array(pose['translation'])[:, None]             # ego -> global
-        pc = PointCloud(scan.astype(np.float32))
+        bb = self.box_from_anno(anno)
+        pc = self._global_scan(anno['sample_data_lidar'])
         if self.preload_offset > 0:                               # crop_pc_axis_aligned(pc, bb, offset=preload_offset)
             c = bb.corners()
             lo, hi = c.min(1) - self.preload_offset, c.max(1) + self.preload_offset
             pc = PointCloud(pc.points[:, ((pc.points > lo[:, None]) & (pc.points < hi[:, None])).all(0)])
         return {"pc": pc, "3d_bbox": bb, 'meta': anno}
+
+    def _global_scan(self, sd):
+        """A LiDAR sample_data's whole scan, sensor -> ego -> global (nuscenes_data.py:159-167)."""
+        scan = np.fromfile(os.path.join(self.path, sd['filename']), dtype=np.float32).reshape(-1, 5)[:, :3].T.astype(np.float64)
+        cs = self.nusc.get('calibrated_sensor', sd['calibrated_sensor_token'])
+        scan = quat_to_rot(cs['rotation']) @ scan + np.array(cs['translation'])[:, None]                 # sensor -> ego
+        pose = self.nusc.get('ego_pose', sd['ego_pose_token'])
+        scan = quat_to_rot(pose['rotation']) @ scan + np.array(pose['translation'])[:, None]             # ego -> global
+        return PointCloud(scan.astype(np.float32))
+
+    @staticmethod
+    def box_from_anno(anno):
+        """The annotation's box, as annotated in the global frame."""
+        box_anno = anno['box_anno']
+        return Box(box_anno['translation'], box_anno['size'], quat_to_rot(box_anno['rotation']))
+
+    # ---- the per-reader interface of the live tracking command line (track.py): scenes, their scans, their raw point rows
+    @property
+    def scene_list(self):
+        """The split's scenes, in the scene table's order."""
+        return [s['name'] for s in self.nusc.t['scene'] if s['name'] in self._scenes]
+
+    def _scene_scans(self, scene):
+        """A scene's key-frame LIDAR_TOP sample_data records in timestamp order (the only scans the tracklets refer to)."""
+        if not hasattr(self, '_scans_of'):
+            self._scans_of = {}
+            token_of = {s['token']: s['name'] for s in self.nusc.t['scene']}
+            for smp in self.nusc.t['sample']:
+                if 'LIDAR_TOP' in smp['data']:
+                    self._scans_of.setdefault(token_of[smp['scene_token']], []).append(
+                        self.nusc.get('sample_data', smp['data']['LIDAR_TOP']))
+            for sds in self._scans_of.values():
+                sds.sort(key=lambda sd: sd['timestamp'])
+            self._frame_of = {sd['token']: i for sds in self._scans_of.values() for i, sd in enumerate(sds)}
+        return self._scans_of.get(scene, [])
+
+    def scene_frames(self, scene):
+        """A scene's frames: the positions 0 .. n-1 of its key-frame scans in timestamp order."""
+        return list(range(len(self._scene_scans(scene))))
+
+    def anno_frame(self, anno):
+        """(scene, frame) of an annotation."""
+        sd = anno['sample_data_lidar']
+        scene = self.nusc.get('scene', self.nusc.get('sample', sd['sample_token'])['scene_token'])['name']
+        self._scene_scans(scene)
+        return scene, self._frame_of[sd['token']]
+
+    def scan_size(self, scene, frame):
+        """Points in a frame's scan, from the file size (20 bytes per point)."""
+        return os.path.getsize(os.path.join(self.path, self._scene_scans(scene)[frame]['filename'])) // 20
+
+    def raw_scan(self, scene, frame):
+        """The scan's rows as stored ((n, 5) float32) and its two transforms, sensor -> ego then ego -> global (3x4 each)."""
+        sd = self._scene_scans(scene)[frame]
+        rows = np.fromfile(os.path.join(self.path, sd['filename']), dtype=np.float32).reshape(-1, 5)
+        cs = self.nusc.get('calibrated_sensor', sd['calibrated_sensor_token'])
+        pose = self.nusc.get('ego_pose', sd['ego_pose_token'])
+        return rows, [np.hstack([quat_to_rot(r['rotation']), np.array(r['translation'], np.float64)[:, None]]) for r in (cs, pose)]
+
+    def read_scan(self, scene, frame):
+        """A frame's whole scan in the global frame, as `get_frames` gives it with preload_offset=-1."""
+        return self._global_scan(self._scene_scans(scene)[frame])

@@ -10,6 +10,7 @@ width / length swapped into the (w, l, h) order and a rotation of -heading about
 this convention), then rotated and translated into the global frame."""
 import os
 import pickle
+import re
 
 import numpy as np
 
@@ -71,19 +72,95 @@ class WaymoDataset(BaseDataset):
         return [self.get_frames(i, range(n)) for i, n in enumerate(self.tracklet_len_list)]
 
     def _get_frame_from_anno(self, anno, track_id=None):
-        lidar_path = anno['PC']
-        gt = np.array(anno['Box'], dtype=np.float64)
-        with open(lidar_path, 'rb') as f:
-            pts = np.asarray(pickle.load(f)['lidars']['points_xyz'], dtype=np.float64).T            # (3, N), vehicle frame
-        with open(lidar_path.replace('lidar', 'annos'), 'rb') as f:
-            pose = np.reshape(pickle.load(f)['veh_to_global'], [4, 4]).astype(np.float64)
-        R, t = pose[:3, :3], pose[:3, 3]                                                              # veh_pos_to_transform (:170-208)
-        pts = R @ pts + t[:, None]
-        size = [gt[4], gt[3], gt[5]]                                                                  # (l, w, h) -> (w, l, h)
-        bb = Box(R @ gt[0:3] + t, size, R @ _rotz(-gt[-1]))
-        pc = PointCloud(pts.astype(np.float32))
+        bb = self.box_from_anno(anno)
+        pc = self._global_scan(anno['PC'])
         if self.preload_offset > 0:
             c = bb.corners()
             lo, hi = c.min(1) - self.preload_offset, c.max(1) + self.preload_offset
             pc = PointCloud(pc.points[:, ((pc.points > lo[:, None]) & (pc.points < hi[:, None])).all(0)])
         return {"pc": pc, "3d_bbox": bb, 'meta': anno}
+
+    @staticmethod
+    def _pose(lidar_path):
+        with open(lidar_path.replace('lidar', 'annos'), 'rb') as f:
+            return np.reshape(pickle.load(f)['veh_to_global'], [4, 4]).astype(np.float64)
+
+    @staticmethod
+    def _stored_points(lidar_path):
+        with open(lidar_path, 'rb') as f:
+            return pickle.load(f)['lidars']['points_xyz']
+
+    def _global_scan(self, lidar_path):
+        """A frame's whole scan, vehicle -> global (waymo_data.py:121-168)."""
+        pts = np.asarray(self._stored_points(lidar_path), dtype=np.float64).T                      # (3, N), vehicle frame
+        pose = self._pose(lidar_path)
+        R, t = pose[:3, :3], pose[:3, 3]                                                              # veh_pos_to_transform (:170-208)
+        return PointCloud((R @ pts + t[:, None]).astype(np.float32))
+
+    def box_from_anno(self, anno):
+        """The annotation's box in the global frame."""
+        gt = np.array(anno['Box'], dtype=np.float64)
+        pose = self._pose(anno['PC'])
+        R, t = pose[:3, :3], pose[:3, 3]
+        size = [gt[4], gt[3], gt[5]]                                                                  # (l, w, h) -> (w, l, h)
+        return Box(R @ gt[0:3] + t, size, R @ _rotz(-gt[-1]))
+
+    # ---- the per-reader interface of the live tracking command line (track.py): scenes, their scans, their raw point rows
+    _NAME = re.compile(r"seq_(\d+)_frame_(\d+)\.pkl")
+
+    def _scene_and_frame(self, lidar_path):
+        """(scene, frame) of a converter lidar file: from its name `seq_<s>_frame_<f>.pkl`, else from the pickle's scene_name /
+        frame_id."""
+        m = self._NAME.fullmatch(os.path.basename(lidar_path))
+        if m:
+            return m.group(1), int(m.group(2))
+        with open(lidar_path, 'rb') as f:
+            d = pickle.load(f)
+        return str(d['scene_name']), int(d['frame_id'])
+
+    def _scan_index(self):
+        """{scene: {frame: lidar path}} over the lidar directories the tracklets refer to; the scenes in order of first use."""
+        if not hasattr(self, '_scans_of'):
+            self._scans_of, self._frame_of = {}, {}
+            for annos in self.tracklet_anno_list:
+                for a in annos:
+                    self._frame_of[a['PC']] = sf = self._scene_and_frame(a['PC'])
+                    self._scans_of.setdefault(sf[0], {})
+            for d in sorted({os.path.dirname(p) for p in self._frame_of}):
+                for name in sorted(os.listdir(d)):
+                    if name.endswith('.pkl'):
+                        path = os.path.join(d, name)
+                        scene, frame = self._frame_of.get(path) or self._scene_and_frame(path)
+                        if scene in self._scans_of:
+                            self._scans_of[scene][frame] = path
+        return self._scans_of
+
+    @property
+    def scene_list(self):
+        """The scenes the split's tracklets lie in, in order of first appearance."""
+        return list(self._scan_index())
+
+    def scene_frames(self, scene):
+        """A scene's frame ids, in order."""
+        return sorted(self._scan_index().get(scene, {}))
+
+    def anno_frame(self, anno):
+        """(scene, frame) of an annotation."""
+        self._scan_index()
+        return self._frame_of[anno['PC']]
+
+    def scan_size(self, scene, frame):
+        """Points in a frame's scan (reads the frame's lidar file)."""
+        return len(self._stored_points(self._scan_index()[scene][frame]))
+
+    def raw_scan(self, scene, frame):
+        """The scan's rows as stored ((n, 3), float32 or float64) and its one transform, vehicle -> global (3x4)."""
+        path = self._scan_index()[scene][frame]
+        rows = np.asarray(self._stored_points(path))
+        if rows.dtype not in (np.float32, np.float64):
+            rows = rows.astype(np.float64)
+        return rows.reshape(-1, 3), [self._pose(path)[:3]]
+
+    def read_scan(self, scene, frame):
+        """A frame's whole scan in the global frame, as `get_frames` gives it with preload_offset=-1."""
+        return self._global_scan(self._scan_index()[scene][frame])

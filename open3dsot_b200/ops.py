@@ -3,6 +3,7 @@
 torch is used for device memory and the stream only.  Argument checks follow upstream `pointnet2_ops`
 (CHECK_CONTIGUOUS / CHECK_IS_FLOAT / CHECK_IS_INT / CHECK_CUDA -> RuntimeError; "CPU not supported").
 """
+import numpy as np
 import torch
 
 from . import _lib
@@ -304,6 +305,63 @@ def crop_resample(scans, count, frame, center, rot, half, size, seed, key, key_f
           None if prefix is None else prefix_keep.data_ptr(), Np, int(seed) & 0xFFFFFFFF, key.data_ptr(), key_frame.data_ptr(),
           int(perm_stream), int(pick_stream), K, int(size), scratch.data_ptr(), out.data_ptr(), n.data_ptr(), _stream())
     return out, n
+
+
+# ------------------------------------------------------------------ scan ingest for the live tracker's feeds (csrc/scan_ingest.cu)
+# o3d_scan_desc_t, field for field
+SCAN_DESC = np.dtype([("offset", "<i8"), ("rows", "<i4"), ("stride", "<i4"), ("is_f64", "<i4"), ("feed", "<i4"), ("half", "<i4"),
+                      ("n_xf", "<i4"), ("xf", "<f8", (2, 12))])
+assert SCAN_DESC.itemsize == 224
+
+
+def pack_scans(items, head=0):
+    """Pack raw scans for one `scan_ingest` call into one pinned host buffer: [head bytes | descriptors | rows].  `items`: (feed,
+    half, rows, transforms) with rows an (n, stride) float32 / float64 array as stored and transforms a list of at most two 3x4 (or
+    4x4) affine matrices applied in order.  Returns (buffer (uint8 torch tensor, pinned when CUDA is available), descriptors
+    (a SCAN_DESC numpy view into the buffer), byte offset of the descriptors, byte offset of the rows)."""
+    items = list(items)
+    rows = []
+    for feed, _, r, _ in items:
+        r = np.asarray(r)
+        if r.ndim != 2:
+            raise ValueError(f"scan_ingest: the rows of feed {feed} have shape {r.shape}; expected (points, values per row)")
+        rows.append(np.ascontiguousarray(r if r.dtype in (np.float32, np.float64) else r.astype(np.float64)))
+    d0 = -(-int(head) // 16) * 16
+    s0 = d0 + len(items) * SCAN_DESC.itemsize
+    offs, at = [], 0
+    for r in rows:
+        offs.append(at)
+        at += -(-r.nbytes // 16) * 16
+    buf = torch.empty(s0 + at, dtype=torch.uint8, pin_memory=torch.cuda.is_available())
+    host = buf.numpy()
+    desc = host[d0:s0].view(SCAN_DESC)
+    desc["xf"] = 0.0
+    for i, ((feed, half, _, xfs), r, o) in enumerate(zip(items, rows, offs)):
+        xfs = list(xfs)
+        if len(xfs) > 2:
+            raise ValueError(f"scan_ingest: {len(xfs)} transforms for feed {feed}; at most two")
+        for name, v in (("offset", o), ("rows", r.shape[0]), ("stride", r.shape[1]), ("is_f64", int(r.dtype == np.float64)),
+                        ("feed", int(feed)), ("half", int(half)), ("n_xf", len(xfs))):
+            desc[name][i] = v
+        for k, m in enumerate(xfs):
+            desc["xf"][i, k] = np.asarray(m, np.float64)[:3, :4].reshape(12)
+        host[s0 + o:s0 + o + r.nbytes] = r.reshape(-1).view(np.uint8)
+    return buf, desc, d0, s0
+
+
+def scan_ingest(scans, count, desc, dev_buf, desc_at, slab_at):
+    """Write raw scans into the feeds' halves of scans (F, 2, N, 3) fp32 CUDA and set count (F, 2) int64, in one launch
+    (csrc/scan_ingest.cu).  `desc`: the SCAN_DESC host descriptors (checked before the launch); `dev_buf`: the device copy of the
+    `pack_scans` buffer, with the descriptors at byte `desc_at` and the rows from byte `slab_at`."""
+    _chk_f(scans, "scans")
+    _chk_i64(count, "count")
+    F, two, N, _ = scans.shape
+    assert two == 2 and count.shape == (F, 2) and desc.dtype == SCAN_DESC and desc.flags.c_contiguous
+    if not dev_buf.is_cuda or dev_buf.dtype != torch.uint8 or not dev_buf.is_contiguous():
+        raise RuntimeError("dev_buf must be a contiguous uint8 CUDA tensor")
+    base = dev_buf.data_ptr()
+    _call("o3d_scan_ingest", desc.ctypes.data, base + desc_at, len(desc), base + slab_at, dev_buf.numel() - slab_at, F, N,
+          scans.data_ptr(), count.data_ptr(), _stream())
 
 
 # ------------------------------------------------------------------ split evaluation, K tracklets in flight (tracking/batched_tracker.py)

@@ -15,7 +15,17 @@ this tracker takes the scans as they arrive and targets as they appear and disap
   * a slot's draws are keyed by (seed, target id, frame within the target's track), so a target's result does not depend on its
     slot, on the other targets or on `max_targets`.
 Idle slots run on a fixed dummy box and report nothing: the cost of a step follows `max_targets`, not the number of active
-targets.  Ground-truth reference boxes (reference_BB 'previous_gt' / 'current_gt') have no meaning on a live stream, and
+targets.
+
+Feeds.  A feed is one sequence of scans: one sensor, or one recorded scene.  With `feeds=F` the scan buffer is (F, 2, N, 3), every
+slot follows one feed, and each feed has its own ping-pong parity.  `put(feed, points)` (xyz) or `put_raw(feed, rows, transforms)`
+(a scan's point rows as stored, with the reader's affine transforms) stages the next scan of a feed; `advance()` brings every
+staged scan in (host scans: one packed host->device copy and one `o3d_scan_ingest` launch for all feeds, csrc/scan_ingest.cu) and
+replays the one captured step.  A feed that got no scan since the last `advance()` holds still: its slots keep their box, frame
+counter, first-frame flag and parity.  Since draws are keyed by target id and frame within the track, a target's boxes depend
+neither on its feed, nor on the other feeds, nor on F.  `step(points)` is `put(0, points)` + `advance()` for one feed.
+Device memory: feeds * 2 * max_points * 12 bytes of scans, plus per slot the crop scratch and, for the first-frame template
+modes, max_points * 13 bytes of first-frame crop.  Ground-truth reference boxes (reference_BB 'previous_gt' / 'current_gt') have no meaning on a live stream, and
 shape_aggregation 'all' is not supported here; both are refused."""
 import numpy as np
 import torch
@@ -40,11 +50,12 @@ def _box_values(box):
 
 
 class MultiTargetTracker:
-    """`max_targets` slots over scans of at most `max_points` points.  `seed` keys the random draws; `use_graph`: capture the
-    step in a CUDA graph on the first `step()` (eager otherwise).  Call `step(scan)` for every scan of the stream, `add(id, box)`
-    to start a target on the scan just given, `drop(id)` to end it."""
+    """`max_targets` slots over `feeds` scan feeds of at most `max_points` points per scan.  `seed` keys the random draws;
+    `use_graph`: capture the step in a CUDA graph on the first advance (eager otherwise).  With one feed, call `step(scan)` for
+    every scan of the stream; with several, `put` / `put_raw` the feeds' next scans and `advance()`.  `add(id, box, feed=)` starts
+    a target on its feed's most recent scan, `drop(id)` ends it."""
 
-    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True):
+    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1):
         self.model = model.eval()
         self.cfg = cfg = model.config
         self.dev = dev = next(model.parameters()).device
@@ -59,15 +70,22 @@ class MultiTargetTracker:
             raise ValueError("shape_aggregation 'all' is not supported by the live multi-target tracker")
         self.N = N = int(max_points)
         self.K = K = int(max_targets)
-        if N < 1 or K < 1 or K > 65535:
-            raise ValueError(f"max_points={N} and max_targets={K} must be >= 1 (max_targets <= 65535)")
+        self.F = F = int(feeds)
+        if N < 1 or K < 1 or K > 65535 or F < 1:
+            raise ValueError(f"max_points={N}, max_targets={K} and feeds={F} must be >= 1 (max_targets <= 65535)")
         f = dict(device=dev, dtype=torch.float32)
         i64 = dict(device=dev, dtype=torch.int64)
-        self.scans = torch.zeros(2, N, 3, **f)
-        self.count = torch.zeros(2, **i64)
-        self.cur = torch.ones(K, **i64)                  # per slot: the buffer holding the most recent scan (all equal) ...
-        self.prev = torch.zeros(K, **i64)                # ... and the one holding the scan before it
-        self._cur = 1                                     # host mirror of cur
+        self.scans = torch.zeros(F, 2, N, 3, **f)
+        self.count = torch.zeros(F, 2, **i64)
+        # per feed: fed by this advance (0 / 1), the half holding its most recent scan, the half holding the scan before it;
+        # written from the host mirrors below before every step
+        self.fstate = torch.tensor([[0] * F, [1] * F, [0] * F], **i64)
+        self._fcur, self._fprev = [1] * F, [0] * F
+        self.feed_seen = [0] * F                          # scans advanced per feed
+        self._staged = {}                                 # feed -> None (already in its buffer) or (rows, transforms)
+        self.slot_feed = torch.zeros(K, **i64)
+        self.cur = torch.ones(K, **i64)                  # per slot: scan index (2 * feed + half) of its feed's most recent scan ...
+        self.prev = torch.zeros(K, **i64)                # ... and of the scan before it
         self.arange = torch.arange(N, device=dev)
         # slot state; idle slots hold the dummy box
         self.box_c = torch.zeros(K, 3, **f)
@@ -87,10 +105,11 @@ class MultiTargetTracker:
 
     # ------------------------------------------------------------------ one step for all slots, fixed shapes
     def _crop(self, which, box, half, perm, pick, size, prefix=False):
-        scans = self.scans if which is not None else self.scans[:, :0]
+        scans = self.scans.view(2 * self.F, self.N, 3)
+        scans = scans if which is not None else scans[:, :0]
         frame = which if which is not None else self.cur
         pre = (self.first_local, self.first_keep) if prefix else (None, None)
-        out, _ = ops.crop_resample(scans, self.count, frame, box.center, box.rot, half, size, self.seed, self.key, self.t, perm,
+        out, _ = ops.crop_resample(scans, self.count.view(2 * self.F), frame, box.center, box.rot, half, size, self.seed, self.key, self.t, perm,
                                    pick, *pre)
         return out
 
@@ -118,17 +137,19 @@ class MultiTargetTracker:
     def _step(self):
         cfg = self.cfg
         with torch.no_grad(), runtime.static_weights_scope():
-            self.prev.copy_(self.cur)
-            self.cur.neg_().add_(1)
-            self.t.add_(self.active.long())
+            fed, fcur, fprev = self.fstate
+            self.cur.copy_(self.slot_feed * 2 + fcur[self.slot_feed])
+            self.prev.copy_(self.slot_feed * 2 + fprev[self.slot_feed])
+            adv = self.active & (fed[self.slot_feed] != 0)                     # slots of a feed without a new scan hold
+            self.t.add_(adv.long())
             ops.keyed_uniform(self.key, self.t, self.seed, STREAM_LIMIT_BOX, 2, out=self.u_lim)
             box = bx.Box(self.box_c, self.box_s, self.box_r)
             est = best_proposal(self.model(self._inputs(box))["estimation_boxes"])
             new = bx.offset_box(box, est, degrees=cfg.degrees, use_z=cfg.use_z, limit_box=cfg.limit_box, rand=self.u_lim * 2 - 1)
-            a = self.active[:, None]
-            self.box_c.copy_(torch.where(a, new.center, self.box_c))            # idle slots keep the dummy box
+            a = adv[:, None]
+            self.box_c.copy_(torch.where(a, new.center, self.box_c))            # idle and holding slots keep their box
             self.box_r.copy_(torch.where(a[..., None], new.rot, self.box_r))
-            self.first_flag.zero_()
+            self.first_flag.masked_fill_(adv, 0.0)
 
     def _capture(self):
         # the warm-up runs a real step; the state it advances is restored before the captured graph's first replay
@@ -148,36 +169,100 @@ class MultiTargetTracker:
             t.copy_(v)
 
     # ------------------------------------------------------------------ public interface
-    def step(self, points, n_valid=None):
-        """Load the next scan (`points` (n, 3), the first `n_valid` valid; a CUDA tensor, or a host tensor copied without a
-        sync) and advance every active target to it.  Returns `boxes()`: device views of the slots' state, no host sync."""
-        n = points.shape[0]
+    def _feed(self, feed):
+        f = int(feed)
+        if not 0 <= f < self.F:
+            raise ValueError(f"feed {f} out of range: the tracker has feeds 0 .. {self.F - 1}")
+        return f
+
+    def _stage(self, feed, n):
+        f = self._feed(feed)
+        if f in self._staged:
+            raise ValueError(f"feed {f} already has a scan staged: advance() before the next put")
         if n > self.N:
             raise ValueError(f"max_points: the scan has {n} points, the tracker was built for {self.N}")
-        n_valid = n if n_valid is None else int(n_valid)
-        nxt = 1 - self._cur
-        self.scans[nxt, :n].copy_(points, non_blocking=True)
-        self.count[nxt].fill_(min(n_valid, n))
+        return f
+
+    def put(self, feed, points, n_valid=None):
+        """Stage the next scan of `feed`: `points` (n, 3), the first `n_valid` valid.  A CUDA tensor is copied into the feed's next
+        buffer at once; a host tensor or array goes through the packed copy and the ingest kernel of the next `advance()`.  No
+        host sync."""
+        n = points.shape[0]
+        f = self._stage(feed, n)
+        n_valid = n if n_valid is None else min(int(n_valid), n)
+        if isinstance(points, torch.Tensor) and (points.device == self.dev or self.dev.type != "cuda"):
+            nxt = 1 - self._fcur[f]
+            self.scans[f, nxt, :n].copy_(points, non_blocking=True)
+            self.count[f, nxt].fill_(n_valid)
+            self._staged[f] = None
+        else:
+            rows = points.numpy() if isinstance(points, torch.Tensor) else np.asarray(points)
+            self._staged[f] = (rows[:n_valid], ())
+
+    def put_raw(self, feed, rows, transforms=()):
+        """Stage the next scan of `feed` as a reader stores it: `rows` (n, stride) float32 / float64 (x, y, z first, 3 <= stride
+        <= 16) and up to two affine transforms (3x4 or 4x4, applied in order in float64, as the readers apply them on the host).
+        The next `advance()` moves every staged raw scan to the device in one copy and one `o3d_scan_ingest` launch."""
+        rows = np.asarray(rows)
+        if self.dev.type != "cuda":
+            raise RuntimeError("put_raw: scan ingest runs on the GPU; this tracker is not on a CUDA device")
+        if rows.ndim != 2 or not 3 <= rows.shape[1] <= 16:
+            raise ValueError(f"put_raw: rows of shape {rows.shape}; expected (points, 3 .. 16 values per row)")
+        transforms = [np.asarray(m, np.float64) for m in transforms]
+        if len(transforms) > 2 or any(m.shape not in ((3, 4), (4, 4)) for m in transforms):
+            raise ValueError("put_raw: at most two transforms, each 3x4 or 4x4")
+        f = self._stage(feed, rows.shape[0])
+        self._staged[f] = (rows, transforms)
+
+    def advance(self):
+        """Bring in every staged scan and advance the active targets of those feeds to it, in one replay of the captured step;
+        the other feeds hold.  Returns `boxes()`: device views of the slots' state, no host sync."""
+        F, staged = self.F, self._staged
+        raw = [(f, 1 - self._fcur[f], v[0], v[1]) for f, v in sorted(staged.items()) if v is not None]
+        for f in staged:
+            self._fprev[f], self._fcur[f] = self._fcur[f], 1 - self._fcur[f]
+            self.feed_seen[f] += 1
+        state = np.array([[int(f in staged) for f in range(F)], self._fcur, self._fprev], dtype=np.int64)
+        if self.dev.type == "cuda":
+            # one host->device copy per step: the feeds' state, the ingest descriptors and every raw scan's rows
+            buf, desc, d0, s0 = ops.pack_scans(raw, head=state.nbytes)
+            buf.numpy()[:state.nbytes] = state.reshape(-1).view(np.uint8)
+            dev = buf.to(self.dev, non_blocking=True)
+            self.fstate.copy_(dev[:state.nbytes].view(torch.int64).view(3, F))
+            if raw:
+                ops.scan_ingest(self.scans, self.count, desc, dev, d0, s0)
+        else:
+            self.fstate.copy_(torch.from_numpy(state))
         if not self.use_graph:
             self._step()
         else:
             if self.graph is None:
                 self._capture()
             self.graph.replay()
-        self._cur = nxt
-        self.scans_seen += 1
+        self.scans_seen += len(staged)
+        staged.clear()
         return self.boxes()
 
-    def add(self, target_id, box):
-        """Start target `target_id` on the most recent scan with `box` (a data_classes.Box or a tracking.boxes.Box): the box is
-        its result on that scan, and the template's first-frame crop is taken from it.  No host sync."""
+    def step(self, points, n_valid=None):
+        """One-feed form: load the next scan (`points` (n, 3), the first `n_valid` valid; a CUDA tensor, or a host tensor moved
+        without a sync) and advance every active target to it: `put(0, points)` + `advance()`."""
+        if self.F != 1:
+            raise ValueError(f"step() drives a one-feed tracker; with feeds={self.F} use put() / put_raw() and advance()")
+        self.put(0, points, n_valid)
+        return self.advance()
+
+    def add(self, target_id, box, feed=0):
+        """Start target `target_id` on the most recent scan of `feed` with `box` (a data_classes.Box or a tracking.boxes.Box): the
+        box is its result on that scan, and the template's first-frame crop is taken from it.  No host sync."""
         tid = int(target_id)
+        f = self._feed(feed)
         if tid in self.slot_of:
             raise ValueError(f"target_id {tid} is already active")
         if len(self.slot_of) >= self.K:
             raise ValueError(f"max_targets: all {self.K} slots are taken; drop a target first")
-        if self.scans_seen == 0:
-            raise RuntimeError("add() starts a target on the most recent scan: call step() with a scan first")
+        if (self.scans_seen if self.F == 1 else self.feed_seen[f]) == 0:
+            raise RuntimeError(f"add() starts a target on the most recent scan of its feed: call step() / advance() with a scan "
+                               f"of feed {f} first")
         k = min(set(range(self.K)) - set(self.slot_of.values()))
         c, s, r = _box_values(box)
         vals = torch.tensor(np.concatenate([c, s, r.reshape(-1)]), dtype=torch.float32)
@@ -187,11 +272,12 @@ class MultiTargetTracker:
         self.box_s[k].copy_(vals[3:6])
         self.box_r[k].copy_(vals[6:15].view(3, 3))
         if self.mode in ("firstandprevious", "first"):
-            cfg, cur = self.cfg, self._cur
+            cfg, cur = self.cfg, self._fcur[f]
             b = bx.Box(self.box_c[k], self.box_s[k], self.box_r[k])
-            local, keep, _ = bx.crop_and_center(self.scans[cur], b, offset=cfg.model_bb_offset, scale=cfg.model_bb_scale)
+            local, keep, _ = bx.crop_and_center(self.scans[f, cur], b, offset=cfg.model_bb_offset, scale=cfg.model_bb_scale)
             self.first_local[k].copy_(local)
-            self.first_keep[k].copy_(keep & (self.arange < self.count[cur]))
+            self.first_keep[k].copy_(keep & (self.arange < self.count[f, cur]))
+        self.slot_feed[k].fill_(f)
         # fill_ on a view, not `x[k] = value`: indexed assignment of a Python scalar copies it from the host and synchronises
         self.first_flag[k].fill_(1.0)
         self.active[k].fill_(True)
@@ -211,6 +297,7 @@ class MultiTargetTracker:
         self.box_r[k].copy_(torch.eye(3, device=self.dev))
         self.key[k].zero_()
         self.t[k].zero_()
+        self.slot_feed[k].zero_()
         if self.mode in ("firstandprevious", "first"):
             self.first_keep[k].zero_()
 
@@ -265,4 +352,146 @@ def track_stream(model, scans, starts, ends, max_targets, seed=0, max_points=Non
         for (t, live, _), h in zip(records, host):
             for tid, k in live.items():
                 out.setdefault(tid, {})[t] = Box(h[k, 0:3], h[k, 3:6], h[k, 6:15].reshape(3, 3))
+    return out
+
+
+def scene_peak(n_frames, starts, ends):
+    """The largest number of a scene's targets active at once (a target is active from its start frame through its end frame,
+    both included; without an end it runs to the scene's last frame)."""
+    delta = [0] * (n_frames + 1)
+    for t, group in starts.items():
+        for tid, _ in group:
+            delta[t] += 1
+            delta[min(ends.get(tid, n_frames - 1), n_frames - 1) + 1] -= 1
+    peak = live = 0
+    for d in delta:
+        live += d
+        peak = max(peak, live)
+    return peak
+
+
+def feed_schedule(lengths, peaks, feeds, max_targets):
+    """When and on which feed every scene runs.  Scenes are admitted longest first (ties in scene order); the next scene waits
+    for a free feed and for `peaks[i]` free slots, the most targets it has active at once, which stay reserved until it ends.  A
+    feed is reused from the step after its scene's last frame.  Returns [(scene, feed, first step)] in admission order; scene i
+    runs its frame t at step first + t."""
+    n = len(lengths)
+    for i in range(n):
+        if lengths[i] < 1:
+            raise ValueError(f"scene {i} has no frames")
+        if peaks[i] > max_targets:
+            raise ValueError(f"max_targets={max_targets}: scene {i} has {peaks[i]} targets active at once and can never fit")
+    order = sorted(range(n), key=lambda i: -lengths[i])
+    free_feeds, free_slots, running, out = list(range(int(feeds))), int(max_targets), [], []
+    step, q = 0, 0
+    while q < n:
+        for e, i, f in [r for r in running if r[0] < step]:
+            running.remove((e, i, f))
+            free_feeds.append(f)
+            free_slots += peaks[i]
+        free_feeds.sort()
+        while q < n and free_feeds and peaks[order[q]] <= free_slots:
+            i = order[q]
+            f = free_feeds.pop(0)
+            free_slots -= peaks[i]
+            running.append((step + lengths[i] - 1, i, f))
+            out.append((i, f, step))
+            q += 1
+        if q < n:
+            step = min(e for e, _, _ in running) + 1
+    return out
+
+
+def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256):
+    """Track many scenes through one tracker with `feeds` scan feeds (`feed_schedule` decides which scene runs when and where).
+    `scenes`: [{"frames": number of scans, "scan": t -> the scene's scan t, either (rows, transforms) for `put_raw` or an (n, 3)
+    tensor / array for `put`, "starts": {t: [(id, Box), ...]}, "ends": {id: last t}}]; a target without an end runs to its scene's
+    last frame, and target ids are unique over all scenes.  `max_points`: the scan buffer's size (required).
+    A host thread reads the next step's scans while the current step runs; the boxes are read back from the device every
+    `chunk` steps.  Returns, per scene, {id: {t: data_classes.Box}} from the frame a target starts on to its last frame."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    from ..datasets.data_classes import Box
+    if max_points is None:
+        raise ValueError("track_feeds: give max_points, the largest scan of the scenes")
+    scene_of, last = {}, []
+    for i, sc in enumerate(scenes):
+        T = int(sc["frames"])
+        for group in sc["starts"].values():
+            for tid, _ in group:
+                if tid in scene_of:
+                    raise ValueError(f"target id {tid} appears in scenes {scene_of[tid]} and {i}; ids must be unique")
+                scene_of[tid] = i
+        drops = {}
+        for group in sc["starts"].values():
+            for tid, _ in group:
+                drops.setdefault(min(sc["ends"].get(tid, T - 1), T - 1), []).append(tid)
+        last.append(drops)
+    lengths = [int(sc["frames"]) for sc in scenes]
+    peaks = [scene_peak(lengths[i], sc["starts"], sc["ends"]) for i, sc in enumerate(scenes)]
+    sched = feed_schedule(lengths, peaks, feeds, max_targets)
+    n_steps = max((s0 + lengths[i] for i, _, s0 in sched), default=0)
+    work = [[] for _ in range(n_steps)]                                        # per step: (feed, scene, frame)
+    first = {}
+    for i, f, s0 in sched:
+        first[i] = s0
+        for t in range(lengths[i]):
+            work[s0 + t].append((f, i, t))
+    trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, feeds=feeds)
+    out = [{} for _ in scenes]
+    pending, inflight = [], []
+
+    def load(step):
+        return [(f, i, t, scenes[i]["scan"](t)) for f, i, t in work[step]]
+
+    def read_back():                                                          # start a chunk's device -> host copy
+        snaps = torch.stack([r[2] for r in pending])
+        host = torch.empty(snaps.shape, dtype=snaps.dtype, pin_memory=snaps.is_cuda)
+        host.copy_(snaps, non_blocking=True)
+        done = torch.cuda.Event() if snaps.is_cuda else None
+        if done is not None:
+            done.record()
+        inflight.append(([(s, live) for s, live, _ in pending], host, done))
+        pending.clear()
+
+    def decode():                                                             # finish the oldest chunk
+        recs, host, done = inflight.pop(0)
+        if done is not None:
+            done.synchronize()
+        h = host.double().numpy()
+        for (s, live), hs in zip(recs, h):
+            for tid, k in live.items():
+                i = scene_of[tid]
+                out[i].setdefault(tid, {})[s - first[i]] = Box(hs[k, 0:3], hs[k, 3:6], hs[k, 6:15].reshape(3, 3))
+
+    with ThreadPoolExecutor(max_workers=1) as pool:
+        nxt = pool.submit(load, 0) if n_steps else None
+        for s in range(n_steps):
+            items = nxt.result()
+            if s + 1 < n_steps:
+                nxt = pool.submit(load, s + 1)                               # read ahead while this step runs
+            for f, i, t, scan in items:
+                if isinstance(scan, tuple):
+                    trk.put_raw(f, *scan)
+                else:
+                    trk.put(f, torch.as_tensor(scan))
+            trk.advance()
+            for f, i, t, _ in items:
+                for tid, box in scenes[i]["starts"].get(t, ()):
+                    trk.add(tid, box, feed=f)
+            live = trk.targets()
+            if live:
+                pending.append((s, live, trk.snapshot()))
+            for f, i, t, _ in items:
+                for tid in last[i].get(t, ()):
+                    if tid in live:
+                        trk.drop(tid)
+            if len(pending) >= chunk:
+                read_back()
+                if len(inflight) > 1:
+                    decode()
+    if pending:
+        read_back()
+    while inflight:
+        decode()
     return out

@@ -8,6 +8,10 @@ Reports, per scan size:
   * kernel level at --kernel-targets: o3d_crop_resample against crop_box_frame -> keyed_uniform x 2 -> resample on identical inputs
     (a firstandprevious template crop: a first-frame prefix of N candidates + the scan), time per call and peak memory above the
     inputs, after checking that both give the same bits.
+  * feeds (--feeds, --per-feed targets each): scans/s and target-frames/s of one tracker advancing F feeds per step, with every
+    scan given as raw nuScenes-like rows ((n, 5) float32 and two affine transforms), prepared either by the host (numpy float64
+    transforms, then `put`) or by the device (`put_raw`, one `o3d_scan_ingest` launch per step); host seconds per step spent
+    preparing the scans are reported for both, timed in the same run.
 Times are CUDA-event times over --frames steps (--reps calls for the kernels) after --warmup untimed ones per shape.  Weights
 are untrained (the timing does not depend on them).  The card's name and power limit are printed with the numbers."""
 import argparse
@@ -15,6 +19,7 @@ import json
 import os
 import subprocess
 import sys
+import time
 
 import numpy as np
 import torch
@@ -78,6 +83,53 @@ def bench_b1(net, scans, boxes, K, warmup, frames):
     return frames / (ms / 1e3)
 
 
+def _xf(yaw, t):
+    c, s = np.cos(yaw), np.sin(yaw)
+    return np.array([[c, -s, 0.0, t[0]], [s, c, 0.0, t[1]], [0.0, 0.0, 1.0, t[2]]])
+
+
+def _inverse(m):
+    r = m[:, :3].T
+    return np.hstack([r, -(r @ m[:, 3])[:, None]])
+
+
+def bench_feeds(net, scans_np, boxes, F, per_feed, warmup, frames, device_ingest):
+    """F feeds of `per_feed` targets; every feed replays the scene's scans as sensor rows (n, 5) + (sensor -> ego, ego -> global)."""
+    to_ego, to_global = _xf(0.3, (1.0, 0.0, 1.8)), _xf(-1.1, (400.0, 1100.0, 0.0))
+    to_sensor = _inverse(to_ego) @ np.vstack([_inverse(to_global), [0, 0, 0, 1]])
+    rows = []
+    for s in scans_np:
+        r = np.zeros((s.shape[0], 5), np.float32)
+        r[:, :3] = (s.astype(np.float64) @ to_sensor[:, :3].T + to_sensor[:, 3]).astype(np.float32)
+        rows.append(r)
+    trk = MultiTargetTracker(net, scans_np[0].shape[0], F * per_feed, seed=0, feeds=F)
+    host_s = [0.0]
+
+    def one(t):
+        t0 = time.perf_counter()
+        for f in range(F):
+            if device_ingest:
+                trk.put_raw(f, rows[t], (to_ego, to_global))
+            else:
+                p = rows[t][:, :3].T.astype(np.float64)
+                p = to_ego[:, :3] @ p + to_ego[:, 3][:, None]
+                p = to_global[:, :3] @ p + to_global[:, 3][:, None]
+                trk.put(f, np.ascontiguousarray(p.T, dtype=np.float32))
+        trk.advance()
+        host_s[0] += time.perf_counter() - t0
+
+    one(0)
+    for f in range(F):
+        for j in range(per_feed):
+            trk.add(f * per_feed + j, boxes[j][0], feed=f)
+    for i in range(warmup):
+        one(1 + i)
+    torch.cuda.synchronize()
+    host_s[0] = 0.0
+    ms = timed(lambda i: one(1 + warmup + i), frames)
+    return frames / (ms / 1e3), host_s[0] / frames
+
+
 def bench_kernel(cfg, scans, boxes, K, reps):
     """A firstandprevious template crop of K targets on a (2, N, 3) scan pair: fused against the three-kernel sequence."""
     dev = "cuda"
@@ -131,6 +183,8 @@ def main(argv=None):
     p.add_argument("--targets", type=int, nargs="+", default=[1, 8, 32, 64, 128])
     p.add_argument("--b1-targets", type=int, nargs="+", default=[1, 8, 32])
     p.add_argument("--kernel-targets", type=int, nargs="+", default=[64, 128])
+    p.add_argument("--feeds", type=int, nargs="+", default=[1, 4, 16])
+    p.add_argument("--per-feed", type=int, default=8)
     p.add_argument("--frames", type=int, default=20)
     p.add_argument("--warmup", type=int, default=3)
     p.add_argument("--reps", type=int, default=50)
@@ -142,7 +196,7 @@ def main(argv=None):
     net = get_model(cfg.net_model)(cfg).cuda().eval()
     info = gpu_info()
     print(f"# {info}; {os.path.basename(a.cfg)}; {a.frames} timed steps after {a.warmup} warm-up steps per shape", flush=True)
-    kmax = max(a.targets + a.b1_targets + a.kernel_targets)
+    kmax = max(a.targets + a.b1_targets + a.kernel_targets + [a.per_feed])
     results = {"gpu": info, "cfg": os.path.basename(a.cfg), "rows": []}
     for n in a.points:
         scene = synthetic_scene(n_frames=2 + a.warmup + a.frames, n_points=n, n_objects=kmax, seed=7, extent=70.0)
@@ -163,6 +217,16 @@ def main(argv=None):
             results["rows"].append({"points": n, "K": K, "tracker": "kernel", **r})
             print(f"kernel  N={n:6d} K={K:3d}: fused {r['fused_ms']:.3f} ms / {r['fused_peak_mb']:.0f} MB, three kernels "
                   f"{r['unfused_ms']:.3f} ms / {r['unfused_peak_mb']:.0f} MB (mean survivors {r['survivors_mean']:.0f})", flush=True)
+        for F in a.feeds:
+            for dev_ingest in (False, True):
+                sps, host = bench_feeds(net, scene["scans"], scene["boxes"], F, a.per_feed, a.warmup, a.frames, dev_ingest)
+                how = "device" if dev_ingest else "host"
+                results["rows"].append({"points": n, "feeds": F, "K": F * a.per_feed, "tracker": "feeds", "scan_prep": how,
+                                        "steps_per_s": sps, "scans_per_s": sps * F, "target_frames_per_s": sps * F * a.per_feed,
+                                        "host_s_per_step": host})
+                print(f"feeds   N={n:6d} F={F:3d} K={F * a.per_feed:3d} {how:6s} transforms: {sps * F:8.1f} scans/s  "
+                      f"{sps * F * a.per_feed:9.1f} target-frames/s  host {host * 1e3:7.2f} ms/step", flush=True)
+                torch.cuda.empty_cache()
         del scans
         torch.cuda.empty_cache()
     print(json.dumps(results))
