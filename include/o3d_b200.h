@@ -268,6 +268,13 @@ typedef struct o3d_stack_t {
                                  saves one elementwise add per parameter and call); 0 = overwritten                            */
     const void* prepared;     /* non-NULL (inference only): parameter block filled by o3d_stack_prepare(); the forward then
                                  neither packs weights nor finalises BatchNorm                                            */
+    int precision;            /* operands of the tensor-core forward GEMMs: 0 = 3xTF32 (default, fp32-grade), 1 = BF16 operands with
+                                 FP32 accumulation.  1 is for inference on a prepared block only: o3d_stack_forward returns
+                                 O3D_ERR_ARG with training, keep_for_backward or no `prepared`, and the prepare / size calls
+                                 refuse a training descriptor.  The block then holds one bf16 image per weight tile (2 bytes per
+                                 weight instead of 8) and the forward takes the bf16 pw_tc / sa_fused kernels.  Layers that the
+                                 plan sends to the exact-fp32 CUDA-core kernels (K < 32, P < 16, ...) stay fp32 either way;
+                                 accumulation, BatchNorm, ReLU, pooling and the first SA layer's coordinate term are fp32 too. */
 } o3d_stack_t;
 
 long long o3d_stack_workspace_bytes(const o3d_stack_t* d, int backward);
@@ -286,7 +293,8 @@ int o3d_stack_backward(const o3d_stack_t* d, const float* x, const void* ws_fwd,
  * body of _PointnetSAModuleBase.forward — QueryAndGroup (pointnet2/utils/pointnet2_utils.py:299-339), the SharedMLP and the
  * max-pool over nsample (pointnet2/utils/pointnet2_modules.py:58-76) — for one (grouper, mlp) scale.
  * d describes the SharedMLP in the reference's layout: xyz_first = 1, c0 = feature channels C, cin[0] = 3 + C, every cout <= 256,
- * C <= 288; P / K0 / S / training / lift are ignored.  o3d_sa_fused_prepare() packs the weights (pre-tiled TF32 hi | lo images) and
+ * C <= 288; P / K0 / S / lift are ignored, and training too unless precision = 1, which it refuses.  o3d_sa_fused_prepare() packs the
+ * weights (pre-tiled TF32 hi | lo images, or with precision = 1 one bf16 image per tile for the BF16 kernel) and
  * folds BatchNorm + bias into per-channel scale / shift once; `block` (o3d_sa_fused_prepared_bytes() bytes) then serves every call.
  * xyz [B, N, 3], new_xyz [B, M, 3], feat_cl [B, N, ldf] channels-last (NULL iff c0 == 0), out [B * M, ldo] channels-last,
  * idx (nullable) [B, M, nsample] receives the ball-query result.  nsample must divide 64 and M be a multiple of 64 / nsample. */

@@ -104,7 +104,11 @@ class StackDesc(ctypes.Structure):
                 ("weight", _P8), ("bias", _P8), ("gamma", _P8), ("beta", _P8),
                 ("running_mean", _P8), ("running_var", _P8), ("num_batches_tracked", _P8),
                 ("d_weight", _P8), ("d_bias", _P8), ("d_gamma", _P8), ("d_beta", _P8),
-                ("lift", ctypes.POINTER(LiftDesc)), ("accumulate", _i), ("prepared", _p)]
+                ("lift", ctypes.POINTER(LiftDesc)), ("accumulate", _i), ("prepared", _p),
+                ("precision", _i)]
+
+# o3d_stack_t.precision
+PRECISION_TF32X3, PRECISION_BF16 = 0, 1
 
 _lib = None
 

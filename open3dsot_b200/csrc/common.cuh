@@ -166,8 +166,14 @@ __device__ __forceinline__ uint32_t o3d_lanemask_lt() {
 }
 // o3d_pw_fwd_tc (pwmlp_tc.cu) with the direction of its walk over the position tiles: reverse = last tile first.  The
 // exported entry always walks forward; the stack sequencer (stack.cu) alternates the direction from layer to layer.
+// bf16: wtiles holds bf16 images (o3d_stack_t.precision = 1) and the BF16 kernel runs.
 int o3d_pw_fwd_tc_dir(const float* x, int ldx, const float* in_scale, const float* in_shift, int in_relu, const void* wtiles,
                       const float* bias, int P, int K, int N, float* y, int ldy, double* sum, double* sumsq, int S, float* ymax,
-                      float* ymin, int32_t* arg, int ldp, void* stream, bool reverse);
+                      float* ymin, int32_t* arg, int ldp, void* stream, bool reverse, bool bf16);
+// o3d_pw_fwd_tc_lift with the operand precision (as above)
+struct o3d_lift_t;
+int o3d_pw_fwd_tc_lift_prec(const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu,
+                            const void* wtiles, const float* bias, int P, int K, int N, float* y, int ldy, double* sum,
+                            double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp, void* stream, bool bf16);
 
 #endif

@@ -224,6 +224,13 @@ struct TcDy {
     }
 };
 
+// BF16 operands (inference precision 1): the same loader, its transformed rows rounded to bf16 (cvt.rn) where the 3xTF32
+// path splits them into hi / lo; the kernel then stores one bf16 image per stage and issues 2 wgmma k16 per k-block.  A wrapper
+// type rather than a flag, so that each precision is its own instantiation with no runtime branch in the hot loop.
+template <class L> struct Bf16 : L {};
+template <class L> struct is_bf16 { static constexpr bool value = false; };
+template <class L> struct is_bf16<Bf16<L>> { static constexpr bool value = true; };
+
 // ---- epilogues: thread = one output channel `ch`, called once per 32-position column group ------------------
 // LD: compile-time row stride of y (0 = use the runtime ldy)
 template <int LD>
@@ -450,6 +457,8 @@ __device__ __forceinline__ void stage_acc(const float (&acc)[R], float* stg, int
 template <class BLoad, class Epi>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     pw_tc_kernel(BLoad bl, const uint8_t* __restrict__ wtiles, int P, int K, int Nw, int nkb, Epi epi, int rev) {
+    constexpr bool BF = is_bf16<BLoad>::value;
+    constexpr int WBYTES = BF ? BF_TILE_BYTES : 2 * TILE_BYTES;   // weight image per (channel tile, k-block)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* tail = smem + TC_STAGES * TC_STAGE_BYTES + 2 * TC_EPI_BYTES;
@@ -505,11 +514,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             for (int kb = 0; kb < nkb; ++kb) {
                 o3d_mbar_wait(full + stage, phase);
                 const uint32_t sb = o3d_smem_u32(smem + stage * TC_STAGE_BYTES);
-                const uint32_t xb = sb + 2 * TILE_BYTES + h * (TILE_BYTES / 2);    // rows h*64.. of the activation tile
                 wgmma_fence_acc(acc);
                 wgmma_fence();
-                wgmma_3xtf32_kblock<128>(acc, make_desc(xb), make_desc(xb + TILE_BYTES), make_desc(sb), make_desc(sb + TILE_BYTES),
-                                         kb == 0);
+                if constexpr (BF) {
+                    const uint32_t xb = sb + 2 * TILE_BYTES + h * (BF_TILE_BYTES / 2);
+                    wgmma_bf16_kblock<128>(acc, make_desc_sw64(xb), make_desc_sw64(sb), kb == 0);
+                } else {
+                    const uint32_t xb = sb + 2 * TILE_BYTES + h * (TILE_BYTES / 2);    // rows h*64.. of the activation tile
+                    wgmma_3xtf32_kblock<128>(acc, make_desc(xb), make_desc(xb + TILE_BYTES), make_desc(sb), make_desc(sb + TILE_BYTES),
+                                             kb == 0);
+                }
                 wgmma_commit();
                 wgmma_wait<0>();
                 wgmma_fence_acc(acc);
@@ -570,9 +584,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         while (c0.t < n_ptiles) {
             o3d_mbar_wait(empty + stage, phase ^ 1);
             if (pt == 0) {
-                o3d_mbar_expect_tx(full + stage, 2 * TILE_BYTES);
-                o3d_bulk_g2s(smem + stage * TC_STAGE_BYTES, wtiles + ((size_t)mt0 * nkb + c0.kb) * (2 * TILE_BYTES), 2 * TILE_BYTES,
-                             full + stage);
+                o3d_mbar_expect_tx(full + stage, WBYTES);
+                o3d_bulk_g2s(smem + stage * TC_STAGE_BYTES, wtiles + ((size_t)mt0 * nkb + c0.kb) * WBYTES, WBYTES, full + stage);
                 const int tn = c0.t + (int)gridDim.x;
                 if (c0.kb == 0 && tn < n_ptiles) bl.prefetch_rows(tile_of(tn) * TC_N, TC_N, P);   // next tile of this CTA -> L2
             }
@@ -581,9 +594,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const float4 v = bl.finish(r0, f0, i, c0.p0 + row0 + i, P);
-                const uint32_t off = sw128(row0 + i, chunk);
-                *reinterpret_cast<float4*>(xhi + off) = hi_part(v);
-                *reinterpret_cast<float4*>(xlo + off) = lo_part(v);
+                if constexpr (BF) {
+                    *reinterpret_cast<uint2*>(xhi + sw64(row0 + i, chunk >> 1) + (chunk & 1) * 8) = pack_bf16x4(v);
+                } else {
+                    const uint32_t off = sw128(row0 + i, chunk);
+                    *reinterpret_cast<float4*>(xhi + off) = hi_part(v);
+                    *reinterpret_cast<float4*>(xlo + off) = lo_part(v);
+                }
             }
             o3d_fence_proxy_async();              // generic-proxy stores -> visible to the tensor core (async proxy)
             o3d_mbar_arrive(full + stage);
@@ -829,7 +846,7 @@ extern "C" int o3d_pw_tc_pretile(const float* w, int ldw, int rows, int K, void*
 
 int o3d_pw_fwd_tc_dir(const float* x, int ldx, const float* in_scale, const float* in_shift, int in_relu, const void* wtiles,
                       const float* bias, int P, int K, int N, float* y, int ldy, double* sum, double* sumsq, int S, float* ymax,
-                      float* ymin, int32_t* arg, int ldp, void* stream, bool reverse) {
+                      float* ymin, int32_t* arg, int ldp, void* stream, bool reverse, bool bf16) {
     O3D_REQUIRE(x && wtiles, O3D_ERR_ARG, "o3d_pw_fwd_tc: null pointer");
     O3D_REQUIRE(P >= 0 && K >= 4 && N >= 1 && (K & 3) == 0 && (ldx & 3) == 0, O3D_ERR_ARG, "o3d_pw_fwd_tc: bad sizes");
     O3D_REQUIRE(S == 0 || (P % S == 0 && 64 % S == 0 && ymax && ymin && arg), O3D_ERR_ARG,
@@ -839,6 +856,15 @@ int o3d_pw_fwd_tc_dir(const float* x, int ldx, const float* in_scale, const floa
     TcAct bl{x, ldx, in_scale, in_shift, in_relu};
     // the usual activation widths get a compile-time row stride (immediate store offsets in the epilogue)
     cudaStream_t st = (cudaStream_t)stream;
+    if (bf16) {
+        Bf16<TcAct> bb{bl};
+#define O3D_FWD_ARGS bb, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, reverse, st
+        if (ldy == 64) return launch_fwd<64>(O3D_FWD_ARGS);
+        if (ldy == 128) return launch_fwd<128>(O3D_FWD_ARGS);
+        if (ldy == 256) return launch_fwd<256>(O3D_FWD_ARGS);
+        return launch_fwd<0>(O3D_FWD_ARGS);
+#undef O3D_FWD_ARGS
+    }
 #define O3D_FWD_ARGS bl, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, reverse, st
     if (ldy == 64) return launch_fwd<64>(O3D_FWD_ARGS);
     if (ldy == 128) return launch_fwd<128>(O3D_FWD_ARGS);
@@ -851,7 +877,7 @@ extern "C" int o3d_pw_fwd_tc(const float* x, int ldx, const float* in_scale, con
                              const void* wtiles, const float* bias, int P, int K, int N, float* y, int ldy, double* sum,
                              double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp, void* stream) {
     return o3d_pw_fwd_tc_dir(x, ldx, in_scale, in_shift, in_relu, wtiles, bias, P, K, N, y, ldy, sum, sumsq, S, ymax, ymin, arg,
-                             ldp, stream, false);
+                             ldp, stream, false, false);
 }
 
 namespace {
@@ -962,10 +988,9 @@ extern "C" int o3d_pw_wgrad_tc_lift(const float* g, int ldg, const float* y, int
     return launch_wgrad(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
 }
 
-extern "C" int o3d_pw_fwd_tc_lift(const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift,
-                                  int in_relu, const void* wtiles, const float* bias, int P, int K, int N, float* y, int ldy,
-                                  double* sum, double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp,
-                                  void* stream) {
+int o3d_pw_fwd_tc_lift_prec(const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu,
+                            const void* wtiles, const float* bias, int P, int K, int N, float* y, int ldy, double* sum,
+                            double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp, void* stream, bool bf16) {
     O3D_REQUIRE(lf && (gidx || !lf->z) && wtiles, O3D_ERR_ARG, "o3d_pw_fwd_tc_lift: null pointer");
     O3D_REQUIRE(P >= 0 && K >= 32 && N >= 1 && (K & 3) == 0 && lf->ldz == K, O3D_ERR_ARG, "o3d_pw_fwd_tc_lift: bad sizes");
     O3D_REQUIRE(S == 0 || (P % S == 0 && 64 % S == 0 && ymax && ymin && arg), O3D_ERR_ARG,
@@ -974,10 +999,27 @@ extern "C" int o3d_pw_fwd_tc_lift(const o3d_lift_t* lf, const int32_t* gidx, con
     const int Nw = (N + 3) & ~3;
     const TcLift bl = make_tclift(lf, gidx, in_scale, in_shift, in_relu);
     cudaStream_t st = (cudaStream_t)stream;
+    if (bf16) {
+        const Bf16<TcLift> bb{bl};
+#define O3D_FWD_ARGS bb, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, false, st
+        if (ldy == 64) return launch_fwd<64>(O3D_FWD_ARGS);
+        if (ldy == 128) return launch_fwd<128>(O3D_FWD_ARGS);
+        if (ldy == 256) return launch_fwd<256>(O3D_FWD_ARGS);
+        return launch_fwd<0>(O3D_FWD_ARGS);
+#undef O3D_FWD_ARGS
+    }
 #define O3D_FWD_ARGS bl, wtiles, bias, P, K, Nw, y, ldy, sum, sumsq, S, ymax, ymin, arg, ldp, false, st
     if (ldy == 64) return launch_fwd<64>(O3D_FWD_ARGS);
     if (ldy == 128) return launch_fwd<128>(O3D_FWD_ARGS);
     if (ldy == 256) return launch_fwd<256>(O3D_FWD_ARGS);
     return launch_fwd<0>(O3D_FWD_ARGS);
 #undef O3D_FWD_ARGS
+}
+
+extern "C" int o3d_pw_fwd_tc_lift(const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift,
+                                  int in_relu, const void* wtiles, const float* bias, int P, int K, int N, float* y, int ldy,
+                                  double* sum, double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp,
+                                  void* stream) {
+    return o3d_pw_fwd_tc_lift_prec(lf, gidx, in_scale, in_shift, in_relu, wtiles, bias, P, K, N, y, ldy, sum, sumsq, S, ymax, ymin,
+                                   arg, ldp, stream, false);
 }

@@ -34,6 +34,9 @@ constexpr int SF_POS = 64;                  // positions per CTA
 constexpr int SF_THREADS = 288;
 constexpr int SF_ACT_KB = 2 * SF_POS * 128; // bytes per activation k-block: hi | lo
 constexpr int SF_WTILE = 2 * TILE_BYTES;    // one weight tile (128 channels x 32 k): hi | lo
+// BF16 variant: one bf16 image per k-block / tile instead of hi | lo, rows of 64 bytes (SWIZZLE_64B)
+template <bool BF> constexpr int SF_ACT_KB_OF = BF ? SF_POS * TC_BF_ROW : SF_ACT_KB;
+template <bool BF> constexpr int SF_WTILE_OF = BF ? BF_TILE_BYTES : SF_WTILE;
 constexpr int SF_MAX_SLOTS = 6;
 constexpr int SF_MISC = 128 + SF_POS * 4 + SF_POS * 16;   // barriers | idx | rel
 
@@ -55,14 +58,19 @@ __device__ __forceinline__ float2 ld2g(const float* p) { return __ldg(reinterpre
 __device__ __forceinline__ void sts_v4(uint32_t a, const float4& v) {
     asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
+__device__ __forceinline__ void sts_v2(uint32_t a, const uint2& v) {
+    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(a), "r"(v.x), "r"(v.y) : "memory");
+}
 
 // One layer on the two warpgroups.  NT = output channels per warpgroup: 64 (a one-tile layer, split) or 128 (tile h).
 // Every warpgroup walks every weight tile of the layer (waits for it, releases it) so that the ring's phases stay in step.
-template <int NT>
+// BF: bf16 operands (one wgmma k16 pair per k-block), the layer's output rounded to bf16 where the 3xTF32 path splits it.
+template <int NT, bool BF>
 __device__ __forceinline__ void sf_layer(const SfParams& prm, int l, uint8_t* act, uint8_t* ring, uint64_t* full, uint64_t* empty,
                                          int& slot, int& phase, const uint8_t* __restrict__ block, const float4* s_rel, int g0,
                                          float* __restrict__ out, int ldo) {
     const SfLayer& L = prm.l[l];
+    constexpr int ACT_KB = SF_ACT_KB_OF<BF>, WTILE = SF_WTILE_OF<BF>;
     const int h = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
     float acc[NT / 2];
 #pragma unroll
@@ -72,12 +80,15 @@ __device__ __forceinline__ void sf_layer(const SfParams& prm, int l, uint8_t* ac
             for (int kb = 0; kb < L.nkb; ++kb) {
                 o3d_mbar_wait(full + slot, phase);
                 if (NT == 64 || mt == h) {
-                    const uint32_t wb = o3d_smem_u32(ring + slot * SF_WTILE) + (NT == 64 ? h * (TILE_BYTES / 2) : 0);
-                    const uint32_t ab = o3d_smem_u32(act + kb * SF_ACT_KB);
+                    const uint32_t wb = o3d_smem_u32(ring + slot * WTILE) + (NT == 64 ? h * (WTILE / (BF ? 2 : 4)) : 0);
+                    const uint32_t ab = o3d_smem_u32(act + kb * ACT_KB);
                     wgmma_fence_acc(acc);
                     wgmma_fence();
-                    wgmma_3xtf32_kblock<NT>(acc, make_desc(ab), make_desc(ab + SF_ACT_KB / 2), make_desc(wb), make_desc(wb + TILE_BYTES),
-                                            kb == 0);
+                    if constexpr (BF)
+                        wgmma_bf16_kblock<NT>(acc, make_desc_sw64(ab), make_desc_sw64(wb), kb == 0);
+                    else
+                        wgmma_3xtf32_kblock<NT>(acc, make_desc(ab), make_desc(ab + SF_ACT_KB / 2), make_desc(wb),
+                                                make_desc(wb + TILE_BYTES), kb == 0);
                     wgmma_commit();
                     wgmma_wait<0>();
                     wgmma_fence_acc(acc);
@@ -121,7 +132,9 @@ __device__ __forceinline__ void sf_layer(const SfParams& prm, int l, uint8_t* ac
                 a1 = fmaf(wx2.y, rel[r].z, fmaf(wx1.y, rel[r].y, fmaf(wx0.y, rel[r].x, a1)));
             }
             const float v0 = fmaxf(fmaf(a0, sc.x, sh.x), floor_v), v1 = fmaxf(fmaf(a1, sc.y, sh.y), floor_v);
-            if (!last) {
+            if (!last && BF) {
+                *reinterpret_cast<uint32_t*>(act + (ch >> 5) * ACT_KB + sw64(pos, (ch & 31) >> 3) + (ch & 7) * 2) = pack_bf16x2(v0, v1);
+            } else if (!last) {
                 uint8_t* dst = act + (ch >> 5) * SF_ACT_KB + sw128(pos, (ch & 31) >> 2) + (ch & 3) * 4;
                 const float h0 = hi1(v0), h1 = hi1(v1);
                 *reinterpret_cast<float2*>(dst) = make_float2(h0, h1);
@@ -150,15 +163,17 @@ __device__ __forceinline__ void sf_layer(const SfParams& prm, int l, uint8_t* ac
     }
 }
 
+template <bool BF>
 __global__ void __launch_bounds__(SF_THREADS, 1)
     sa_fused_kernel(const SfParams prm, const uint8_t* __restrict__ block, const float* __restrict__ xyz,
                     const float* __restrict__ new_xyz, const float* __restrict__ feat, float* __restrict__ out, int ldo,
                     int32_t* __restrict__ idx_out) {
+    constexpr int ACT_KB = SF_ACT_KB_OF<BF>, WTILE = SF_WTILE_OF<BF>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* act = smem;
     uint8_t* ring = smem + prm.act_bytes;
-    uint8_t* misc = ring + prm.nslot * SF_WTILE;
+    uint8_t* misc = ring + prm.nslot * WTILE;
     uint64_t* full = reinterpret_cast<uint64_t*>(misc);       // [SF_MAX_SLOTS] weight tile landed
     uint64_t* empty = full + SF_MAX_SLOTS;                    // [SF_MAX_SLOTS] both warpgroups are done with the slot
     int32_t* s_idx = reinterpret_cast<int32_t*>(misc + 128);
@@ -187,9 +202,9 @@ __global__ void __launch_bounds__(SF_THREADS, 1)
                 if (!L.mma) continue;
                 for (int t = 0; t < L.n_mt * L.nkb; ++t) {
                     o3d_mbar_wait(empty + slot, phase ^ 1);
-                    o3d_mbar_expect_tx(full + slot, SF_WTILE);
-                    o3d_bulk_g2s(ring + slot * SF_WTILE, src, SF_WTILE, full + slot);
-                    src += SF_WTILE;
+                    o3d_mbar_expect_tx(full + slot, WTILE);
+                    o3d_bulk_g2s(ring + slot * WTILE, src, WTILE, full + slot);
+                    src += WTILE;
                     if (++slot == nslot) { slot = 0; phase ^= 1; }
                 }
             }
@@ -240,7 +255,8 @@ __global__ void __launch_bounds__(SF_THREADS, 1)
             const int chunk = tid & 7, r0 = tid >> 3;    // rows r0 and r0 + 32, 16-byte chunk `chunk` of every k-block
             const float* f0 = feat + ((size_t)b * N + s_idx[r0]) * prm.ldf + chunk * 4;
             const float* f1 = feat + ((size_t)b * N + s_idx[r0 + 32]) * prm.ldf + chunk * 4;
-            const uint32_t o0 = sw128(r0, chunk), o1 = sw128(r0 + 32, chunk);
+            const uint32_t o0 = BF ? sw64(r0, chunk >> 1) + (chunk & 1) * 8 : sw128(r0, chunk);
+            const uint32_t o1 = BF ? sw64(r0 + 32, chunk >> 1) + (chunk & 1) * 8 : sw128(r0 + 32, chunk);
             const int nkb = prm.l[0].nkb;
             for (int kb0 = 0; kb0 < nkb; kb0 += 4) {
                 float4 v0[4], v1[4];
@@ -254,12 +270,17 @@ __global__ void __launch_bounds__(SF_THREADS, 1)
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     if (kb0 + j >= nkb) break;
-                    const uint32_t hi = o3d_smem_u32(act) + (uint32_t)((kb0 + j) * SF_ACT_KB);
-                    const uint32_t lo = hi + SF_ACT_KB / 2;
-                    sts_v4(hi + o0, hi_part(v0[j]));
-                    sts_v4(lo + o0, lo_part(v0[j]));
-                    sts_v4(hi + o1, hi_part(v1[j]));
-                    sts_v4(lo + o1, lo_part(v1[j]));
+                    const uint32_t hi = o3d_smem_u32(act) + (uint32_t)((kb0 + j) * ACT_KB);
+                    if constexpr (BF) {
+                        sts_v2(hi + o0, pack_bf16x4(v0[j]));
+                        sts_v2(hi + o1, pack_bf16x4(v1[j]));
+                    } else {
+                        const uint32_t lo = hi + SF_ACT_KB / 2;
+                        sts_v4(hi + o0, hi_part(v0[j]));
+                        sts_v4(lo + o0, lo_part(v0[j]));
+                        sts_v4(hi + o1, hi_part(v1[j]));
+                        sts_v4(lo + o1, lo_part(v1[j]));
+                    }
                 }
             }
         }
@@ -268,8 +289,8 @@ __global__ void __launch_bounds__(SF_THREADS, 1)
         // ---- C / D. per layer: MMAs -> (+ coordinate term) -> BatchNorm + ReLU -> next operand | max-pool
         int slot = 0, phase = 0;
         for (int l = 0; l < prm.n; ++l) {
-            if (prm.l[l].n_mt == 2) sf_layer<128>(prm, l, act, ring, full, empty, slot, phase, block, s_rel, g0, out, ldo);
-            else sf_layer<64>(prm, l, act, ring, full, empty, slot, phase, block, s_rel, g0, out, ldo);
+            if (prm.l[l].n_mt == 2) sf_layer<128, BF>(prm, l, act, ring, full, empty, slot, phase, block, s_rel, g0, out, ldo);
+            else sf_layer<64, BF>(prm, l, act, ring, full, empty, slot, phase, block, s_rel, g0, out, ldo);
         }
     }
 }
@@ -282,7 +303,7 @@ struct SfPackLayer {
     uint32_t vec_off;
     size_t tile_off;
 };
-struct SfPackArgs { SfPackLayer l[O3D_MAX_LAYERS]; uint32_t wx_off; };
+struct SfPackArgs { SfPackLayer l[O3D_MAX_LAYERS]; uint32_t wx_off; int bf16; };
 
 // blockIdx.y = layer; a thread owns 4 consecutive k of one (padded) output channel
 __global__ void sa_fused_pack_kernel(const SfPackArgs args, uint8_t* __restrict__ block) {
@@ -319,6 +340,12 @@ __global__ void sa_fused_pack_kernel(const SfPackArgs args, uint8_t* __restrict_
         for (int j = 0; j < 4; ++j)
             if (k + j < L.kreal) v[j] = L.w[(size_t)n * L.cin + L.col0 + k + j];
     }
+    if (args.bf16) {   // one bf16 image per tile, rounded to nearest even
+        uint8_t* dst = block + L.tile_off + ((size_t)(n >> 7) * L.nkb + (k >> 5)) * BF_TILE_BYTES + sw64(n & 127, (k & 31) >> 3) +
+                       ((k >> 2) & 1) * 8;
+        *reinterpret_cast<uint2*>(dst) = pack_bf16x4(make_float4(v[0], v[1], v[2], v[3]));
+        return;
+    }
     uint8_t* dst = block + L.tile_off + ((size_t)(n >> 7) * L.nkb + (k >> 5)) * SF_WTILE + sw128(n & 127, (k & 31) >> 2);
     *reinterpret_cast<float4*>(dst) = make_float4(hi1(v[0]), hi1(v[1]), hi1(v[2]), hi1(v[3]));
     *reinterpret_cast<float4*>(dst + TILE_BYTES) = make_float4(v[0] - hi1(v[0]), v[1] - hi1(v[1]), v[2] - hi1(v[2]), v[3] - hi1(v[3]));
@@ -329,11 +356,14 @@ struct SfPlan {
     size_t tile_off[O3D_MAX_LAYERS];
     size_t bytes;
     int max_kb;
+    bool bf16;     // d->precision == 1: bf16 weight tiles and the BF16 kernel
 };
 
 // d: the SA layer's SharedMLP as a stack description — xyz_first = 1, c0 = feature channels, K0 = round4(c0) + 4 (unused here)
 bool sf_plan(const o3d_stack_t* d, SfPlan& p) {
     if (!d || d->n_layers < 1 || d->n_layers > O3D_MAX_LAYERS || !d->xyz_first || d->c0 < 0) return false;
+    if (d->precision != 0 && (d->precision != 1 || d->training)) return false;   // bf16 is for inference only
+    p.bf16 = d->precision == 1;
     SfParams& q = p.prm;
     q.n = d->n_layers;
     const int C = d->c0;
@@ -362,7 +392,7 @@ bool sf_plan(const o3d_stack_t* d, SfPlan& p) {
     q.tiles_off = (uint32_t)bytes;
     for (int l = 0; l < q.n; ++l) {
         p.tile_off[l] = bytes;
-        if (q.l[l].mma) bytes += (size_t)q.l[l].n_mt * q.l[l].nkb * SF_WTILE;
+        if (q.l[l].mma) bytes += (size_t)q.l[l].n_mt * q.l[l].nkb * (p.bf16 ? BF_TILE_BYTES : SF_WTILE);
     }
     p.bytes = bytes;
     return true;
@@ -382,6 +412,7 @@ extern "C" int o3d_sa_fused_prepare(const o3d_stack_t* d, void* block, void* str
     O3D_REQUIRE(sf_plan(d, p), O3D_ERR_ARG, "o3d_sa_fused_prepare: this SharedMLP does not fit the fused layer (see o3d_sa_fused_forward)");
     SfPackArgs a{};
     a.wx_off = p.prm.wx_off;
+    a.bf16 = p.bf16;
     int work_max = 0;
     for (int l = 0; l < p.prm.n; ++l) {
         const SfLayer& L = p.prm.l[l];
@@ -421,24 +452,30 @@ extern "C" int o3d_sa_fused_forward(const o3d_stack_t* d, const void* block, con
     SfParams prm = p.prm;
     prm.ldf = ldf; prm.N = N; prm.M = M; prm.S = nsample; prm.BM = B * M;
     prm.radius = radius; prm.radius2 = radius * radius; prm.normalize = normalize;
-    int act = p.max_kb * SF_ACT_KB;
+    const int act_kb = p.bf16 ? SF_ACT_KB_OF<true> : SF_ACT_KB, wtile = p.bf16 ? SF_WTILE_OF<true> : SF_WTILE;
+    int act = p.max_kb * act_kb;
     const int cloud = ((N * 12 + 1023) / 1024) * 1024;
     if (act < cloud) act = cloud;
     if (act < SF_ACT_KB) act = SF_ACT_KB;
-    prm.act_bytes = act;
     const int budget = 227 * 1024 - 1024 - SF_MISC - act;
-    int nslot = budget / SF_WTILE;
+    int nslot = budget / wtile;
     if (nslot > SF_MAX_SLOTS) nslot = SF_MAX_SLOTS;
     int tiles = 0;
     for (int l = 0; l < prm.n; ++l) tiles += prm.l[l].mma ? prm.l[l].n_mt * prm.l[l].nkb : 0;
     if (nslot > tiles && tiles >= 2) nslot = tiles;       // a short stack needs no deeper ring
     O3D_REQUIRE(nslot >= 2, O3D_ERR_ARG, "o3d_sa_fused_forward: N=%d points per cloud do not fit the shared-memory staging", N);
+    if (p.bf16) {   // the last layer's [position][channel] fp32 staging spans the operand and the ring, which bf16 makes smaller
+        const int staging = SF_POS * (p.prm.l[last].n_mt * 128 + 8) * 4;
+        if (act + nslot * wtile < staging) act = ((staging - nslot * wtile + 1023) / 1024) * 1024;
+    }
+    prm.act_bytes = act;
     const int cpc = SF_POS / nsample;
     const int grid = (B * M) / cpc;
     prm.nslot = nslot;
-    const int smem = 1024 + act + nslot * SF_WTILE + SF_MISC;
-    O3D_CUDA(cudaFuncSetAttribute(sa_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "o3d_sa_fused_forward: smem attribute");
-    sa_fused_kernel<<<grid, SF_THREADS, smem, (cudaStream_t)stream>>>(prm, (const uint8_t*)block, xyz, new_xyz, feat_cl, out, ldo, idx);
+    const int smem = 1024 + act + nslot * wtile + SF_MISC;
+    auto kern = p.bf16 ? sa_fused_kernel<true> : sa_fused_kernel<false>;
+    O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "o3d_sa_fused_forward: smem attribute");
+    kern<<<grid, SF_THREADS, smem, (cudaStream_t)stream>>>(prm, (const uint8_t*)block, xyz, new_xyz, feat_cl, out, ldo, idx);
     O3D_CHECK_LAUNCH("o3d_sa_fused_forward");
     return O3D_OK;
 }

@@ -9,6 +9,7 @@
 // stack can be captured into a CUDA graph.
 #include <string.h>
 #include "common.cuh"
+#include "tc_ptx.cuh"
 #include "../../include/o3d_b200.h"
 
 namespace {
@@ -43,7 +44,7 @@ struct PackLayer {
     const float* src; const float* bias; float* wp; float* wt; float* bias_p; uint8_t* tiles_f; uint8_t* tiles_b;
     int cout, cin, Nw, K, xyz_first, Km /* input channels tiled for dgrad */, Npad, Kpad /* iteration space */;
 };
-struct PackArgs { PackLayer l[O3D_MAX_LAYERS]; int c0; };
+struct PackArgs { PackLayer l[O3D_MAX_LAYERS]; int c0; int bf16; /* forward images in bf16 (o3d_stack_t.precision = 1) */ };
 
 // all layers of a stack in one launch: blockIdx.y = layer
 __global__ void pack_weight_kernel(const PackArgs args) {
@@ -77,7 +78,10 @@ __global__ void pack_weight_kernel(const PackArgs args) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) wt[(size_t)(k + j) * Nw + n] = v[j];
     }
-    if (tiles_f && k < nkb_f * 32) {   // forward image: tile (n / 128, k / 32), row n % 128, 16-byte chunk (k % 32) / 4
+    if (tiles_f && k < nkb_f * 32 && args.bf16) {   // bf16 forward image (BF_TILE_BYTES per tile, SWIZZLE_64B), nearest even
+        uint8_t* dst = tiles_f + ((size_t)(n >> 7) * nkb_f + (k >> 5)) * BF_TILE_BYTES + sw64(n & 127, (k & 31) >> 3) + ((k >> 2) & 1) * 8;
+        *reinterpret_cast<uint2*>(dst) = pack_bf16x4(make_float4(v[0], v[1], v[2], v[3]));
+    } else if (tiles_f && k < nkb_f * 32) {   // forward image: tile (n / 128, k / 32), row n % 128, 16-byte chunk (k % 32) / 4
         uint8_t* dst = tiles_f + ((size_t)(n >> 7) * nkb_f + (k >> 5)) * (2 * TILE) + tile_sw128(n & 127, (k & 31) >> 2);
         *reinterpret_cast<float4*>(dst) = make_float4(tf32_hi(v[0]), tf32_hi(v[1]), tf32_hi(v[2]), tf32_hi(v[3]));
         *reinterpret_cast<float4*>(dst + TILE) =
@@ -127,6 +131,7 @@ __global__ void d2f_kernel(const double* __restrict__ src, const float* __restri
 // ---- workspace plan -------------------------------------------------------------------------------------------
 struct Plan {
     int n, P, S, rows;
+    bool bf16;           // precision 1: bf16 forward images and kernels
     bool lift, virt;     // layer 0 lifted (o3d_lift_t); virt: Y0 is never stored (the tensor-core kernels gather it)
     size_t gidx;         // [P] int32: global Z row of every position (forward workspace)
     int Nw[O3D_MAX_LAYERS], K[O3D_MAX_LAYERS];
@@ -144,6 +149,8 @@ struct Plan {
 
 bool make_plan(const o3d_stack_t* d, Plan& p) {
     if (d->n_layers < 1 || d->n_layers > O3D_MAX_LAYERS || d->P < 0 || d->K0 < 4 || (d->K0 & 3)) return false;
+    if (d->precision != 0 && (d->precision != 1 || d->training)) return false;   // bf16 is for inference only
+    p.bf16 = d->precision == 1;
     p.n = d->n_layers; p.P = d->P; p.S = d->S;
     p.rows = d->S > 0 ? d->P / d->S : d->P;
     p.lift = d->lift != nullptr;
@@ -179,7 +186,7 @@ bool make_plan(const o3d_stack_t* d, Plan& p) {
         p.wp[l] = o; o += al(sizeof(float) * (size_t)p.Nw[l] * p.K[l]);
         p.wt[l] = o; o += al(sizeof(float) * (size_t)p.Nw[l] * p.K[l]);
         p.bias[l] = o; o += al(sizeof(float) * p.Nw[l]);
-        p.tiles[l] = o; if (p.tc_f[l]) o += al((size_t)o3d_pw_tc_wtile_bytes(p.Nw[l], p.K[l]));
+        p.tiles[l] = o; if (p.tc_f[l]) o += al((size_t)o3d_pw_tc_wtile_bytes(p.Nw[l], p.K[l]) / (p.bf16 ? 4 : 1));
         p.btiles[l] = o; if (p.tc_b[l]) o += al((size_t)o3d_pw_tc_wtile_bytes(tc_main(p.K[l]), p.Nw[l]));
     }
     p.param_bytes = o;       // everything above depends on the parameters only (eval mode): o3d_stack_prepare() fills it once
@@ -227,6 +234,7 @@ template <class T> inline const T* at(const uint8_t* ws, size_t off) { return re
 int pack_params(const o3d_stack_t* d, const Plan& p, uint8_t* ws, int keep_for_backward, cudaStream_t st) {
         PackArgs pa{};
         pa.c0 = d->c0;
+        pa.bf16 = p.bf16;
         int work_max = 0;
         for (int l = 0; l < p.n; ++l) {
             const int Nw = p.Nw[l], K = p.K[l];
@@ -294,6 +302,8 @@ extern "C" int o3d_stack_prepare(const o3d_stack_t* d, void* block, void* stream
 extern "C" int o3d_stack_forward(const o3d_stack_t* d, const float* x, void* ws_fwd, float* out, int keep_for_backward,
                                  void* stream) {
     O3D_REQUIRE(d && (x || d->lift) && ws_fwd && out, O3D_ERR_ARG, "o3d_stack_forward: null pointer");
+    O3D_REQUIRE(d->precision == 0 || (d->precision == 1 && d->prepared && !d->training && !keep_for_backward), O3D_ERR_ARG,
+                "o3d_stack_forward: precision %d needs inference on a prepared block (no training, no keep_for_backward)", d->precision);
     Plan p;
     O3D_REQUIRE(make_plan(d, p), O3D_ERR_ARG, "o3d_stack_forward: bad stack description");
     O3D_REQUIRE(p.S == 0 || (128 % p.S == 0 && p.P % p.S == 0), O3D_ERR_ARG, "o3d_stack_forward: group size %d", p.S);
@@ -332,13 +342,13 @@ extern "C" int o3d_stack_forward(const o3d_stack_t* d, const float* x, void* ws_
             // lifted layer: one gather pass = row indices + batch statistics (+ Y0 itself on the CUDA-core fallback)
             rc = o3d_lift_stats(d->lift, p.P, Nw, at<int32_t>(ws, p.gidx), p.virt ? nullptr : y, sum, sumsq, stream);
         } else if (l == 1 && p.virt) {
-            rc = o3d_pw_fwd_tc_lift(d->lift, at<int32_t>(ws, p.gidx), in_scale, in_shift, in_relu, wsp + p.tiles[l], bias, p.P, K,
-                                    cout, y, Nw, sum, sumsq, pool ? p.S : 0, ymax, ymin, arg, Nw, stream);
+            rc = o3d_pw_fwd_tc_lift_prec(d->lift, at<int32_t>(ws, p.gidx), in_scale, in_shift, in_relu, wsp + p.tiles[l], bias, p.P,
+                                         K, cout, y, Nw, sum, sumsq, pool ? p.S : 0, ymax, ymin, arg, Nw, stream, p.bf16);
         } else if (p.tc_f[l]) {
             // snake order: layer 0 starts where the grouping kernel finished (the end), layer 1 where layer 0 finished, ...
             void* tiles = wsp + p.tiles[l];
             rc = o3d_pw_fwd_tc_dir(cur, cur_ld, in_scale, in_shift, in_relu, tiles, bias, p.P, K, cout, y, Nw, sum, sumsq,
-                                   pool ? p.S : 0, ymax, ymin, arg, Nw, stream, (l & 1) == 0);
+                                   pool ? p.S : 0, ymax, ymin, arg, Nw, stream, (l & 1) == 0, p.bf16);
         } else {
             rc = o3d_pw_fwd(cur, cur_ld, in_scale, in_shift, in_relu, wt, Nw, bias, p.P, K, cout, y, Nw, sum, sumsq,
                             pool ? p.S : 0, ymax, ymin, arg, Nw, stream);
@@ -376,6 +386,7 @@ extern "C" int o3d_stack_forward(const o3d_stack_t* d, const float* x, void* ws_
 extern "C" int o3d_stack_backward(const o3d_stack_t* d, const float* x, const void* ws_fwd, void* ws_bwd, const float* out,
                                   const float* dout, float* dx, void* stream) {
     O3D_REQUIRE(d && (x || d->lift) && ws_fwd && ws_bwd && out && dout, O3D_ERR_ARG, "o3d_stack_backward: null pointer");
+    O3D_REQUIRE(d->precision == 0, O3D_ERR_ARG, "o3d_stack_backward: precision %d is for inference only", d->precision);
     Plan p;
     O3D_REQUIRE(make_plan(d, p), O3D_ERR_ARG, "o3d_stack_backward: bad stack description");
     if (p.P == 0) return O3D_OK;

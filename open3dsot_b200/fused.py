@@ -157,6 +157,16 @@ def _derived(weight, tag, make):
     return _static_cached(tag, None, [weight], lambda: make().detach())
 
 
+def _precision_code(training, need_grad):
+    """o3d_stack_t.precision of a forward under the current runtime.inference_precision(); bf16 refuses autograd and training"""
+    if runtime.inference_precision() == "fp32":
+        return _lib.PRECISION_TF32X3
+    if need_grad or training:
+        raise RuntimeError("bf16 inference precision: forward passes that need a gradient, and modules in training mode, run in "
+                           "fp32 only (leave runtime.inference_precision_scope('bf16'))")
+    return _lib.PRECISION_BF16
+
+
 def _prepare_stack(d, device):
     """the stack's prepared block: packed weights and folded running statistics (o3d_stack_prepare)"""
     L = _lib.lib()
@@ -223,10 +233,11 @@ class _StackFn(torch.autograd.Function):
             d.lift = ctypes.pointer(lf)
         L = _lib.lib()
         need_grad = meta.grad_mode and any(ctx.needs_input_grad)   # (needs_input_grad mirrors requires_grad even under no_grad)
+        d.precision = _precision_code(meta.training, need_grad)
         block = None            # inference with static weights: the prepared block, referenced here until the forward is enqueued
         if not need_grad and not meta.training and runtime.static_weights():
             lifted = False if lift is None else (z is not None, s is not None)
-            shape = (P, K0, meta.S, lifted, runtime.tc_level(), meta.xyz_first, meta.c0)
+            shape = (P, K0, meta.S, lifted, runtime.tc_level(), meta.xyz_first, meta.c0, d.precision)
             block = _static_cached("stack", shape, meta.params + meta.stats, lambda: _prepare_stack(d, dev))
             d.prepared = block.data_ptr()
         nbytes = L.o3d_stack_workspace_bytes(ctypes.byref(d), 0)
@@ -350,8 +361,9 @@ def _sa_fused_forward(specs, xyz, new_xyz, feat_cl, C, radius, S, normalize):
     npoint = new_xyz.shape[1]
     meta = _Meta(specs, S, False, xyz_first=True, c0=C)
     d = _describe(meta, B * npoint * S, _r4(C) + 4, meta.params)
+    d.precision = _precision_code(False, False)
     if runtime.static_weights():
-        block = _static_cached("sa_fused", None, meta.params + meta.stats, lambda: _sa_fused_prepare(d, xyz.device))
+        block = _static_cached("sa_fused", d.precision, meta.params + meta.stats, lambda: _sa_fused_prepare(d, xyz.device))
     else:
         block = _sa_fused_prepare(d, xyz.device)
     ldo = _r4(meta.cout[-1])

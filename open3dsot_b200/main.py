@@ -23,6 +23,9 @@ def parse_args(argv=None):
     p.add_argument('--log_dir', type=str, default=None, help='log location')
     p.add_argument('--test', action='store_true', default=False, help='test mode')
     p.add_argument('--preloading', action='store_true', default=False, help='preload dataset into memory')
+    p.add_argument('--precision', choices=('fp32', 'bf16'), default='fp32',
+                   help='--test: operand precision of the tensor-core layers (bf16: BF16 operands, FP32 accumulation); '
+                        'training is fp32 only')
     return p.parse_args(argv)
 
 
@@ -60,7 +63,7 @@ def main(argv=None):
                 load_weights(model, load_lightning_checkpoint(cfg.checkpoint)["state_dict"])
             tracklets = get_dataset(cfg, type='test', split=cfg.test_split)
             from .tracking.evaluate import evaluate_sharded
-            res = evaluate_sharded(model, tracklets, slots=32, seed=0)
+            res = evaluate_sharded(model, tracklets, slots=32, seed=0, precision=cfg.precision)
             out = {"checkpoint": cfg.checkpoint, "split": cfg.test_split, "success": res["success"],
                    "precision": res["precision"], "frames": res["frames"]}
             if rank == 0:

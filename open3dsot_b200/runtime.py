@@ -89,6 +89,45 @@ def static_weights_scope():
         _STATIC_WEIGHTS = old
 
 
+# Operand precision of the tensor-core forward GEMMs in inference (include/o3d_b200.h o3d_stack_t.precision): "fp32" = 3xTF32
+# (default, fp32-grade), "bf16" = BF16 operands with FP32 accumulation.  Only inference_precision_scope() changes it.
+PRECISIONS = ("fp32", "bf16")
+_PRECISION = "fp32"
+
+
+def inference_precision() -> str:
+    return _PRECISION
+
+
+def check_precision(precision) -> str:
+    """`precision` if it is one of PRECISIONS, else a ValueError"""
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be one of {PRECISIONS}, got {precision!r}")
+    return precision
+
+
+@contextlib.contextmanager
+def inference_precision_scope(precision):
+    """`with runtime.inference_precision_scope("bf16"):` — eval-mode forward passes without autograd run their tensor-core GEMMs
+    (the fused SA layer and the pw_tc forward) on BF16 operands with FP32 accumulation.  A bf16 block is a prepared parameter
+    block, so the scope also turns on static weights (static_weights_scope); its blocks are cached beside the fp32 ones.  A
+    forward that needs a gradient, or a module in training mode, raises a RuntimeError inside a "bf16" scope.  Layers that run on
+    the exact-fp32 CUDA-core kernels, and everything outside the MLP stacks (FPS, ball query, cross-correlation, box math), stay
+    fp32.  "fp32" leaves every result as it is outside the scope."""
+    global _PRECISION
+    check_precision(precision)
+    old = _PRECISION
+    _PRECISION = precision
+    try:
+        if precision == "bf16":
+            with static_weights_scope():
+                yield
+        else:
+            yield
+    finally:
+        _PRECISION = old
+
+
 # In-place accumulation of parameter gradients: a stack's backward ADDS its weight / bias / BatchNorm gradients straight into the
 # parameters' existing `.grad` buffers (and returns no gradient for them) instead of materialising them and letting autograd's
 # AccumulateGrad issue one elementwise add per parameter — ~130 launches per BAT step.  Only valid for `loss.backward()` onto

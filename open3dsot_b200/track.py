@@ -28,6 +28,8 @@ def parse_args(argv=None):
     p.add_argument('--max_targets', type=int, default=64, help='tracker slots (targets in flight at once)')
     p.add_argument('--max_points', type=int, default=None, help='scan buffer size (default: the largest scan streamed)')
     p.add_argument('--seed', type=int, default=0, help='key of the random draws')
+    p.add_argument('--precision', choices=('fp32', 'bf16'), default='fp32',
+                   help='operand precision of the tensor-core layers (bf16: BF16 operands, FP32 accumulation)')
     return p.parse_args(argv)
 
 
@@ -65,7 +67,7 @@ def _yaw(rot, up_axis):
     return float(np.arctan2(rot[1, 0], rot[0, 0]))
 
 
-def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0):
+def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, precision="fp32"):
     """Track every scene of `dataset`'s split and write `out_path`; returns {"success", "precision", "frames", "scenes"}."""
     from .tracking.multi_tracker import track_feeds
     from .utils.metrics import Precision, Success, estimateAccuracy, estimateOverlap
@@ -85,7 +87,8 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0):
             ends[tr["index"]] = pos[tr["end"]]
         scenes.append({"frames": len(p["frames"]), "starts": starts, "ends": ends,
                        "scan": lambda t, p=p: dataset.raw_scan(p["scene"], p["frames"][t])})
-    results = track_feeds(model, scenes, max(1, min(len(scenes), max_targets)), max_targets, seed=seed, max_points=max_points)
+    results = track_feeds(model, scenes, max(1, min(len(scenes), max_targets)), max_targets, seed=seed, max_points=max_points,
+                          precision=precision)
     overlaps, distances = [[] for _ in annos], [[] for _ in annos]
     with open(out_path, "w") as f:
         for p, res in zip(plan, results):
@@ -143,7 +146,8 @@ def main(argv=None):
     model = get_model(cfg.net_model)(cfg).cuda()
     if args.checkpoint is not None:
         load_weights(model, load_lightning_checkpoint(args.checkpoint)["state_dict"])
-    out = run(model, data, args.out, max_targets=args.max_targets, max_points=args.max_points, seed=args.seed)
+    out = run(model, data, args.out, max_targets=args.max_targets, max_points=args.max_points, seed=args.seed,
+              precision=args.precision)
     out.update({"checkpoint": args.checkpoint, "split": args.split, "out": args.out})
     print(json.dumps(out), flush=True)
     return out

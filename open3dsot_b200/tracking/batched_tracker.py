@@ -120,7 +120,9 @@ class BatchedDeviceTracker:
     (the key of their random draws; default 0..n-1); `max_points`: padded scan size (default: the largest scan);
     `history`: starting capacity (points per slot) of the 'all' template history, raised by `run()` when a slot needs more."""
 
-    def __init__(self, model, tracklets, slots, seed=0, ids=None, max_points=None, use_graph=True, history=HISTORY_POINTS):
+    def __init__(self, model, tracklets, slots, seed=0, ids=None, max_points=None, use_graph=True, history=HISTORY_POINTS,
+                 precision="fp32"):
+        self.precision = runtime.check_precision(precision)
         self.model = model.eval()
         self.cfg = cfg = model.config
         self.dev = dev = next(model.parameters()).device
@@ -228,7 +230,7 @@ class BatchedDeviceTracker:
 
     def _step(self):
         cfg, P = self.cfg, self.pool
-        with torch.no_grad(), runtime.static_weights_scope():
+        with torch.no_grad(), runtime.static_weights_scope(), runtime.inference_precision_scope(self.precision):
             active = self.frame >= 0
             f = self.frame.clamp(min=0)                                        # idle slots track pool frame 0, unrecorded
             self._draw(f - P.first[f])

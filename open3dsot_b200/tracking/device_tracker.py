@@ -52,9 +52,12 @@ def tracking_modes(model):
 class DeviceTracker:
     """`reset(points, box)` on a tracklet's first frame, then `step(points, n_valid, ref_box)` per frame.  `seed` keys the
     random draws; `history`: starting capacity (points) of the 'all' template history.  Motion models (M2-Track) ignore
-    shape_aggregation and reference_BB, as the reference's MotionBaseModel does."""
+    shape_aggregation and reference_BB, as the reference's MotionBaseModel does.  `precision`: "fp32" (3xTF32 GEMMs, default) or
+    "bf16" (BF16 operands, FP32 accumulation: runtime.inference_precision_scope) for the network's tensor-core layers."""
 
-    def __init__(self, model, max_points, use_graph=True, seed=1, history=HISTORY_POINTS):
+    def __init__(self, model, max_points, use_graph=True, seed=1, history=HISTORY_POINTS, precision="fp32"):
+        from .. import runtime
+        self.precision = runtime.check_precision(precision)
         self.model = model.eval()
         self.cfg = model.config
         self.dev = next(model.parameters()).device
@@ -229,7 +232,7 @@ class DeviceTracker:
         cfg = self.cfg
         from .. import runtime
         # the tracker never changes the weights: eval-mode stacks pack them / fold their BatchNorm once, not per frame
-        with torch.no_grad(), runtime.static_weights_scope():
+        with torch.no_grad(), runtime.static_weights_scope(), runtime.inference_precision_scope(self.precision):
             out = self.model(self._inputs())
             est = out["estimation_boxes"][0]                                   # (num_proposal, 5) or (4,)
             if est.dim() == 2:

@@ -18,7 +18,7 @@ def evaluate(model, sequences, progress=None):
     return {"success": succ.compute(), "precision": prec.compute(), "frames": frames, "results": results}
 
 
-def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 << 30, use_graph=True, ids=None):
+def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 << 30, use_graph=True, ids=None, precision="fp32"):
     """`evaluate()` with `slots` tracklets in flight on the device (tracking/batched_tracker.py): one graph replay per frame
     step for all of them, overlap and centre distance computed on the device, one device-to-host copy per chunk of tracklets
     whose padded frames fit `max_resident_bytes` (a tracklet is never split).  The random draws of a tracklet are keyed by
@@ -29,14 +29,18 @@ def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 <
     its ground truth against itself sits exactly on Success's top threshold.
     The model's shape_aggregation (including 'all': every past frame's crop, kept in a per-slot history whose bytes count
     against `max_resident_bytes`) and reference_BB ('previous_gt' / 'current_gt': the search area and the box update use the
-    ground truth of the previous / current frame, and the result box takes its size) are honoured as the host loop does."""
+    ground truth of the previous / current frame, and the result box takes its size) are honoured as the host loop does.
+    `precision`: "fp32" or "bf16", the tensor-core operand precision of the network (BatchedDeviceTracker)."""
     import numpy as np
+
+    from .. import runtime
 
     from ..datasets import data_classes
     from ..utils.metrics import estimateAccuracy, estimateOverlap
     from .batched_tracker import BatchedDeviceTracker, history_bytes, plan_chunks, pool_frame_bytes
     from .device_tracker import HISTORY_POINTS, tracking_modes
 
+    runtime.check_precision(precision)
     sequences = list(sequences)
     cfg = model.config
     dim, up = cfg.IoU_space, cfg.up_axis
@@ -61,7 +65,7 @@ def evaluate_batched(model, sequences, slots=64, seed=0, max_resident_bytes=16 <
             if all(lengths[j] < 2 for j in chunk):
                 continue
             trk = BatchedDeviceTracker(model, [sequences[j] for j in chunk], slots, seed=seed, ids=[ids[j] for j in chunk],
-                                       max_points=npts, use_graph=use_graph)
+                                       max_points=npts, use_graph=use_graph, precision=precision)
             ov, di, cen, rot = trk.run()
             offsets = trk.plan["offsets"]
             del trk
@@ -118,7 +122,7 @@ def gather_shards(n, ids, local):
 def evaluate_sharded(model, sequences, slots=64, seed=0, **kw):
     """`evaluate_batched` split across the ranks of a process group (shard_plan): each rank tracks its tracklets with their
     draws keyed by their index in `sequences`, and every rank returns the whole split's result.  With one rank it is
-    `evaluate_batched`."""
+    `evaluate_batched`; `kw` (e.g. `precision`) goes to it."""
     from .. import ddp
     sequences = list(sequences)
     if not ddp.is_distributed():

@@ -55,7 +55,8 @@ class MultiTargetTracker:
     every scan of the stream; with several, `put` / `put_raw` the feeds' next scans and `advance()`.  `add(id, box, feed=)` starts
     a target on its feed's most recent scan, `drop(id)` ends it."""
 
-    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1):
+    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1, precision="fp32"):
+        self.precision = runtime.check_precision(precision)
         self.model = model.eval()
         self.cfg = cfg = model.config
         self.dev = dev = next(model.parameters()).device
@@ -136,7 +137,7 @@ class MultiTargetTracker:
 
     def _step(self):
         cfg = self.cfg
-        with torch.no_grad(), runtime.static_weights_scope():
+        with torch.no_grad(), runtime.static_weights_scope(), runtime.inference_precision_scope(self.precision):
             fed, fcur, fprev = self.fstate
             self.cur.copy_(self.slot_feed * 2 + fcur[self.slot_feed])
             self.prev.copy_(self.slot_feed * 2 + fprev[self.slot_feed])
@@ -321,16 +322,17 @@ class MultiTargetTracker:
         return {tid: Box(host[k, 0:3], host[k, 3:6], host[k, 6:15].reshape(3, 3)) for tid, k in self.slot_of.items()}
 
 
-def track_stream(model, scans, starts, ends, max_targets, seed=0, max_points=None, use_graph=True):
+def track_stream(model, scans, starts, ends, max_targets, seed=0, max_points=None, use_graph=True, precision="fp32"):
     """Track targets through a stream of scans.  `scans`: iterable of (n, 3) tensors; `starts`: {frame: [(id, Box), ...]} — each
     target starts on that scan with that box; `ends`: {id: last frame} (a target without an entry runs to the end of the
     stream).  `max_points`: the scan buffer's size (default: the largest scan, which needs the whole stream up front).
     Returns {id: {frame: data_classes.Box}}, from the frame a target starts on to its last frame; the device is read back once."""
     from ..datasets.data_classes import Box
+    runtime.check_precision(precision)
     if max_points is None:
         scans = list(scans)
         max_points = max((s.shape[0] for s in scans), default=1)
-    trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph)
+    trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, precision=precision)
     dev = trk.dev
     records = []                                                              # (frame, {id: slot}, device snapshot)
     for t, pts in enumerate(scans):
@@ -402,7 +404,7 @@ def feed_schedule(lengths, peaks, feeds, max_targets):
     return out
 
 
-def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256):
+def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32"):
     """Track many scenes through one tracker with `feeds` scan feeds (`feed_schedule` decides which scene runs when and where).
     `scenes`: [{"frames": number of scans, "scan": t -> the scene's scan t, either (rows, transforms) for `put_raw` or an (n, 3)
     tensor / array for `put`, "starts": {t: [(id, Box), ...]}, "ends": {id: last t}}]; a target without an end runs to its scene's
@@ -412,6 +414,7 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
     from concurrent.futures import ThreadPoolExecutor
 
     from ..datasets.data_classes import Box
+    runtime.check_precision(precision)
     if max_points is None:
         raise ValueError("track_feeds: give max_points, the largest scan of the scenes")
     scene_of, last = {}, []
@@ -437,7 +440,7 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
         first[i] = s0
         for t in range(lengths[i]):
             work[s0 + t].append((f, i, t))
-    trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, feeds=feeds)
+    trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, feeds=feeds, precision=precision)
     out = [{} for _ in scenes]
     pending, inflight = [], []
 

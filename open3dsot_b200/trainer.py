@@ -31,6 +31,8 @@ def check_supported(cfg):
         raise ValueError(f"gradient_clip_val: {cfg.gradient_clip_val} is not supported; only 0 (no clipping) is")
     if cfg.get("random_sample", False):
         raise ValueError("random_sample: True is not supported; epochs pass over every frame (random_sample: False)")
+    if str(cfg.get("precision", "fp32")) != "fp32":
+        raise ValueError(f"precision: {cfg.precision!r} is for inference only (--test); training and its validation run in fp32")
 
 
 def epoch_indices(n, epoch, seed=0, rank=0, world=1):
