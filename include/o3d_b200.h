@@ -326,6 +326,16 @@ int o3d_pw_wgrad_tc_lift(const float* g, int ldg, const float* y, int ldy, const
                          const float* in_scale, const float* in_shift, int in_relu, int P, int Cout, int Cin, float* dw,
                          int lddw, float* part, long long part_floats, void* stream);
 
+/* Both gradients of one layer with Cout, Cin in {64, 128} in one kernel: the dgrad of o3d_pw_dgrad_tc(_lift) into out
+ * [P, Cin] (its ReLU mask and BN-backward sums read x's raw rows when in_scale or in_relu is set, or Y0 when lf is given)
+ * and the weight gradient of o3d_pw_wgrad_tc2 / o3d_pw_wgrad_tc_lift added into dw.  X is x [P, Cin] or, with lf, the lifted
+ * first layer.  part: o3d_pw_wgrad_tc2_workspace_floats() floats; the partials are summed in a fixed order (deterministic). */
+int o3d_pw_bwd_tc(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                  const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, const float* x,
+                  const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu, int P,
+                  int Cout, int Cin, float* out, double* s1, double* s2y, float* dw, int lddw, float* part,
+                  long long part_floats, void* stream);
+
 /* wgrad on the tensor core (operands transposed to K-major SWIZZLE_128B tiles), 128 x 128 tiles of dW per CTA, split over
  * positions; the per-split partial tiles go to `part` (o3d_pw_wgrad_tc2_workspace_floats() floats) and a second kernel adds
  * their sum into dw in a fixed order (deterministic).                                                               */

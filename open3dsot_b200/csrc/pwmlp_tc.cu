@@ -9,6 +9,7 @@
 // into a TF32 "hi" part (the fp32 word with its 13 low mantissa bits cleared) and a "lo" part
 // (x - hi, exact), so that   Xlo*Whi + Xhi*Wlo + Xhi*Whi   carries ~21 mantissa bits — fp32-grade accuracy, which
 // the 1e-4 parity bar needs and a single TF32 pass (10 bits) cannot give.  The role tables are with the kernels below.
+#include <type_traits>
 #include "common.cuh"
 #include "lift.cuh"
 #include "tc_ptx.cuh"
@@ -767,6 +768,254 @@ __global__ void __launch_bounds__(256)
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// pw_bwd_tc_kernel: both gradients of one narrow layer (Cout = M and Cin = N in {64, 128}) in one persistent walk over
+// 64-position tiles, so that every byte the two GEMMs share — dY's g / dpool / y rows and the layer input X — leaves HBM once:
+//   dgrad  out[p, n] = sum_m dY[p, m] Wt[n, m]   (TcDgradEpi: ReLU mask, BN-backward sums, coalesced stores)
+//   wgrad  dW[m, n] += sum_p dY[p, m] X[p, n]    (accumulated in registers over the CTA's tiles, written once to
+//                                                 part[blockIdx.x] and summed in split order by wgrad_reduce_kernel)
+// wgmma takes tf32 operands K-major only, and the two GEMMs contract dY along different axes.  dY is stored once, as dgrad's
+// operand (rows = positions, m contiguous, hi | lo); wgrad's A operand dY^T is read from that image into registers in the
+// wgmma fragment layout (wgmma_tf32_rs_*), and X^T is the producers' transposed store (store_transposed), as in
+// pw_wgrad_tc_kernel.  Every value fed to an MMA is the loaders' finish() output split as the two-kernel path splits it.
+//   warps 0-3, 4-7  consumer warpgroup h: dgrad of the tile's 64 positions x channels h*N/2 .. (m64 n{32,64}, weights from its
+//                   own two-stage ring of pre-tiled images), then wgrad rows m = 64 h .. 64 h + 63 (when M = 128 or h = 0;
+//                   m64 n{64,128}), then the dgrad epilogue from accumulators staged over the dead X^T image
+//   warps 8-11      producers: dY k-blocks and X^T k-blocks of the tile, each operand's raw rows one item ahead; thread 0
+//                   also asks for the CTA's next tile's rows with cp.async.bulk.prefetch.L2
+// Shared memory: dY 4 x 16 KB | X^T 2 x 32 KB (epilogue staging 2 x 17 KB) | weight rings 2 x 2 x 16 KB | barriers, lifted slices.
+constexpr int BW_TP = 64;                               // positions per tile
+constexpr int BW_THREADS = 384;
+constexpr int BW_DY = 0, BW_XT = 64 * 1024, BW_W = 128 * 1024, BW_TAIL = 192 * 1024;
+constexpr int BW_SMEM = BW_TAIL + 256 + 1024 + 4096 + 1024;
+
+template <class XB, int N>
+__global__ void __launch_bounds__(BW_THREADS, 1)
+    pw_bwd_tc_kernel(TcDy da, XB xb, const uint8_t* __restrict__ wtiles, int P, int M, TcDgradEpi<N, std::is_same<XB, TcLift>::value> epi,
+                     float* __restrict__ part) {
+    constexpr int NH = N / 2;                           // dgrad channels per consumer warpgroup
+    constexpr int WSTAGE = 2 * NH * 128;                // one ring stage: hi | lo rows of NH channels
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* tail = smem + BW_TAIL;
+    uint64_t* dy_full = reinterpret_cast<uint64_t*>(tail);
+    uint64_t* dy_empty = dy_full + 1;
+    uint64_t* xt_full = dy_full + 2;
+    uint64_t* xt_empty = dy_full + 3;
+    uint64_t* wfull = dy_full + 4;                      // [2 warpgroups][2 stages]
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nkb = M / TC_K;                           // dY k-blocks (dgrad's K)
+    const int n_ptiles = (P + BW_TP - 1) / BW_TP;
+    const int my_tiles = blockIdx.x < n_ptiles ? (n_ptiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+
+    if (threadIdx.x == 0) {
+        o3d_mbar_init(dy_full, 128);
+        o3d_mbar_init(dy_empty, 8);
+        o3d_mbar_init(xt_full, 128);
+        o3d_mbar_init(xt_empty, 8);
+        for (int s = 0; s < 4; ++s) o3d_mbar_init(wfull + s, 1);
+        o3d_fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp < 8) {
+        const int h = warp >> 2, w = warp & 3, tw = threadIdx.x & 127;
+        uint8_t* wring = smem + BW_W + h * 2 * WSTAGE;
+        const int n_witems = my_tiles * nkb;            // this warpgroup's weight images: (tile, k-block) in walk order
+        auto load_w = [&](int item) {                   // rows h*NH .. of the image of k-block item % nkb, hi and lo
+            const int s = item & 1;
+            const uint8_t* src = wtiles + (size_t)(item % nkb) * (2 * TILE_BYTES) + h * NH * 128;
+            o3d_mbar_expect_tx(wfull + 2 * h + s, WSTAGE);
+            o3d_bulk_g2s(wring + s * WSTAGE, src, NH * 128, wfull + 2 * h + s);
+            o3d_bulk_g2s(wring + s * WSTAGE + NH * 128, src + TILE_BYTES, NH * 128, wfull + 2 * h + s);
+        };
+        if (tw == 0) {
+            if (n_witems > 0) load_w(0);
+            if (n_witems > 1) load_w(1);
+        }
+        const bool do_w = 64 * h < M;                   // wgrad rows of this warpgroup
+        const int n_local = h * NH + (tw % NH);         // epilogue: thread = one output channel x NH / 2 positions
+        const int q = tw / NH;
+        constexpr int PPT = NH / 2;
+        float* stg = reinterpret_cast<float*>(smem + BW_XT + h * (NH * TC_EPI_LD * 4));
+        int32_t* gsm = reinterpret_cast<int32_t*>(tail + 256);           // [2][128] row indices (lifted X)
+        float4* ssm = reinterpret_cast<float4*>(tail + 256 + 1024);      // [2][128] per-position scalars
+        epi.begin(n_local, N);
+        float wacc[N / 2];
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) wacc[i] = 0.f;
+        int witem = 0, tphase = 0, buf = 0;
+        for (int t = blockIdx.x; t < n_ptiles; t += gridDim.x) {
+            const int pt0 = t * BW_TP;
+            {
+                const int32_t* gi = epi.lift_gidx();
+                const float* si = epi.lift_s();
+                if (gi || si) {
+                    if (tw < BW_TP) {
+                        const int pp = min(pt0 + tw, P - 1);
+                        const int slot = buf * TC_N + ((pt0 + tw) & (TC_N - 1));
+                        if (gi && h == 0) gsm[slot] = __ldg(gi + pp);
+                        if (si && h == 1) ssm[slot] = ld4g(si + (size_t)pp * 4);
+                    }
+                    asm volatile("bar.sync 1, 256;" ::: "memory");
+                    epi.set_tile(gsm + buf * TC_N, ssm + buf * TC_N);
+                }
+            }
+            const int pb = pt0 + q * PPT;
+            // ---- dgrad: D[64 positions, NH channels] over the nkb k-blocks of dY
+            float dacc[NH / 2];
+#pragma unroll
+            for (int i = 0; i < NH / 2; ++i) dacc[i] = 0.f;
+            o3d_mbar_wait(dy_full, tphase);
+            for (int kb = 0; kb < nkb; ++kb, ++witem) {
+                o3d_mbar_wait(wfull + 2 * h + (witem & 1), (witem >> 1) & 1);
+                const uint32_t ab = o3d_smem_u32(smem + BW_DY + kb * TILE_BYTES);   // hi | lo, 8 KB each
+                const uint32_t bb = o3d_smem_u32(wring + (witem & 1) * WSTAGE);
+                wgmma_fence_acc(dacc);
+                wgmma_fence();
+                wgmma_3xtf32_kblock<NH>(dacc, make_desc(ab), make_desc(ab + TILE_BYTES / 2), make_desc(bb), make_desc(bb + NH * 128),
+                                        kb == 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(dacc);
+                asm volatile("bar.sync %0, 128;" ::"r"(2 + h) : "memory");   // the warpgroup is done with this ring stage
+                if (tw == 0 && witem + 2 < n_witems) load_w(witem + 2);
+            }
+            // ---- wgrad: dW[64 h + 0..63, 0..N-1] += dY^T . X over the tile's 64 positions (8 k-steps)
+            o3d_mbar_wait(xt_full, tphase);
+            if (do_w) {
+                const int mr = 16 * w + (lane >> 2);                 // fragment rows mr, mr + 8 of this warpgroup's 64
+                const uint8_t* dyk = smem + BW_DY + (2 * h + (w >> 1)) * (TILE_BYTES);   // k-block of channels 64 h + mr
+                const int mc = mr & 31;
+                const uint32_t xt = o3d_smem_u32(smem + BW_XT);
+#pragma unroll 1
+                for (int ks = 0; ks < BW_TP / 8; ++ks) {
+                    uint32_t ahi[4], alo[4];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const int p = ks * 8 + (lane & 3) + 4 * (i >> 1), m = mc + 8 * (i & 1);
+                        const uint32_t off = sw128(p, m >> 2) + 4 * (m & 3);
+                        ahi[i] = *reinterpret_cast<const uint32_t*>(dyk + off);
+                        alo[i] = *reinterpret_cast<const uint32_t*>(dyk + TILE_BYTES / 2 + off);
+                    }
+                    const uint32_t xb0 = xt + (ks >> 2) * (2 * TILE_BYTES) + (ks & 3) * 32;
+                    const uint64_t bhi = make_desc(xb0), blo = make_desc(xb0 + TILE_BYTES);
+                    wgmma_fence_acc(wacc);
+                    wgmma_fence();
+                    if constexpr (N == 128) {
+                        wgmma_tf32_rs_n128(wacc, alo, bhi);
+                        wgmma_tf32_rs_n128(wacc, ahi, blo);
+                        wgmma_tf32_rs_n128(wacc, ahi, bhi);
+                    } else {
+                        wgmma_tf32_rs_n64(wacc, alo, bhi);
+                        wgmma_tf32_rs_n64(wacc, ahi, blo);
+                        wgmma_tf32_rs_n64(wacc, ahi, bhi);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();                                  // the fragments' registers are re-used by the next step
+                    wgmma_fence_acc(wacc);
+                }
+            }
+            __syncwarp();
+            if (lane == 0) o3d_mbar_arrive(dy_empty);
+            // the first column group's input rows are requested only now: held across the MMAs they would push the lifted
+            // instantiations past the register budget
+            epi.prefetch(n_local, N, pb, P);
+            asm volatile("bar.sync 4, 256;" ::: "memory");           // both warpgroups are done with X^T: staging goes over it
+            stage_acc(dacc, stg, TC_EPI_LD);
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + h) : "memory");
+            const float* row = stg + (tw % NH) * TC_EPI_LD + q * PPT;
+#pragma unroll 1
+            for (int cg = 0; cg < PPT / 16; ++cg) {
+                uint32_t r[16];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float4 v = *reinterpret_cast<const float4*>(row + cg * 16 + 4 * j);
+                    r[4 * j] = __float_as_uint(v.x); r[4 * j + 1] = __float_as_uint(v.y);
+                    r[4 * j + 2] = __float_as_uint(v.z); r[4 * j + 3] = __float_as_uint(v.w);
+                }
+                epi.group(r, n_local, N, pb + cg * 16, P);
+                if (cg + 1 < PPT / 16) epi.prefetch(n_local, N, pb + (cg + 1) * 16, P);
+            }
+            __syncwarp();
+            if (lane == 0) o3d_mbar_arrive(xt_empty);
+            tphase ^= 1;
+            buf ^= 1;
+        }
+        epi.end(n_local, N);
+        if (do_w) {
+            float* __restrict__ out = part + (size_t)blockIdx.x * TC_M * TC_N;
+#pragma unroll
+            for (int i = 0; i < N / 2; i += 4) {
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+                    const int m = 64 * h + 16 * w + (lane >> 2) + 8 * rr, n = 8 * (i >> 2) + 2 * (lane & 3);
+                    *reinterpret_cast<float2*>(out + (size_t)m * TC_N + n) = make_float2(wacc[i + 2 * rr], wacc[i + 2 * rr + 1]);
+                }
+            }
+        }
+    } else {
+        // ===================================================== producers (4 warps, 128 threads)
+        const int pt = threadIdx.x - 256;
+        const int chunk = pt & 7, row0 = (pt >> 3) * 4;               // dY: 4 neighbouring rows, 4 channels of a k-block
+        const int pw = warp - 8, c4 = pw * 4 + (lane & 3), prow0 = lane >> 2;   // X^T: 4 channels x positions prow0 + 8 i
+        constexpr int NXH = N / 64;                                   // X^T pieces per 32-position k-block (64 channels each)
+        const int n_items_x = 2 * NXH;
+        // dY items (tile, kb) and X^T items (tile, j = 32-position half, channel half) are two flat sequences, each walked
+        // with its raw rows one item ahead
+        struct It { int t, i; };
+        TcDy::Batch<4> ra{};
+        typename XB::template Batch<4> rb{};
+        It ca{(int)blockIdx.x, 0}, cb{(int)blockIdx.x, 0};
+        auto fetch_a = [&](const It& c) {
+            if (c.t < n_ptiles) da.fetch(ra, c.t * BW_TP + row0, 1, P, c.i * TC_K + chunk * 4, M);
+        };
+        auto fetch_b = [&](const It& c) {
+            if (c.t < n_ptiles)
+                xb.fetch(rb, c.t * BW_TP + (c.i >> (NXH - 1)) * TC_K + prow0, 8, P, (c.i & (NXH - 1)) * 64 + c4 * 4, N);
+        };
+        fetch_a(ca);
+        fetch_b(cb);
+        if (pt == 0 && ca.t < n_ptiles) { da.prefetch_rows(ca.t * BW_TP, BW_TP, P); xb.prefetch_rows(ca.t * BW_TP, BW_TP, P); }
+        int tphase = 0;
+        for (int t = blockIdx.x; t < n_ptiles; t += gridDim.x) {
+            const int pt0 = t * BW_TP;
+            if (pt == 0) {
+                const int tn = t + (int)gridDim.x;
+                if (tn < n_ptiles) { da.prefetch_rows(tn * BW_TP, BW_TP, P); xb.prefetch_rows(tn * BW_TP, BW_TP, P); }
+            }
+            o3d_mbar_wait(dy_empty, tphase ^ 1);
+            for (int kb = 0; kb < nkb; ++kb) {
+                const int k = kb * TC_K + chunk * 4;
+                const TcDy::Coef cf = da.prep(k, M);
+                uint8_t* hi = smem + BW_DY + kb * TILE_BYTES;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float4 v = da.finish(ra, cf, i, pt0 + row0 + i, P);
+                    const uint32_t off = sw128(row0 + i, chunk);
+                    *reinterpret_cast<float4*>(hi + off) = hi_part(v);
+                    *reinterpret_cast<float4*>(hi + TILE_BYTES / 2 + off) = lo_part(v);
+                }
+                if (++ca.i == nkb) { ca.i = 0; ca.t += gridDim.x; }
+                fetch_a(ca);
+            }
+            o3d_fence_proxy_async();
+            o3d_mbar_arrive(dy_full);
+            o3d_mbar_wait(xt_empty, tphase ^ 1);
+            for (int it = 0; it < n_items_x; ++it) {
+                const int j = it >> (NXH - 1), cl = (it & (NXH - 1)) * 64 + c4 * 4;
+                store_transposed(xb, rb, xb.prep(cl, N), smem + BW_XT + j * (2 * TILE_BYTES), cl, pt0 + j * TC_K, prow0, P);
+                if (++cb.i == n_items_x) { cb.i = 0; cb.t += gridDim.x; }
+                fetch_b(cb);
+            }
+            o3d_fence_proxy_async();
+            o3d_mbar_arrive(xt_full);
+            tphase ^= 1;
+        }
+    }
+}
+
 // Pre-tile a weight matrix W[rows, ld] (rows = output channels, k contiguous) into the per-(m_tile, k-block) shared-memory
 // images the kernel bulk-copies: [hi 16 KB | lo 16 KB], K-major SWIZZLE_128B, zero padded.
 __global__ void w_pretile_kernel(const float* __restrict__ W, int ld, int rows, int K, int nkb, uint8_t* __restrict__ out) {
@@ -1022,4 +1271,68 @@ extern "C" int o3d_pw_fwd_tc_lift(const o3d_lift_t* lf, const int32_t* gidx, con
                                   void* stream) {
     return o3d_pw_fwd_tc_lift_prec(lf, gidx, in_scale, in_shift, in_relu, wtiles, bias, P, K, N, y, ldy, sum, sumsq, S, ymax, ymin,
                                    arg, ldp, stream, false);
+}
+
+namespace {
+template <class XB, int N>
+int launch_bwd(const TcDy& da, const XB& xb, const void* wtiles_t, int P, int M, const TcDgradEpi<N, std::is_same<XB, TcLift>::value>& ep,
+               float* dw, int lddw, float* part, long long part_floats, cudaStream_t st) {
+    auto kern = pw_bwd_tc_kernel<XB, N>;
+    O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_SMEM), "o3d_pw_bwd_tc");
+    const int n_ptiles = (P + BW_TP - 1) / BW_TP;
+    int gx = o3d_num_sms();
+    if (gx > n_ptiles) gx = n_ptiles;
+    O3D_REQUIRE(part_floats >= (long long)gx * TC_M * TC_N, O3D_ERR_ARG, "o3d_pw_bwd_tc: workspace too small");
+    kern<<<gx, BW_THREADS, BW_SMEM, st>>>(da, xb, (const uint8_t*)wtiles_t, P, M, ep, part);
+    O3D_CHECK_LAUNCH("o3d_pw_bwd_tc");
+    dim3 rg((N / 4 + 31) / 32, M);
+    wgrad_reduce_kernel<<<rg, 256, 0, st>>>(part, gx, TC_M, TC_N, M, N, dw, lddw);
+    O3D_CHECK_LAUNCH("o3d_pw_bwd_tc: reduce");
+    return O3D_OK;
+}
+
+template <class XB>
+int bwd_tc_impl(const TcDy& da, const XB& xb, const void* wtiles_t, int P, int Cout, int Cin, float* out, const float* yprev,
+                const LiftView* lv, const float* pscale, const float* pshift, int prelu, double* s1, double* s2y, float* dw,
+                int lddw, float* part, long long part_floats, cudaStream_t st) {
+    constexpr bool LIFT = std::is_same<XB, TcLift>::value;
+    auto fill = [&](auto& ep) {
+        if constexpr (LIFT) ep.lv = *lv;
+        ep.out = out; ep.ldo = Cin; ep.yprev = yprev; ep.ldyp = Cin; ep.scale = pscale; ep.shift = pshift; ep.relu = prelu;
+        ep.s1g = s1; ep.s2y = s2y;
+    };
+    if (Cin == 64) {
+        TcDgradEpi<64, LIFT> ep{};
+        fill(ep);
+        return launch_bwd<XB, 64>(da, xb, wtiles_t, P, Cout, ep, dw, lddw, part, part_floats, st);
+    }
+    TcDgradEpi<128, LIFT> ep{};
+    fill(ep);
+    return launch_bwd<XB, 128>(da, xb, wtiles_t, P, Cout, ep, dw, lddw, part, part_floats, st);
+}
+}  // namespace
+
+extern "C" int o3d_pw_bwd_tc(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                             const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, const float* x,
+                             const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu,
+                             int P, int Cout, int Cin, float* out, double* s1, double* s2y, float* dw, int lddw, float* part,
+                             long long part_floats, void* stream) {
+    O3D_REQUIRE((g || dpool) && wtiles_t && (x || lf) && out && dw && part, O3D_ERR_ARG, "o3d_pw_bwd_tc: null pointer");
+    O3D_REQUIRE((Cout == 64 || Cout == 128) && (Cin == 64 || Cin == 128) && (lddw & 3) == 0, O3D_ERR_ARG,
+                "o3d_pw_bwd_tc: channel counts must be 64 or 128");
+    O3D_REQUIRE(!lf || ((gidx || !lf->z) && (lf->z || lf->s) && lf->ldz == Cin), O3D_ERR_ARG, "o3d_pw_bwd_tc: lift descriptor");
+    if (P == 0) return O3D_OK;
+    const TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1)};
+    cudaStream_t st = (cudaStream_t)stream;
+    if (lf) {
+        TcLift xb = make_tclift(lf, gidx, in_scale, in_shift, in_relu);
+        const LiftView lv = xb.lv;
+        return bwd_tc_impl(da, xb, wtiles_t, P, Cout, Cin, out, nullptr, &lv, in_scale, in_shift, in_relu, s1, s2y, dw, lddw, part,
+                           part_floats, st);
+    }
+    // the ReLU mask / BN-backward sums read the layer input's raw rows when the previous layer has a BN or a ReLU
+    const float* yprev = (in_scale || in_relu) ? x : nullptr;
+    const TcAct xb{x, Cin, in_scale, in_shift, in_relu};
+    return bwd_tc_impl(da, xb, wtiles_t, P, Cout, Cin, out, yprev, nullptr, in_scale, in_shift, in_relu, s1, s2y, dw, lddw, part,
+                       part_floats, st);
 }

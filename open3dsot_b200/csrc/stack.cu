@@ -138,6 +138,7 @@ struct Plan {
     // tensor-core kernels per layer: forward, dgrad, weight gradient (split-K over positions into the `wpart` workspace, partial
     // tiles summed in a fixed order: deterministic)
     bool tc_f[O3D_MAX_LAYERS], tc_b[O3D_MAX_LAYERS], tc_w[O3D_MAX_LAYERS];
+    bool fused_bwd[O3D_MAX_LAYERS];   // dgrad and wgrad of the layer in one kernel (o3d_pw_bwd_tc)
     // forward (persisted) offsets
     size_t wp[O3D_MAX_LAYERS], wt[O3D_MAX_LAYERS], bias[O3D_MAX_LAYERS], y[O3D_MAX_LAYERS], vec[O3D_MAX_LAYERS],
         stat[O3D_MAX_LAYERS], tiles[O3D_MAX_LAYERS];
@@ -177,6 +178,15 @@ bool make_plan(const o3d_stack_t* d, Plan& p) {
         p.virt = p.tc_f[1] && p.tc_b[1] && (p.tc_w[1] || !d->training) && tc_main(p.K[1]) == p.K[1] && p.K[1] % 32 == 0;
         if (p.virt) p.tc_w[1] = true;
     }
+    // Both gradients of a narrow layer in one pass over its operands (o3d_pw_bwd_tc): 64 or 128 channels on both sides.  Every
+    // CTA writes, and the reduction re-reads, a whole 128 x 128 partial tile (8.6 MB per layer on 132 SMs), which pays only
+    // once the stream the fused kernel saves (3 P C floats) is several times larger: on an H100, a dense 128 -> 128 layer is
+    // 4 % slower fused at P = 32,768 and 11 % faster at 65,536 (DESIGN.md section 5).  The crossover also stays above the P
+    // (<= ~51k) at which tests/test_gpu_stack_paths.py and test_gpu_lift_paths.py pin the two-kernel backward.
+    constexpr int P_FUSED_BWD = 65536;
+    for (int l = 0; l < p.n; ++l)
+        p.fused_bwd[l] = d->training && p.tc_b[l] && p.tc_w[l] && (p.Nw[l] == 64 || p.Nw[l] == 128) &&
+                         (p.K[l] == 64 || p.K[l] == 128) && d->P >= P_FUSED_BWD;
     // statistics block first (one memset)
     p.stat_all = o;
     for (int l = 0; l < p.n; ++l) { p.stat[l] = o; o += al(sizeof(double) * 2 * p.Nw[l]); }
@@ -462,6 +472,19 @@ extern "C" int o3d_stack_backward(const o3d_stack_t* d, const float* x, const vo
         const float* psc = (l > 0 && d->has_bn[l - 1]) ? pvec : nullptr;
         const float* psh = (l > 0 && d->has_bn[l - 1]) ? pvec + Kp : nullptr;
         const int prelu = l > 0 ? d->relu[l - 1] : 0;
+        if (p.fused_bwd[l] && (l > 0 || dx) && d->d_weight[l]) {
+            float* gout = l > 0 ? at<float>(wb, p.gbuf[gsel]) : dx;
+            const bool want = l > 0 && (d->has_bn[l - 1] || d->bias[l - 1] != nullptr);
+            const bool lifted = l == 1 && p.virt;
+            rc = o3d_pw_bwd_tc(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, wf + p.btiles[l], lifted ? nullptr : xin,
+                               lifted ? d->lift : nullptr, lifted ? at<int32_t>(wf, p.gidx) : nullptr, psc, psh, prelu, p.P, Nl, K,
+                               gout, want ? s1(l - 1) : nullptr, want ? s1(l - 1) + K : nullptr, at<float>(wb, p.dwp[l]), K,
+                               at<float>(wb, p.wpart), p.wpart_floats, stream);
+            if (rc) return rc;
+            g = gout;
+            gsel ^= 1;
+            continue;
+        }
         if (l > 0 || dx) {
             float* gout = l > 0 ? at<float>(wb, p.gbuf[gsel]) : dx;
             const bool mask = l > 0 && (d->has_bn[l - 1] || d->relu[l - 1]);
