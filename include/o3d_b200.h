@@ -274,7 +274,15 @@ typedef struct o3d_stack_t {
                                  refuse a training descriptor.  The block then holds one bf16 image per weight tile (2 bytes per
                                  weight instead of 8) and the forward takes the bf16 pw_tc / sa_fused kernels.  Layers that the
                                  plan sends to the exact-fp32 CUDA-core kernels (K < 32, P < 16, ...) stay fp32 either way;
-                                 accumulation, BatchNorm, ReLU, pooling and the first SA layer's coordinate term are fp32 too. */
+                                 accumulation, BatchNorm, ReLU, pooling and the first SA layer's coordinate term are fp32 too.
+                                 2 = BF16 training: BF16 operands with FP32 accumulation for the tensor-core forward, dgrad and
+                                 wgrad GEMMs.  Valid with training = 1 only (with or without keep_for_backward, and in
+                                 o3d_stack_backward); the size and prepare calls refuse it for an eval-mode descriptor.  The
+                                 weights are rounded to bf16 once per call when they are packed (the forward and the dgrad
+                                 images, 8 KB per tile instead of 32 KB), and each GEMM input row where 3xTF32 would split it.
+                                 The stored pre-BN outputs, batch statistics, BN-backward sums, ReLU masks, pooling, the split-K
+                                 partial tiles and their fixed-order reduction, the lifted layer's gather / scatter passes and
+                                 every CUDA-core layer stay fp32.                                                          */
 } o3d_stack_t;
 
 long long o3d_stack_workspace_bytes(const o3d_stack_t* d, int backward);

@@ -109,8 +109,8 @@ class StackDesc(ctypes.Structure):
                 ("lift", ctypes.POINTER(LiftDesc)), ("accumulate", _i), ("prepared", _p),
                 ("precision", _i)]
 
-# o3d_stack_t.precision
-PRECISION_TF32X3, PRECISION_BF16 = 0, 1
+# o3d_stack_t.precision: 3xTF32 (default), BF16 inference (eval mode only), BF16 training (training mode only)
+PRECISION_TF32X3, PRECISION_BF16, PRECISION_BF16_TRAIN = 0, 1, 2
 
 _lib = None
 

@@ -175,5 +175,29 @@ struct o3d_lift_t;
 int o3d_pw_fwd_tc_lift_prec(const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu,
                             const void* wtiles, const float* bias, int P, int K, int N, float* y, int ldy, double* sum,
                             double* sumsq, int S, float* ymax, float* ymin, int32_t* arg, int ldp, void* stream, bool bf16);
+// The training backward's tensor-core GEMMs (o3d_pw_dgrad_tc, o3d_pw_dgrad_tc_lift, o3d_pw_wgrad_tc2, o3d_pw_wgrad_tc_lift,
+// o3d_pw_bwd_tc) with the operand precision.  bf16 (o3d_stack_t.precision = 2): BF16 operands, FP32 accumulation, and
+// wtiles_t holds the bf16 dgrad images.
+int o3d_pw_dgrad_tc_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                         const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, int P, int Cout, int Cin,
+                         float* out, int ldo, const float* yprev, int ldyp, const float* pscale, const float* pshift, int prelu,
+                         double* s1, double* s2y, void* stream, bool bf16);
+int o3d_pw_dgrad_tc_lift_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                              const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, int P, int Cout,
+                              int Cin, float* out, int ldo, const o3d_lift_t* lf, const int32_t* gidx, const float* pscale,
+                              const float* pshift, int prelu, double* s1, double* s2y, void* stream, bool bf16);
+int o3d_pw_wgrad_tc2_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                          const float* dpool, const int32_t* sel, int S, int ldp, const float* x, int ldx, const float* in_scale,
+                          const float* in_shift, int in_relu, int P, int Cout, int Cin, float* dw, int lddw, float* part,
+                          long long part_floats, void* stream, bool bf16);
+int o3d_pw_wgrad_tc_lift_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                              const float* dpool, const int32_t* sel, int S, int ldp, const o3d_lift_t* lf, const int32_t* gidx,
+                              const float* in_scale, const float* in_shift, int in_relu, int P, int Cout, int Cin, float* dw,
+                              int lddw, float* part, long long part_floats, void* stream, bool bf16);
+int o3d_pw_bwd_tc_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                       const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, const float* x,
+                       const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu, int P,
+                       int Cout, int Cin, float* out, double* s1, double* s2y, float* dw, int lddw, float* part,
+                       long long part_floats, void* stream, bool bf16);
 
 #endif

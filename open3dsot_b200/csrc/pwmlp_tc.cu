@@ -225,12 +225,15 @@ struct TcDy {
     }
 };
 
-// BF16 operands (inference precision 1): the same loader, its transformed rows rounded to bf16 (cvt.rn) where the 3xTF32
-// path splits them into hi / lo; the kernel then stores one bf16 image per stage and issues 2 wgmma k16 per k-block.  A wrapper
-// type rather than a flag, so that each precision is its own instantiation with no runtime branch in the hot loop.
+// BF16 operands (o3d_stack_t.precision 1, inference, and 2, training): the same loader, its transformed rows rounded to bf16
+// (cvt.rn) where the 3xTF32 path splits them into hi / lo; the kernel then stores one bf16 image per stage and issues 2 wgmma
+// k16 per 32-wide k-block.  A wrapper type rather than a flag, so that each precision is its own instantiation with no runtime
+// branch in the hot loop.
 template <class L> struct Bf16 : L {};
 template <class L> struct is_bf16 { static constexpr bool value = false; };
 template <class L> struct is_bf16<Bf16<L>> { static constexpr bool value = true; };
+template <class L> struct is_lift { static constexpr bool value = std::is_same<L, TcLift>::value; };
+template <class L> struct is_lift<Bf16<L>> { static constexpr bool value = is_lift<L>::value; };
 
 // ---- epilogues: thread = one output channel `ch`, called once per 32-position column group ------------------
 // LD: compile-time row stride of y (0 = use the runtime ldy)
@@ -648,9 +651,26 @@ __device__ __forceinline__ void store_transposed(const L& ld, const typename L::
     }
 }
 
+// BF16 (XB = Bf16<...>): no transpose.  The producers store both operands' rows position-major into the 64-byte-swizzle image
+// of the forward path, dY at the stage's start and X WG_BF_X bytes on, each as four 32-channel sub-images of 32 positions
+// (WG_BF_SUB bytes apart); the consumers read them MN-major (wgmma_bf16_tt_*, make_desc_sw64_mn): 2 k16 MMAs per k-block.
+constexpr int WG_BF_SUB = TC_K * TC_BF_ROW;             // 2 KB: 32 positions x 32 channels
+constexpr int WG_BF_X = 4 * WG_BF_SUB;
+
+template <class L>
+__device__ __forceinline__ void store_rows_bf16(const L& ld, const typename L::template Batch<4>& raw, const typename L::Coef& cf,
+                                                uint8_t* img, int sub, int c_local, int p_first, int prow0, int pend) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int pl = prow0 + 8 * i;
+        st_bf16_row4(img, sub, pl, c_local, ld.finish(raw, cf, i, p_first + pl, pend));
+    }
+}
+
 template <class XB>
 __global__ void __launch_bounds__(WG_THREADS, 1)
     pw_wgrad_tc_kernel(TcDy da, XB xb, int P, int M, int N, int chunk, float* __restrict__ part) {
+    constexpr bool BF = is_bf16<XB>::value;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * 4 * TILE_BYTES);
@@ -681,11 +701,19 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
         for (int kb = 0; kb < nkb; ++kb) {
             o3d_mbar_wait(full + stage, phase);
             const uint32_t sb = o3d_smem_u32(smem + stage * 4 * TILE_BYTES);
-            const uint32_t ab = sb + h * (TILE_BYTES / 2);                 // dY rows (channels) m0 + h*64 ..
             wgmma_fence_acc(acc);
             wgmma_fence();
-            wgmma_3xtf32_kblock<128>(acc, make_desc(ab), make_desc(ab + TILE_BYTES), make_desc(sb + 2 * TILE_BYTES),
-                                     make_desc(sb + 3 * TILE_BYTES), kb == 0);
+            if constexpr (BF) {
+                const uint32_t ab = sb + h * 2 * WG_BF_SUB;                   // dY channels m0 + h*64 .. : sub-images 2h, 2h+1
+#pragma unroll
+                for (int ks = 0; ks < 2; ++ks)
+                    wgmma_bf16_tt_n128(acc, make_desc_sw64_mn(ab + ks * 1024, WG_BF_SUB),
+                                       make_desc_sw64_mn(sb + WG_BF_X + ks * 1024, WG_BF_SUB), (kb == 0 && ks == 0) ? 0u : 1u);
+            } else {
+                const uint32_t ab = sb + h * (TILE_BYTES / 2);                 // dY rows (channels) m0 + h*64 ..
+                wgmma_3xtf32_kblock<128>(acc, make_desc(ab), make_desc(ab + TILE_BYTES), make_desc(sb + 2 * TILE_BYTES),
+                                         make_desc(sb + 3 * TILE_BYTES), kb == 0);
+            }
             wgmma_commit();
             wgmma_wait<0>();
             wgmma_fence_acc(acc);
@@ -729,8 +757,13 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
             uint8_t* sbase = smem + stage * 4 * TILE_BYTES;
             // the per-channel coefficients are re-read (L1-resident) per k-block: kept live across the loop they push the
             // lifted operand's producer past the 128-register budget
-            store_transposed(da, ra, da.prep(m0 + c4 * 4, M), sbase, c4 * 4, kpos(kb), prow0, pend);
-            store_transposed(xb, rb, xb.prep(n0 + c4 * 4, N), sbase + 2 * TILE_BYTES, c4 * 4, kpos(kb), prow0, pend);
+            if constexpr (BF) {
+                store_rows_bf16(da, ra, da.prep(m0 + c4 * 4, M), sbase, WG_BF_SUB, c4 * 4, kpos(kb), prow0, pend);
+                store_rows_bf16(xb, rb, xb.prep(n0 + c4 * 4, N), sbase + WG_BF_X, WG_BF_SUB, c4 * 4, kpos(kb), prow0, pend);
+            } else {
+                store_transposed(da, ra, da.prep(m0 + c4 * 4, M), sbase, c4 * 4, kpos(kb), prow0, pend);
+                store_transposed(xb, rb, xb.prep(n0 + c4 * 4, N), sbase + 2 * TILE_BYTES, c4 * 4, kpos(kb), prow0, pend);
+            }
             o3d_fence_proxy_async();
             o3d_mbar_arrive(full + stage);
             if (kb + 1 < nkb) fetch(kb + 1);
@@ -788,13 +821,19 @@ constexpr int BW_TP = 64;                               // positions per tile
 constexpr int BW_THREADS = 384;
 constexpr int BW_DY = 0, BW_XT = 64 * 1024, BW_W = 128 * 1024, BW_TAIL = 192 * 1024;
 constexpr int BW_SMEM = BW_TAIL + 256 + 1024 + 4096 + 1024;
+// BF16 (XB = Bf16<...>): dY is stored once as a bf16 64-byte-swizzle image, rows = positions, one 4 KB image per 32-channel
+// k-block.  dgrad reads it as its K-major A operand; wgrad reads the same image MN-major (transposed) as its A operand, in place
+// of the register-fed dY^T fragments.  X is stored position-major the same way (one 4 KB image per 32 channels) as wgrad's
+// MN-major B operand, with no transposed store, and the weight ring carries the bf16 dgrad images (one k16 pair per k-block).
+constexpr int BW_BF_SUB = BW_TP * TC_BF_ROW;            // 4 KB: 64 positions x 32 channels
 
 template <class XB, int N>
 __global__ void __launch_bounds__(BW_THREADS, 1)
-    pw_bwd_tc_kernel(TcDy da, XB xb, const uint8_t* __restrict__ wtiles, int P, int M, TcDgradEpi<N, std::is_same<XB, TcLift>::value> epi,
+    pw_bwd_tc_kernel(TcDy da, XB xb, const uint8_t* __restrict__ wtiles, int P, int M, TcDgradEpi<N, is_lift<XB>::value> epi,
                      float* __restrict__ part) {
+    constexpr bool BF = is_bf16<XB>::value;
     constexpr int NH = N / 2;                           // dgrad channels per consumer warpgroup
-    constexpr int WSTAGE = 2 * NH * 128;                // one ring stage: hi | lo rows of NH channels
+    constexpr int WSTAGE = BF ? NH * TC_BF_ROW : 2 * NH * 128;   // one ring stage: the bf16 rows, or hi | lo rows of NH channels
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* tail = smem + BW_TAIL;
@@ -825,10 +864,15 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
         const int n_witems = my_tiles * nkb;            // this warpgroup's weight images: (tile, k-block) in walk order
         auto load_w = [&](int item) {                   // rows h*NH .. of the image of k-block item % nkb, hi and lo
             const int s = item & 1;
-            const uint8_t* src = wtiles + (size_t)(item % nkb) * (2 * TILE_BYTES) + h * NH * 128;
             o3d_mbar_expect_tx(wfull + 2 * h + s, WSTAGE);
-            o3d_bulk_g2s(wring + s * WSTAGE, src, NH * 128, wfull + 2 * h + s);
-            o3d_bulk_g2s(wring + s * WSTAGE + NH * 128, src + TILE_BYTES, NH * 128, wfull + 2 * h + s);
+            if constexpr (BF) {
+                const uint8_t* src = wtiles + (size_t)(item % nkb) * BF_TILE_BYTES + h * NH * TC_BF_ROW;
+                o3d_bulk_g2s(wring + s * WSTAGE, src, WSTAGE, wfull + 2 * h + s);
+            } else {
+                const uint8_t* src = wtiles + (size_t)(item % nkb) * (2 * TILE_BYTES) + h * NH * 128;
+                o3d_bulk_g2s(wring + s * WSTAGE, src, NH * 128, wfull + 2 * h + s);
+                o3d_bulk_g2s(wring + s * WSTAGE + NH * 128, src + TILE_BYTES, NH * 128, wfull + 2 * h + s);
+            }
         };
         if (tw == 0) {
             if (n_witems > 0) load_w(0);
@@ -870,12 +914,16 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
             o3d_mbar_wait(dy_full, tphase);
             for (int kb = 0; kb < nkb; ++kb, ++witem) {
                 o3d_mbar_wait(wfull + 2 * h + (witem & 1), (witem >> 1) & 1);
-                const uint32_t ab = o3d_smem_u32(smem + BW_DY + kb * TILE_BYTES);   // hi | lo, 8 KB each
                 const uint32_t bb = o3d_smem_u32(wring + (witem & 1) * WSTAGE);
                 wgmma_fence_acc(dacc);
                 wgmma_fence();
-                wgmma_3xtf32_kblock<NH>(dacc, make_desc(ab), make_desc(ab + TILE_BYTES / 2), make_desc(bb), make_desc(bb + NH * 128),
-                                        kb == 0);
+                if constexpr (BF) {
+                    wgmma_bf16_kblock<NH>(dacc, make_desc_sw64(o3d_smem_u32(smem + BW_DY + kb * BW_BF_SUB)), make_desc_sw64(bb), kb == 0);
+                } else {
+                    const uint32_t ab = o3d_smem_u32(smem + BW_DY + kb * TILE_BYTES);   // hi | lo, 8 KB each
+                    wgmma_3xtf32_kblock<NH>(dacc, make_desc(ab), make_desc(ab + TILE_BYTES / 2), make_desc(bb), make_desc(bb + NH * 128),
+                                            kb == 0);
+                }
                 wgmma_commit();
                 wgmma_wait<0>();
                 wgmma_fence_acc(dacc);
@@ -884,7 +932,22 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
             }
             // ---- wgrad: dW[64 h + 0..63, 0..N-1] += dY^T . X over the tile's 64 positions (8 k-steps)
             o3d_mbar_wait(xt_full, tphase);
-            if (do_w) {
+            if constexpr (BF) {
+                if (do_w) {   // rows m = 64 h .. : dY images 2h, 2h+1 read MN-major; X images read MN-major; 4 k16 steps
+                    const uint32_t ab = o3d_smem_u32(smem + BW_DY + 2 * h * BW_BF_SUB), xb0 = o3d_smem_u32(smem + BW_XT);
+                    wgmma_fence_acc(wacc);
+                    wgmma_fence();
+#pragma unroll
+                    for (int ks = 0; ks < BW_TP / 16; ++ks) {
+                        const uint64_t ad = make_desc_sw64_mn(ab + ks * 1024, BW_BF_SUB), bd = make_desc_sw64_mn(xb0 + ks * 1024, BW_BF_SUB);
+                        if constexpr (N == 128) wgmma_bf16_tt_n128(wacc, ad, bd, 1u);
+                        else wgmma_bf16_tt_n64(wacc, ad, bd, 1u);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_acc(wacc);
+                }
+            } else if (do_w) {
                 const int mr = 16 * w + (lane >> 2);                 // fragment rows mr, mr + 8 of this warpgroup's 64
                 const uint8_t* dyk = smem + BW_DY + (2 * h + (w >> 1)) * (TILE_BYTES);   // k-block of channels 64 h + mr
                 const int mc = mr & 31;
@@ -989,13 +1052,19 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
             for (int kb = 0; kb < nkb; ++kb) {
                 const int k = kb * TC_K + chunk * 4;
                 const TcDy::Coef cf = da.prep(k, M);
-                uint8_t* hi = smem + BW_DY + kb * TILE_BYTES;
+                if constexpr (BF) {
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float4 v = da.finish(ra, cf, i, pt0 + row0 + i, P);
-                    const uint32_t off = sw128(row0 + i, chunk);
-                    *reinterpret_cast<float4*>(hi + off) = hi_part(v);
-                    *reinterpret_cast<float4*>(hi + TILE_BYTES / 2 + off) = lo_part(v);
+                    for (int i = 0; i < 4; ++i)
+                        st_bf16_row4(smem + BW_DY + kb * BW_BF_SUB, 0, row0 + i, chunk * 4, da.finish(ra, cf, i, pt0 + row0 + i, P));
+                } else {
+                    uint8_t* hi = smem + BW_DY + kb * TILE_BYTES;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const float4 v = da.finish(ra, cf, i, pt0 + row0 + i, P);
+                        const uint32_t off = sw128(row0 + i, chunk);
+                        *reinterpret_cast<float4*>(hi + off) = hi_part(v);
+                        *reinterpret_cast<float4*>(hi + TILE_BYTES / 2 + off) = lo_part(v);
+                    }
                 }
                 if (++ca.i == nkb) { ca.i = 0; ca.t += gridDim.x; }
                 fetch_a(ca);
@@ -1005,7 +1074,10 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
             o3d_mbar_wait(xt_empty, tphase ^ 1);
             for (int it = 0; it < n_items_x; ++it) {
                 const int j = it >> (NXH - 1), cl = (it & (NXH - 1)) * 64 + c4 * 4;
-                store_transposed(xb, rb, xb.prep(cl, N), smem + BW_XT + j * (2 * TILE_BYTES), cl, pt0 + j * TC_K, prow0, P);
+                if constexpr (BF)
+                    store_rows_bf16(xb, rb, xb.prep(cl, N), smem + BW_XT + j * (TC_K * TC_BF_ROW), BW_BF_SUB, cl, pt0 + j * TC_K, prow0, P);
+                else
+                    store_transposed(xb, rb, xb.prep(cl, N), smem + BW_XT + j * (2 * TILE_BYTES), cl, pt0 + j * TC_K, prow0, P);
                 if (++cb.i == n_items_x) { cb.i = 0; cb.t += gridDim.x; }
                 fetch_b(cb);
             }
@@ -1061,8 +1133,8 @@ int launch_fwd(const BLoad& bl, const void* wtiles, const float* bias, int P, in
     return launch_tc(bl, (const uint8_t*)wtiles, P, K, Nw, ep, reverse, st, "o3d_pw_fwd_tc");
 }
 
-template <int LD, bool LIFT = false>
-int launch_dgrad(const TcDy& bl, const void* wtiles_t, int P, int Cout, int Cin, float* out, int ldo, const float* yprev,
+template <int LD, bool LIFT = false, class BL>
+int launch_dgrad(const BL& bl, const void* wtiles_t, int P, int Cout, int Cin, float* out, int ldo, const float* yprev,
                  int ldyp, const float* pscale, const float* pshift, int prelu, double* s1, double* s2y, cudaStream_t st,
                  const LiftView* lv = nullptr) {
     if constexpr (!LIFT) {
@@ -1133,21 +1205,32 @@ namespace {
 int dgrad_tc_impl(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
                   const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, int P, int Cout, int Cin,
                   float* out, int ldo, const float* yprev, int ldyp, const float* pscale, const float* pshift, int prelu,
-                  double* s1, double* s2y, void* stream, const LiftView* lv) {
+                  double* s1, double* s2y, void* stream, const LiftView* lv, bool bf16) {
     O3D_REQUIRE((g || dpool) && wtiles_t && out, O3D_ERR_ARG, "o3d_pw_dgrad_tc: null pointer");
     O3D_REQUIRE((Cout & 3) == 0 && (Cin & 3) == 0, O3D_ERR_ARG, "o3d_pw_dgrad_tc: channel counts must be multiples of 4");
     if (P == 0) return O3D_OK;
     TcDy bl{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1)};
     cudaStream_t st = (cudaStream_t)stream;
     const int ld = (!yprev || ldyp == ldo) ? ldo : 0;   // one compile-time stride serves both out and yprev
-#define O3D_DG_ARGS bl, wtiles_t, P, Cout, Cin, out, ldo, yprev, ldyp, pscale, pshift, prelu, s1, s2y, st, lv
-    if (ld == 64) return launch_dgrad<64>(O3D_DG_ARGS);
-    if (ld == 128) return launch_dgrad<128>(O3D_DG_ARGS);
-    if (ld == 256) return launch_dgrad<256>(O3D_DG_ARGS);
-    return launch_dgrad<0>(O3D_DG_ARGS);
+    auto run = [&](const auto& ldr) {
+#define O3D_DG_ARGS ldr, wtiles_t, P, Cout, Cin, out, ldo, yprev, ldyp, pscale, pshift, prelu, s1, s2y, st, lv
+        if (ld == 64) return launch_dgrad<64>(O3D_DG_ARGS);
+        if (ld == 128) return launch_dgrad<128>(O3D_DG_ARGS);
+        if (ld == 256) return launch_dgrad<256>(O3D_DG_ARGS);
+        return launch_dgrad<0>(O3D_DG_ARGS);
 #undef O3D_DG_ARGS
+    };
+    return bf16 ? run(Bf16<TcDy>{bl}) : run(bl);   // bf16: wtiles_t holds bf16 images (o3d_stack_t.precision = 2)
 }
 }  // namespace
+
+int o3d_pw_dgrad_tc_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                         const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, int P, int Cout, int Cin,
+                         float* out, int ldo, const float* yprev, int ldyp, const float* pscale, const float* pshift, int prelu,
+                         double* s1, double* s2y, void* stream, bool bf16) {
+    return dgrad_tc_impl(g, ldg, y, ldy, a, b, cc, dpool, sel, S, ldp, wtiles_t, P, Cout, Cin, out, ldo, yprev, ldyp, pscale,
+                         pshift, prelu, s1, s2y, stream, nullptr, bf16);
+}
 
 extern "C" int o3d_pw_dgrad_tc(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b,
                                const float* cc, const float* dpool, const int32_t* sel, int S, int ldp,
@@ -1155,19 +1238,27 @@ extern "C" int o3d_pw_dgrad_tc(const float* g, int ldg, const float* y, int ldy,
                                int ldyp, const float* pscale, const float* pshift, int prelu, double* s1, double* s2y,
                                void* stream) {
     return dgrad_tc_impl(g, ldg, y, ldy, a, b, cc, dpool, sel, S, ldp, wtiles_t, P, Cout, Cin, out, ldo, yprev, ldyp, pscale,
-                         pshift, prelu, s1, s2y, stream, nullptr);
+                         pshift, prelu, s1, s2y, stream, nullptr, false);
 }
 
 // dgrad whose input side is a lifted first layer: the ReLU mask and the BatchNorm-backward sums use Y0 gathered from Z
+int o3d_pw_dgrad_tc_lift_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                              const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, int P, int Cout,
+                              int Cin, float* out, int ldo, const o3d_lift_t* lf, const int32_t* gidx, const float* pscale,
+                              const float* pshift, int prelu, double* s1, double* s2y, void* stream, bool bf16) {
+    O3D_REQUIRE(lf && (gidx || !lf->z) && (lf->z || lf->s) && lf->ldz == Cin, O3D_ERR_ARG, "o3d_pw_dgrad_tc_lift: lift descriptor");
+    const LiftView lv{lf->z, lf->ldz, lf->z ? gidx : nullptr, lf->s, lf->u};
+    return dgrad_tc_impl(g, ldg, y, ldy, a, b, cc, dpool, sel, S, ldp, wtiles_t, P, Cout, Cin, out, ldo, nullptr, 0, pscale,
+                         pshift, prelu, s1, s2y, stream, &lv, bf16);
+}
+
 extern "C" int o3d_pw_dgrad_tc_lift(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b,
                                     const float* cc, const float* dpool, const int32_t* sel, int S, int ldp,
                                     const void* wtiles_t, int P, int Cout, int Cin, float* out, int ldo,
                                     const o3d_lift_t* lf, const int32_t* gidx, const float* pscale, const float* pshift,
                                     int prelu, double* s1, double* s2y, void* stream) {
-    O3D_REQUIRE(lf && (gidx || !lf->z) && (lf->z || lf->s) && lf->ldz == Cin, O3D_ERR_ARG, "o3d_pw_dgrad_tc_lift: lift descriptor");
-    const LiftView lv{lf->z, lf->ldz, lf->z ? gidx : nullptr, lf->s, lf->u};
-    return dgrad_tc_impl(g, ldg, y, ldy, a, b, cc, dpool, sel, S, ldp, wtiles_t, P, Cout, Cin, out, ldo, nullptr, 0, pscale,
-                         pshift, prelu, s1, s2y, stream, &lv);
+    return o3d_pw_dgrad_tc_lift_prec(g, ldg, y, ldy, a, b, cc, dpool, sel, S, ldp, wtiles_t, P, Cout, Cin, out, ldo, lf, gidx, pscale,
+                                     pshift, prelu, s1, s2y, stream, false);
 }
 
 namespace {
@@ -1208,25 +1299,33 @@ extern "C" long long o3d_pw_wgrad_tc2_workspace_floats(void) {
     return (long long)o3d_num_sms() * TC_M * TC_N;   // splits <= #SMs / tiles of dW, so splits * Mt * Nt <= #SMs * 128 * 128
 }
 
-extern "C" int o3d_pw_wgrad_tc2(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b,
-                                const float* cc, const float* dpool, const int32_t* sel, int S, int ldp, const float* x,
-                                int ldx, const float* in_scale, const float* in_shift, int in_relu, int P, int Cout,
-                                int Cin, float* dw, int lddw, float* part, long long part_floats, void* stream) {
+int o3d_pw_wgrad_tc2_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                          const float* dpool, const int32_t* sel, int S, int ldp, const float* x, int ldx, const float* in_scale,
+                          const float* in_shift, int in_relu, int P, int Cout, int Cin, float* dw, int lddw, float* part,
+                          long long part_floats, void* stream, bool bf16) {
     O3D_REQUIRE((g || dpool) && x && dw && part, O3D_ERR_ARG, "o3d_pw_wgrad_tc2: null pointer");
     O3D_REQUIRE((Cout & 3) == 0 && (Cin & 3) == 0 && (ldx & 3) == 0 && (lddw & 3) == 0, O3D_ERR_ARG,
                 "o3d_pw_wgrad_tc2: channel counts / leading dimensions must be multiples of 4");
     if (P == 0) return O3D_OK;
     TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1)};
     TcAct xb{x, ldx, in_scale, in_shift, in_relu};
+    if (bf16) return launch_wgrad(da, Bf16<TcAct>{xb}, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
     return launch_wgrad(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
 }
 
+extern "C" int o3d_pw_wgrad_tc2(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b,
+                                const float* cc, const float* dpool, const int32_t* sel, int S, int ldp, const float* x,
+                                int ldx, const float* in_scale, const float* in_shift, int in_relu, int P, int Cout,
+                                int Cin, float* dw, int lddw, float* part, long long part_floats, void* stream) {
+    return o3d_pw_wgrad_tc2_prec(g, ldg, y, ldy, a, b, cc, dpool, sel, S, ldp, x, ldx, in_scale, in_shift, in_relu, P, Cout, Cin,
+                                 dw, lddw, part, part_floats, stream, false);
+}
+
 // ---- lifted first layer (o3d_lift_t): the next layer's GEMMs read Y0 through TcLift / the lifted dgrad epilogue ----------
-extern "C" int o3d_pw_wgrad_tc_lift(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b,
-                                    const float* cc, const float* dpool, const int32_t* sel, int S, int ldp,
-                                    const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift,
-                                    int in_relu, int P, int Cout, int Cin, float* dw, int lddw, float* part,
-                                    long long part_floats, void* stream) {
+int o3d_pw_wgrad_tc_lift_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                              const float* dpool, const int32_t* sel, int S, int ldp, const o3d_lift_t* lf, const int32_t* gidx,
+                              const float* in_scale, const float* in_shift, int in_relu, int P, int Cout, int Cin, float* dw,
+                              int lddw, float* part, long long part_floats, void* stream, bool bf16) {
     O3D_REQUIRE((g || dpool) && lf && (gidx || !lf->z) && dw && part, O3D_ERR_ARG, "o3d_pw_wgrad_tc_lift: null pointer");
     O3D_REQUIRE((Cout & 3) == 0 && (Cin & 3) == 0 && lf->ldz == Cin && (lddw & 3) == 0, O3D_ERR_ARG,
                 "o3d_pw_wgrad_tc_lift: channel counts / leading dimensions");
@@ -1234,7 +1333,17 @@ extern "C" int o3d_pw_wgrad_tc_lift(const float* g, int ldg, const float* y, int
     TcDy da{g, ldg, y, ldy, a, b, cc, dpool, sel, S > 0 ? S : 1, ldp, ilog2_exact(S > 0 ? S : 1)};
     TcLift xb = make_tclift(lf, gidx, in_scale, in_shift, in_relu);
     xb.la = TC_K;      // a producer thread's next fetch lies one k-block of positions further
+    if (bf16) return launch_wgrad(da, Bf16<TcLift>{xb}, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
     return launch_wgrad(da, xb, P, Cout, Cin, dw, lddw, part, part_floats, (cudaStream_t)stream);
+}
+
+extern "C" int o3d_pw_wgrad_tc_lift(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b,
+                                    const float* cc, const float* dpool, const int32_t* sel, int S, int ldp,
+                                    const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift,
+                                    int in_relu, int P, int Cout, int Cin, float* dw, int lddw, float* part,
+                                    long long part_floats, void* stream) {
+    return o3d_pw_wgrad_tc_lift_prec(g, ldg, y, ldy, a, b, cc, dpool, sel, S, ldp, lf, gidx, in_scale, in_shift, in_relu, P, Cout,
+                                     Cin, dw, lddw, part, part_floats, stream, false);
 }
 
 int o3d_pw_fwd_tc_lift_prec(const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu,
@@ -1275,7 +1384,7 @@ extern "C" int o3d_pw_fwd_tc_lift(const o3d_lift_t* lf, const int32_t* gidx, con
 
 namespace {
 template <class XB, int N>
-int launch_bwd(const TcDy& da, const XB& xb, const void* wtiles_t, int P, int M, const TcDgradEpi<N, std::is_same<XB, TcLift>::value>& ep,
+int launch_bwd(const TcDy& da, const XB& xb, const void* wtiles_t, int P, int M, const TcDgradEpi<N, is_lift<XB>::value>& ep,
                float* dw, int lddw, float* part, long long part_floats, cudaStream_t st) {
     auto kern = pw_bwd_tc_kernel<XB, N>;
     O3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_SMEM), "o3d_pw_bwd_tc");
@@ -1295,7 +1404,7 @@ template <class XB>
 int bwd_tc_impl(const TcDy& da, const XB& xb, const void* wtiles_t, int P, int Cout, int Cin, float* out, const float* yprev,
                 const LiftView* lv, const float* pscale, const float* pshift, int prelu, double* s1, double* s2y, float* dw,
                 int lddw, float* part, long long part_floats, cudaStream_t st) {
-    constexpr bool LIFT = std::is_same<XB, TcLift>::value;
+    constexpr bool LIFT = is_lift<XB>::value;
     auto fill = [&](auto& ep) {
         if constexpr (LIFT) ep.lv = *lv;
         ep.out = out; ep.ldo = Cin; ep.yprev = yprev; ep.ldyp = Cin; ep.scale = pscale; ep.shift = pshift; ep.relu = prelu;
@@ -1312,11 +1421,11 @@ int bwd_tc_impl(const TcDy& da, const XB& xb, const void* wtiles_t, int P, int C
 }
 }  // namespace
 
-extern "C" int o3d_pw_bwd_tc(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
-                             const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, const float* x,
-                             const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu,
-                             int P, int Cout, int Cin, float* out, double* s1, double* s2y, float* dw, int lddw, float* part,
-                             long long part_floats, void* stream) {
+int o3d_pw_bwd_tc_prec(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                       const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, const float* x,
+                       const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu, int P,
+                       int Cout, int Cin, float* out, double* s1, double* s2y, float* dw, int lddw, float* part,
+                       long long part_floats, void* stream, bool bf16) {
     O3D_REQUIRE((g || dpool) && wtiles_t && (x || lf) && out && dw && part, O3D_ERR_ARG, "o3d_pw_bwd_tc: null pointer");
     O3D_REQUIRE((Cout == 64 || Cout == 128) && (Cin == 64 || Cin == 128) && (lddw & 3) == 0, O3D_ERR_ARG,
                 "o3d_pw_bwd_tc: channel counts must be 64 or 128");
@@ -1327,12 +1436,27 @@ extern "C" int o3d_pw_bwd_tc(const float* g, int ldg, const float* y, int ldy, c
     if (lf) {
         TcLift xb = make_tclift(lf, gidx, in_scale, in_shift, in_relu);
         const LiftView lv = xb.lv;
+        if (bf16)
+            return bwd_tc_impl(da, Bf16<TcLift>{xb}, wtiles_t, P, Cout, Cin, out, nullptr, &lv, in_scale, in_shift, in_relu, s1, s2y,
+                               dw, lddw, part, part_floats, st);
         return bwd_tc_impl(da, xb, wtiles_t, P, Cout, Cin, out, nullptr, &lv, in_scale, in_shift, in_relu, s1, s2y, dw, lddw, part,
                            part_floats, st);
     }
     // the ReLU mask / BN-backward sums read the layer input's raw rows when the previous layer has a BN or a ReLU
     const float* yprev = (in_scale || in_relu) ? x : nullptr;
     const TcAct xb{x, Cin, in_scale, in_shift, in_relu};
+    if (bf16)
+        return bwd_tc_impl(da, Bf16<TcAct>{xb}, wtiles_t, P, Cout, Cin, out, yprev, nullptr, in_scale, in_shift, in_relu, s1, s2y, dw,
+                           lddw, part, part_floats, st);
     return bwd_tc_impl(da, xb, wtiles_t, P, Cout, Cin, out, yprev, nullptr, in_scale, in_shift, in_relu, s1, s2y, dw, lddw, part,
                        part_floats, st);
+}
+
+extern "C" int o3d_pw_bwd_tc(const float* g, int ldg, const float* y, int ldy, const float* a, const float* b, const float* cc,
+                             const float* dpool, const int32_t* sel, int S, int ldp, const void* wtiles_t, const float* x,
+                             const o3d_lift_t* lf, const int32_t* gidx, const float* in_scale, const float* in_shift, int in_relu,
+                             int P, int Cout, int Cin, float* out, double* s1, double* s2y, float* dw, int lddw, float* part,
+                             long long part_floats, void* stream) {
+    return o3d_pw_bwd_tc_prec(g, ldg, y, ldy, a, b, cc, dpool, sel, S, ldp, wtiles_t, x, lf, gidx, in_scale, in_shift, in_relu, P,
+                              Cout, Cin, out, s1, s2y, dw, lddw, part, part_floats, stream, false);
 }

@@ -44,7 +44,7 @@ struct PackLayer {
     const float* src; const float* bias; float* wp; float* wt; float* bias_p; uint8_t* tiles_f; uint8_t* tiles_b;
     int cout, cin, Nw, K, xyz_first, Km /* input channels tiled for dgrad */, Npad, Kpad /* iteration space */;
 };
-struct PackArgs { PackLayer l[O3D_MAX_LAYERS]; int c0; int bf16; /* forward images in bf16 (o3d_stack_t.precision = 1) */ };
+struct PackArgs { PackLayer l[O3D_MAX_LAYERS]; int c0; int bf16; /* bf16 images (o3d_stack_t.precision = 1 or 2) */ };
 
 // all layers of a stack in one launch: blockIdx.y = layer
 __global__ void pack_weight_kernel(const PackArgs args) {
@@ -94,6 +94,12 @@ __global__ void pack_weight_kernel(const PackArgs args) {
             const int row = k + j;
             if (row >= ((Km + 127) / 128) * 128) continue;
             const float val = row < Km ? v[j] : 0.f;
+            if (args.bf16) {   // bf16 dgrad image (BF_TILE_BYTES per tile, SWIZZLE_64B): element (row, n) is 2 bytes in its chunk
+                uint8_t* dst = tiles_b + ((size_t)(row >> 7) * nkb_b + (n >> 5)) * BF_TILE_BYTES + sw64(row & 127, (n & 31) >> 3) +
+                               (n & 7) * 2;
+                *reinterpret_cast<uint16_t*>(dst) = (uint16_t)(pack_bf16x2(val, 0.f) & 0xFFFFu);
+                continue;
+            }
             uint8_t* dst = tiles_b + ((size_t)(row >> 7) * nkb_b + (n >> 5)) * (2 * TILE) + tile_sw128(row & 127, (n & 31) >> 2) +
                            (n & 3) * 4;
             *reinterpret_cast<float*>(dst) = tf32_hi(val);
@@ -131,7 +137,7 @@ __global__ void d2f_kernel(const double* __restrict__ src, const float* __restri
 // ---- workspace plan -------------------------------------------------------------------------------------------
 struct Plan {
     int n, P, S, rows;
-    bool bf16;           // precision 1: bf16 forward images and kernels
+    bool bf16;           // precision 1 / 2: bf16 weight images and kernels
     bool lift, virt;     // layer 0 lifted (o3d_lift_t); virt: Y0 is never stored (the tensor-core kernels gather it)
     size_t gidx;         // [P] int32: global Z row of every position (forward workspace)
     int Nw[O3D_MAX_LAYERS], K[O3D_MAX_LAYERS];
@@ -150,8 +156,9 @@ struct Plan {
 
 bool make_plan(const o3d_stack_t* d, Plan& p) {
     if (d->n_layers < 1 || d->n_layers > O3D_MAX_LAYERS || d->P < 0 || d->K0 < 4 || (d->K0 & 3)) return false;
-    if (d->precision != 0 && (d->precision != 1 || d->training)) return false;   // bf16 is for inference only
-    p.bf16 = d->precision == 1;
+    // precision 1 (BF16 inference) is for eval mode only, precision 2 (BF16 training) for training mode only
+    if (d->precision != 0 && !(d->precision == 1 && !d->training) && !(d->precision == 2 && d->training)) return false;
+    p.bf16 = d->precision != 0;
     p.n = d->n_layers; p.P = d->P; p.S = d->S;
     p.rows = d->S > 0 ? d->P / d->S : d->P;
     p.lift = d->lift != nullptr;
@@ -197,7 +204,8 @@ bool make_plan(const o3d_stack_t* d, Plan& p) {
         p.wt[l] = o; o += al(sizeof(float) * (size_t)p.Nw[l] * p.K[l]);
         p.bias[l] = o; o += al(sizeof(float) * p.Nw[l]);
         p.tiles[l] = o; if (p.tc_f[l]) o += al((size_t)o3d_pw_tc_wtile_bytes(p.Nw[l], p.K[l]) / (p.bf16 ? 4 : 1));
-        p.btiles[l] = o; if (p.tc_b[l]) o += al((size_t)o3d_pw_tc_wtile_bytes(tc_main(p.K[l]), p.Nw[l]));
+        // (the dgrad images are bf16 in BF16 training only: inference never writes them, and its blocks keep their size)
+        p.btiles[l] = o; if (p.tc_b[l]) o += al((size_t)o3d_pw_tc_wtile_bytes(tc_main(p.K[l]), p.Nw[l]) / (d->precision == 2 ? 4 : 1));
     }
     p.param_bytes = o;       // everything above depends on the parameters only (eval mode): o3d_stack_prepare() fills it once
     for (int l = 0; l < p.n; ++l) {
@@ -312,8 +320,10 @@ extern "C" int o3d_stack_prepare(const o3d_stack_t* d, void* block, void* stream
 extern "C" int o3d_stack_forward(const o3d_stack_t* d, const float* x, void* ws_fwd, float* out, int keep_for_backward,
                                  void* stream) {
     O3D_REQUIRE(d && (x || d->lift) && ws_fwd && out, O3D_ERR_ARG, "o3d_stack_forward: null pointer");
-    O3D_REQUIRE(d->precision == 0 || (d->precision == 1 && d->prepared && !d->training && !keep_for_backward), O3D_ERR_ARG,
-                "o3d_stack_forward: precision %d needs inference on a prepared block (no training, no keep_for_backward)", d->precision);
+    O3D_REQUIRE(d->precision == 0 || (d->precision == 1 && d->prepared && !d->training && !keep_for_backward) ||
+                    (d->precision == 2 && d->training),
+                O3D_ERR_ARG, "o3d_stack_forward: precision %d needs inference on a prepared block (precision 1: no training, no "
+                "keep_for_backward) or training (precision 2)", d->precision);
     Plan p;
     O3D_REQUIRE(make_plan(d, p), O3D_ERR_ARG, "o3d_stack_forward: bad stack description");
     O3D_REQUIRE(p.S == 0 || (128 % p.S == 0 && p.P % p.S == 0), O3D_ERR_ARG, "o3d_stack_forward: group size %d", p.S);
@@ -396,7 +406,8 @@ extern "C" int o3d_stack_forward(const o3d_stack_t* d, const float* x, void* ws_
 extern "C" int o3d_stack_backward(const o3d_stack_t* d, const float* x, const void* ws_fwd, void* ws_bwd, const float* out,
                                   const float* dout, float* dx, void* stream) {
     O3D_REQUIRE(d && (x || d->lift) && ws_fwd && ws_bwd && out && dout, O3D_ERR_ARG, "o3d_stack_backward: null pointer");
-    O3D_REQUIRE(d->precision == 0, O3D_ERR_ARG, "o3d_stack_backward: precision %d is for inference only", d->precision);
+    O3D_REQUIRE(d->precision == 0 || d->precision == 2, O3D_ERR_ARG, "o3d_stack_backward: precision %d is for inference only",
+                d->precision);
     Plan p;
     O3D_REQUIRE(make_plan(d, p), O3D_ERR_ARG, "o3d_stack_backward: bad stack description");
     if (p.P == 0) return O3D_OK;
@@ -476,10 +487,10 @@ extern "C" int o3d_stack_backward(const o3d_stack_t* d, const float* x, const vo
             float* gout = l > 0 ? at<float>(wb, p.gbuf[gsel]) : dx;
             const bool want = l > 0 && (d->has_bn[l - 1] || d->bias[l - 1] != nullptr);
             const bool lifted = l == 1 && p.virt;
-            rc = o3d_pw_bwd_tc(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, wf + p.btiles[l], lifted ? nullptr : xin,
-                               lifted ? d->lift : nullptr, lifted ? at<int32_t>(wf, p.gidx) : nullptr, psc, psh, prelu, p.P, Nl, K,
-                               gout, want ? s1(l - 1) : nullptr, want ? s1(l - 1) + K : nullptr, at<float>(wb, p.dwp[l]), K,
-                               at<float>(wb, p.wpart), p.wpart_floats, stream);
+            rc = o3d_pw_bwd_tc_prec(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, wf + p.btiles[l], lifted ? nullptr : xin,
+                                    lifted ? d->lift : nullptr, lifted ? at<int32_t>(wf, p.gidx) : nullptr, psc, psh, prelu, p.P, Nl,
+                                    K, gout, want ? s1(l - 1) : nullptr, want ? s1(l - 1) + K : nullptr, at<float>(wb, p.dwp[l]), K,
+                                    at<float>(wb, p.wpart), p.wpart_floats, stream, p.bf16);
             if (rc) return rc;
             g = gout;
             gsel ^= 1;
@@ -493,15 +504,15 @@ extern "C" int o3d_stack_backward(const o3d_stack_t* d, const float* x, const vo
             double* ps1 = want ? s1(l - 1) : nullptr;
             double* ps2 = want ? s1(l - 1) + K : nullptr;
             if (l == 1 && p.virt) {
-                rc = o3d_pw_dgrad_tc_lift(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, wf + p.btiles[l], p.P, Nl, K, gout, K, d->lift,
-                                          at<int32_t>(wf, p.gidx), psc, psh, prelu, ps1, ps2, stream);
+                rc = o3d_pw_dgrad_tc_lift_prec(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, wf + p.btiles[l], p.P, Nl, K, gout, K,
+                                               d->lift, at<int32_t>(wf, p.gidx), psc, psh, prelu, ps1, ps2, stream, p.bf16);
             } else if (p.tc_b[l]) {
                 // tensor cores on the first floor(K/128)*128 input channels, exact CUDA-core kernel on the ragged tail
                 // (the xyz / box-cloud extras of a first layer)
                 const int Km = tc_main(K);
                 const void* tiles = wf + p.btiles[l];   // written by the forward pass's pack kernel
-                rc = o3d_pw_dgrad_tc(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, tiles, p.P, Nl, Km, gout, K, yprev, K, psc, psh,
-                                     prelu, ps1, ps2, stream);
+                rc = o3d_pw_dgrad_tc_prec(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, tiles, p.P, Nl, Km, gout, K, yprev, K, psc, psh,
+                                          prelu, ps1, ps2, stream, p.bf16);
                 if (rc) return rc;
                 // the ragged tail of a first layer holds (dx,dy,dz,0): skipped when the caller needs no coordinate gradient
                 const bool tail_wanted = !(l == 0 && d->dx_cols > 0 && d->dx_cols <= Km);
@@ -520,14 +531,14 @@ extern "C" int o3d_stack_backward(const o3d_stack_t* d, const float* x, const vo
         if (d->d_weight[l]) {
             float* dwp = at<float>(wb, p.dwp[l]);
             if (l == 1 && p.virt) {
-                rc = o3d_pw_wgrad_tc_lift(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, d->lift, at<int32_t>(wf, p.gidx), psc, psh, prelu,
-                                          p.P, Nl, K, dwp, K, at<float>(wb, p.wpart), p.wpart_floats, stream);
+                rc = o3d_pw_wgrad_tc_lift_prec(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, d->lift, at<int32_t>(wf, p.gidx), psc, psh,
+                                               prelu, p.P, Nl, K, dwp, K, at<float>(wb, p.wpart), p.wpart_floats, stream, p.bf16);
             } else if (p.tc_w[l]) {
                 // tensor-core part: the first floor(K/128)*128 input channels; ragged tail (xyz / box-cloud extras)
                 // goes through the exact CUDA-core kernel on the remaining columns
                 const int Kmain = tc_main(K);
-                rc = o3d_pw_wgrad_tc2(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, xin, K, psc, psh, prelu, p.P, Nl, Kmain, dwp, K,
-                                      at<float>(wb, p.wpart), p.wpart_floats, stream);
+                rc = o3d_pw_wgrad_tc2_prec(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, xin, K, psc, psh, prelu, p.P, Nl, Kmain, dwp,
+                                           K, at<float>(wb, p.wpart), p.wpart_floats, stream, p.bf16);
                 if (rc) return rc;
                 if (K > Kmain)
                     rc = o3d_pw_wgrad(gl, Nl, yl, Nl, a, b, cc, dpl, sel, Sg, Nl, xin + Kmain, K, psc ? psc + Kmain : nullptr,

@@ -191,15 +191,76 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
 }
 __device__ __forceinline__ uint2 pack_bf16x4(const float4& v) { return make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w)); }
 
+__device__ __forceinline__ void wgmma_bf16_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
 // BF16 product of one 32-wide k-block: D += A.B over 2 k16 steps (descriptors of the k-block's first column)
 template <int N>
 __device__ __forceinline__ void wgmma_bf16_kblock(float (&d)[N / 2], uint64_t a, uint64_t b, bool first) {
 #pragma unroll
     for (int ks = 0; ks < 2; ++ks) {
         const uint64_t adv = (uint64_t)((ks * 32) >> 4);
-        if constexpr (N == 64) wgmma_bf16_n64(d, a + adv, b + adv, (first && ks == 0) ? 0u : 1u);
+        if constexpr (N == 32) wgmma_bf16_n32(d, a + adv, b + adv, (first && ks == 0) ? 0u : 1u);
+        else if constexpr (N == 64) wgmma_bf16_n64(d, a + adv, b + adv, (first && ks == 0) ? 0u : 1u);
         else wgmma_bf16_n128(d, a + adv, b + adv, (first && ks == 0) ? 0u : 1u);
     }
+}
+
+// ---- BF16 with both operands MN-major (the weight-gradient GEMMs of BF16 training) ------------------------------------------
+// The training operands dY and X are position-major in global memory, and position is the weight gradient's K.  For 16-bit
+// types wgmma reads MN-major shared-memory operands through its transpose bits (imm-trans-a = imm-trans-b = 1), so the
+// producers store the rows as they come, in the same 64-byte-swizzle image as the K-major path: row = position, 64 bytes =
+// 32 channels, 16-byte chunk c of row r at r * 64 + ((c ^ ((r >> 1) & 3)) << 4).  Read MN-major, that image is the PTX ISA's
+// canonical SWIZZLE_64B MN-major layout  ((T,4,m),(8,k)) : ((1,T,LBO),(4T,SBO))  with T = 8 bf16: a 512-byte atom holds 32
+// channels x 8 positions, LBO is the byte distance between the atoms of consecutive 32-channel groups and SBO the distance
+// between consecutive 8-position groups (512 here).  A k16 step is two 8-position groups: +1024 bytes.
+__device__ __forceinline__ uint64_t make_desc_sw64_mn(uint32_t smem_addr, uint32_t lbo) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+    d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+    d |= (uint64_t)(512 >> 4) << 32;
+    d |= (uint64_t)2 << 62;
+    return d;
+}
+
+// D += A[64 x k16, MN-major] . B[N x k16, MN-major]^T, bf16 inputs, fp32 accumulation (accumulate = 0: D is overwritten)
+__device__ __forceinline__ void wgmma_bf16_tt_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+__device__ __forceinline__ void wgmma_bf16_tt_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+// bf16 operand row store into an MN-major / K-major 64-byte-swizzle image made of 32-channel sub-images `sub` bytes apart:
+// channels c .. c + 3 (c % 4 == 0) of local row r
+__device__ __forceinline__ void st_bf16_row4(uint8_t* img, int sub, int r, int c, const float4& v) {
+    *reinterpret_cast<uint2*>(img + (c >> 5) * sub + sw64(r, (c & 31) >> 3) + (c & 4) * 2) = pack_bf16x4(v);
 }
 
 }  // namespace

@@ -119,9 +119,12 @@ class FlatAdam:
 
 
 class TrainStep:
-    """`step(batch) -> loss` for a model exposing `training_step(batch, idx)`; `batch` is a dict of device tensors."""
+    """`step(batch) -> loss` for a model exposing `training_step(batch, idx)`; `batch` is a dict of device tensors.
+    `precision`: "fp32" (3xTF32 GEMMs, default) or "bf16" (BF16 operands with FP32 accumulation in the tensor-core GEMMs of the
+    MLP stacks, runtime.training_precision_scope); the eager steps and the captured one both run in it."""
 
-    def __init__(self, model, lr=1e-3, weight_decay=0.0, use_graph=True, warmup=3, capture_collective=True):
+    def __init__(self, model, lr=1e-3, weight_decay=0.0, use_graph=True, warmup=3, capture_collective=True, precision="fp32"):
+        self.precision = runtime.check_precision(precision)
         self.model = model
         self.capture_collective = capture_collective
         self.flat = ddp.FlatParams(model)
@@ -199,6 +202,10 @@ class TrainStep:
                 self.static_loss = self._fwd_bwd(self.static_batch)
 
     def step(self, batch):
+        with runtime.training_precision_scope(self.precision):
+            return self._step(batch)
+
+    def _step(self, batch):
         self.calls += 1
         if not self.use_graph or self.calls <= self.warmup:
             return self._eager(batch)

@@ -158,8 +158,11 @@ def _derived(weight, tag, make):
 
 
 def _precision_code(training, need_grad):
-    """o3d_stack_t.precision of a forward under the current runtime.inference_precision(); bf16 refuses autograd and training"""
+    """o3d_stack_t.precision of a forward under the current runtime.inference_precision() and, for a stack in training mode,
+    runtime.training_precision(); bf16 inference refuses autograd and training"""
     if runtime.inference_precision() == "fp32":
+        if training and runtime.training_precision() == "bf16":
+            return _lib.PRECISION_BF16_TRAIN
         return _lib.PRECISION_TF32X3
     if need_grad or training:
         raise RuntimeError("bf16 inference precision: forward passes that need a gradient, and modules in training mode, run in "

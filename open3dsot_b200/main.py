@@ -26,6 +26,9 @@ def parse_args(argv=None):
     p.add_argument('--precision', choices=('fp32', 'bf16'), default='fp32',
                    help='--test: operand precision of the tensor-core layers (bf16: BF16 operands, FP32 accumulation); '
                         'training is fp32 only')
+    p.add_argument('--train_precision', choices=('fp32', 'bf16'), default='fp32',
+                   help='training: operand precision of the tensor-core GEMMs of the training steps (bf16: BF16 operands, FP32 '
+                        'accumulation, fp32 weights and optimizer state); validation runs in fp32; --test ignores it')
     return p.parse_args(argv)
 
 

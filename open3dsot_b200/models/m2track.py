@@ -57,7 +57,9 @@ class M2TRACK(base_model.MotionBaseModel):
 
         seg_out = self.seg_pointnet(x)
         seg_logits = seg_out[:, :2, :]
-        pred_cls = torch.argmax(seg_logits, dim=1, keepdim=True)                      # (B,1,N)
+        # the point mask and the motion state are arg-max decisions on computed logits: routed through runtime.choose so that a
+        # parity test can hold them fixed (a no-op otherwise)
+        pred_cls = runtime.choose("m2_segment", {"N": N}, lambda: torch.argmax(seg_logits, dim=1, keepdim=True))   # (B,1,N)
         mask_points = x[:, :4, :] * pred_cls
         mask_xyz_t0 = mask_points[:, :3, :N // 2]
         mask_xyz_t1 = mask_points[:, :3, N // 2:]
@@ -72,7 +74,7 @@ class M2TRACK(base_model.MotionBaseModel):
         motion_pred = self._mlp(self.motion_mlp, point_feature)                       # (B,4)
         if self.use_motion_cls:
             motion_state_logits = self._mlp(self.motion_state_mlp, point_feature)     # (B,2)
-            motion_mask = torch.argmax(motion_state_logits, dim=1, keepdim=True)
+            motion_mask = runtime.choose("m2_motion_state", {}, lambda: torch.argmax(motion_state_logits, dim=1, keepdim=True))
             motion_pred_masked = motion_pred * motion_mask
             output_dict['motion_cls'] = motion_state_logits
         else:

@@ -128,6 +128,33 @@ def inference_precision_scope(precision):
         _PRECISION = old
 
 
+# Operand precision of the tensor-core GEMMs of stacks in training mode (o3d_stack_t.precision 2): "fp32" = 3xTF32 (default),
+# "bf16" = BF16 operands with FP32 accumulation in the forward, data-gradient and weight-gradient GEMMs.  Only
+# training_precision_scope() changes it; engine.TrainStep(precision=...) opens it around its steps.
+_TRAIN_PRECISION = "fp32"
+
+
+def training_precision() -> str:
+    return _TRAIN_PRECISION
+
+
+@contextlib.contextmanager
+def training_precision_scope(precision):
+    """`with runtime.training_precision_scope("bf16"):` — MLP stacks in training mode run their tensor-core forward, dgrad and
+    wgrad GEMMs on BF16 operands with FP32 accumulation (include/o3d_b200.h, o3d_stack_t.precision = 2).  Parameters, gradients,
+    optimizer state, BatchNorm statistics, the stored layer outputs and every layer on the CUDA-core kernels stay fp32.
+    Eval-mode stacks, with or without autograd, ignore the scope, so a validation inside it runs as it would outside.  "fp32"
+    leaves every result as it is outside the scope."""
+    global _TRAIN_PRECISION
+    check_precision(precision)
+    old = _TRAIN_PRECISION
+    _TRAIN_PRECISION = precision
+    try:
+        yield
+    finally:
+        _TRAIN_PRECISION = old
+
+
 # In-place accumulation of parameter gradients: a stack's backward ADDS its weight / bias / BatchNorm gradients straight into the
 # parameters' existing `.grad` buffers (and returns no gradient for them) instead of materialising them and letting autograd's
 # AccumulateGrad issue one elementwise add per parameter — ~130 launches per BAT step.  Only valid for `loss.backward()` onto
@@ -181,10 +208,11 @@ def composed_mode():
 
 
 # ---- discrete-choice hook (parity tests only) -------------------------------------------------------------------
-# The forward pass takes three kinds of data-dependent DISCRETE decisions on computed values: the ball query of every
-# set-abstraction layer (on input coordinates in the backbone, on VOTED coordinates in the RPN), and BoxAwareXCorr's top-k
-# over predicted box clouds.  A neighbour that sits within fp32 round-off of the radius / of the k-th distance can fall the
-# other way on the GPU than in the CPU oracle, which changes downstream floats by O(1e-3) without any kernel being wrong.
+# The forward pass takes data-dependent DISCRETE decisions on computed values: the ball query of every set-abstraction layer
+# (on input coordinates in the backbone, on VOTED coordinates in the RPN), BoxAwareXCorr's top-k over predicted box clouds, and
+# M2-Track's arg-max point mask and motion state ("m2_segment", "m2_motion_state").  A neighbour that sits within fp32
+# round-off of the radius / of the k-th distance can fall the other way on the GPU than in the CPU oracle, which changes
+# downstream floats by O(1e-3) without any kernel being wrong.
 # Parity tests install a hook that (a) records the product's own choice and (b) may substitute the oracle's, so that the
 # float path is compared at 1e-4 with identical discrete choices.  hook(kind, info, compute) -> int32 tensor; `compute()`
 # evaluates the product's choice.  None (the default) = no hook: the product path is unchanged.

@@ -33,6 +33,8 @@ def check_supported(cfg):
         raise ValueError("random_sample: True is not supported; epochs pass over every frame (random_sample: False)")
     if str(cfg.get("precision", "fp32")) != "fp32":
         raise ValueError(f"precision: {cfg.precision!r} is for inference only (--test); training and its validation run in fp32")
+    if cfg.get("train_precision", "fp32") not in ("fp32", "bf16"):
+        raise ValueError(f"train_precision: {cfg.train_precision!r} is not supported; only 'fp32' and 'bf16' are")
 
 
 def epoch_indices(n, epoch, seed=0, rank=0, world=1):
@@ -157,7 +159,9 @@ class Trainer:
             cls = DeviceMotionSampler if str(cfg.get("train_type", "")).lower() == "train_motion" else DeviceSiameseSampler
             self.sampler = cls(train_tracklets, cfg, next(model.parameters()).device, seed=self.seed + self.rank)
         self.model.train()
-        self.step = TrainStep(model, lr=self.base_lr, weight_decay=cfg.wd)
+        # the training steps' GEMM precision; validation and test() run in fp32 whatever it is (eval-mode stacks ignore it)
+        self.train_precision = str(cfg.get("train_precision", "fp32"))
+        self.step = TrainStep(model, lr=self.base_lr, weight_decay=cfg.wd, precision=self.train_precision)
         self.step.opt.set_lr(self.lr)
         self._keys = None
 
@@ -222,7 +226,7 @@ class Trainer:
             losses, train_s, steps = self.train_epoch()
             row = {"epoch": epoch, "global_step": self.global_step, "lr": lr, **losses, "success": None, "precision": None,
                    "train_seconds": train_s, "pairs_per_second": steps * self.batch_size * self.world / train_s,
-                   "val_seconds": None}
+                   "val_seconds": None, "train_precision": self.train_precision}
             if (epoch + 1) % self.val_every == 0 and self.val_tracklets:
                 t0 = time.perf_counter()
                 res = self.test(self.val_tracklets)
