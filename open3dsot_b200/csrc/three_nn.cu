@@ -216,6 +216,10 @@ extern "C" int o3d_three_nn_interpolate(const float* unknown, const float* known
                                         void* stream) {
     O3D_REQUIRE(unknown && known && known_feat_cl && out_cl && idx && weight, O3D_ERR_ARG,
                 "o3d_three_nn_interpolate: null pointer");
+    // every unknown point reads the feature rows of its three neighbours (row 0 stands in for a missing one): an empty known
+    // cloud has no row to read
+    O3D_REQUIRE(B >= 0 && n >= 0 && m >= 1, O3D_ERR_ARG, "o3d_three_nn_interpolate: bad sizes B=%d n=%d m=%d (m >= 1)", B, n,
+                m);
     O3D_REQUIRE((c & 3) == 0, O3D_ERR_ARG, "o3d_three_nn_interpolate: c must be a multiple of 4");
     O3D_REQUIRE(((uintptr_t)known_feat_cl & 15) == 0 && ((uintptr_t)out_cl & 15) == 0, O3D_ERR_ALIGN,
                 "o3d_three_nn_interpolate: feature pointers must be 16-byte aligned");
