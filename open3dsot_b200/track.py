@@ -10,12 +10,48 @@ LIDAR_TOP scans in timestamp order (nuScenes).  Every tracklet of `category_name
 frame from its ground-truth box and is dropped after its last annotated frame; nothing else of the ground truth is used.  One
 JSON line per (scene, frame) lists every active target's box; Success / Precision over the annotated frames are printed, with
 the host metric path of `tracking.evaluate` (the first frame of a tracklet scored against its own ground truth).  A target's
-draws are keyed by its tracklet's index in the split, as `evaluate_batched` keys them by default."""
+draws are keyed by its tracklet's index in the split, as `evaluate_batched` keys them by default.
+
+Several classes: `--add_class CFG [CKPT]` (repeatable) adds a class with its own model and weights, tracking its config's
+`category_name`; every config shares the dataset and the reader's frame settings (`check_classes`).  Each class's reader lists
+its tracklets, the scene plans are merged so that every scene streams once for all classes, and one `MultiClassTracker`
+(tracking/multi_class.py) advances every class in one captured step per scan.  `--max_targets` is per class (`K`, or `NAME=K`
+for one class).  Every JSON line's targets carry their "class"; Success / Precision are printed over all frames and per class,
+and a class's boxes are those of a run with its config alone at the same --max_points and --max_targets."""
 import argparse
 import json
 import sys
 
 import numpy as np
+
+
+class _MaxTargets(argparse.Action):
+    """--max_targets K (an int, every class) or NAME=K (repeatable): then a dict {NAME: K, None: the K of the other classes}."""
+
+    def __call__(self, parser, namespace, value, option_string=None):
+        name, eq, k = value.rpartition("=")
+        try:
+            k = int(k)
+        except ValueError:
+            parser.error(f"--max_targets {value}: expected K or NAME=K")
+        cur = getattr(namespace, self.dest)
+        if not eq:
+            if isinstance(cur, dict):
+                cur[None] = k
+            else:
+                setattr(namespace, self.dest, k)
+        elif not name:
+            parser.error(f"--max_targets {value}: expected K or NAME=K")
+        else:
+            if not isinstance(cur, dict):
+                cur = {None: cur}
+            cur[name] = k
+            setattr(namespace, self.dest, cur)
+
+
+def class_targets(max_targets, name):
+    """A class's slots from --max_targets: the int, or the class's NAME=K entry (else the plain K, 64 by default)."""
+    return max_targets.get(name, max_targets[None]) if isinstance(max_targets, dict) else max_targets
 
 
 def parse_args(argv=None):
@@ -25,12 +61,45 @@ def parse_args(argv=None):
     p.add_argument('--path', type=str, required=True, help='dataset root (for KITTI: velodyne/, label_02/, calib/)')
     p.add_argument('--split', type=str, default='test', help='scene split (train / valid / test / *_tiny)')
     p.add_argument('--out', type=str, default='results.jsonl', help='per-frame results, one JSON line per (scene, frame)')
-    p.add_argument('--max_targets', type=int, default=64, help='tracker slots (targets in flight at once)')
+    p.add_argument('--add_class', action='append', nargs='+', metavar=('CFG', 'CKPT'), default=None,
+                   help='track a further class: its config and, optionally, its weights (repeatable); the configs share the '
+                        'dataset and its frame settings')
+    p.add_argument('--max_targets', action=_MaxTargets, default=64,
+                   help='tracker slots per class (targets in flight at once): K for every class, or NAME=K for the class whose '
+                        'category_name is NAME (repeatable)')
     p.add_argument('--max_points', type=int, default=None, help='scan buffer size (default: the largest scan streamed)')
     p.add_argument('--seed', type=int, default=0, help='key of the random draws')
     p.add_argument('--precision', choices=('fp32', 'bf16'), default='fp32',
                    help='operand precision of the tensor-core layers (bf16: BF16 operands, FP32 accumulation)')
-    return p.parse_args(argv)
+    args = p.parse_args(argv)
+    for extra in args.add_class or ():
+        if len(extra) > 2:
+            p.error(f"--add_class takes a config and at most one checkpoint, got {extra}")
+    return args
+
+
+# reader settings that decide which scans a scene's frames are and in which frame their points are: the classes of one run share
+# them, and with them every scan
+FRAME_KEYS = {"kitti": (("coordinate_mode", "velodyne"),), "nuscenes": (("version", "v1.0-trainval"), ("key_frame_only", False)),
+              "waymo": (("tiny", False),)}
+
+
+def check_classes(cfgs, names):
+    """Refuse (SystemExit) classes that cannot share one run: another dataset or other frame settings than the first config, or
+    a category_name that another class already has.  `names`: the config files, for the messages."""
+    first, dataset = cfgs[0], cfgs[0].get("dataset", "kitti")
+    seen = {}
+    for cfg, name in zip(cfgs, names):
+        if cfg.get("dataset", "kitti") != dataset:
+            raise SystemExit(f"{name}: dataset '{cfg.get('dataset', 'kitti')}' differs from {names[0]}'s '{dataset}'; the classes "
+                             f"of one run track the same scans")
+        for key, default in FRAME_KEYS.get(dataset, ()):
+            if cfg.get(key, default) != first.get(key, default):
+                raise SystemExit(f"{name}: {key}={cfg.get(key, default)} differs from {names[0]}'s {key}={first.get(key, default)}; "
+                                 f"the classes of one run read the scans in the same frame")
+        if cfg.category_name in seen:
+            raise SystemExit(f"{name}: category_name '{cfg.category_name}' is already tracked by {seen[cfg.category_name]}")
+        seen[cfg.category_name] = name
 
 
 def scene_plan(dataset):
@@ -53,6 +122,54 @@ def scene_plan(dataset):
             out.append({"scene": scene, "first": first, "last": last, "tracklets": tr,
                         "frames": [f for f in dataset.scene_frames(scene) if first <= f <= last]})
     return out
+
+
+def class_scene_plan(datasets):
+    """`scene_plan` over several classes' readers of one split, {class: reader}, merged by scene: a scene streams once, from the
+    earliest start to the latest end over every class's tracklets, which carry their "class" (`index` stays the tracklet's index in
+    its own reader).  A reader may know only the scenes and frames of its own class (Waymo indexes the scans its tracklets refer
+    to; KITTI extends a scene to its own class's last labelled frame), so a merged scene's frames are those of every reader that
+    plans the scene, and "reader_of" names, per frame, the class whose reader reads that scan: the first, in class order, that
+    lists it.  Scenes in the first reader's order, then any other reader's."""
+    merged = {}
+    for cls, ds in datasets.items():
+        for p in scene_plan(ds):
+            m = merged.setdefault(p["scene"], {"scene": p["scene"], "first": p["first"], "last": p["last"], "tracklets": [],
+                                               "reader_of": {}})
+            m["first"], m["last"] = min(m["first"], p["first"]), max(m["last"], p["last"])
+            m["tracklets"] += [dict(tr, **{"class": cls}) for tr in p["tracklets"]]
+            for f in ds.scene_frames(p["scene"]):
+                m["reader_of"].setdefault(f, cls)
+    order = list(dict.fromkeys(s for ds in datasets.values() for s in ds.scene_list))
+    out = []
+    for scene in order:
+        if scene in merged:
+            m = merged[scene]
+            m["reader_of"] = {f: c for f, c in sorted(m["reader_of"].items()) if m["first"] <= f <= m["last"]}
+            m["frames"] = list(m["reader_of"])
+            out.append(m)
+    return out
+
+
+def class_stream_max_points(datasets, plan):
+    """`stream_max_points` of a merged plan: every frame's scan sized by the reader that reads it."""
+    return max([1] + [datasets[p["reader_of"][f]].scan_size(p["scene"], f) for p in plan for f in p["frames"]])
+
+
+def class_scenes(datasets, plan):
+    """The `track_classes` scenes of a merged plan: targets named (class, tracklet index in its class's reader), starting from
+    their first ground-truth box, every scan read as stored (`raw_scan`) by the reader `plan` assigns to its frame."""
+    scenes = []
+    for p in plan:
+        pos = {f: t for t, f in enumerate(p["frames"])}
+        starts, ends = {}, {}
+        for tr in p["tracklets"]:
+            c, j = tr["class"], tr["index"]
+            starts.setdefault(pos[tr["start"]], []).append(((c, j), datasets[c].box_from_anno(datasets[c].tracklet_anno_list[j][0])))
+            ends[(c, j)] = pos[tr["end"]]
+        scenes.append({"frames": len(p["frames"]), "starts": starts, "ends": ends,
+                       "scan": lambda t, p=p: datasets[p["reader_of"][p["frames"][t]]].raw_scan(p["scene"], p["frames"][t])})
+    return scenes
 
 
 def stream_max_points(dataset, plan):
@@ -112,6 +229,58 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, preci
     return {"success": succ.compute(), "precision": prec.compute(), "frames": sum(len(o) for o in overlaps), "scenes": len(plan)}
 
 
+def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0, precision="fp32"):
+    """`run` for several classes in one pass over the scans: `models`, `datasets` and `max_targets` are {class: ...} (the class
+    is its config's category_name).  Every scene streams once for all classes (class_scene_plan) through one MultiClassTracker;
+    a target's draws are keyed by its tracklet's index in its class's reader, as in a one-class run.  Every JSON line's targets
+    carry their "class".  Returns {"success", "precision", "frames", "scenes"} over every class's frames, and the same per class
+    under "classes"."""
+    from .tracking.multi_class import track_classes
+    from .utils.metrics import Precision, Success, estimateAccuracy, estimateOverlap
+
+    names = list(models)
+    cfg = models[names[0]].config
+    dim, up = cfg.IoU_space, cfg.up_axis
+    plan = class_scene_plan(datasets)
+    if max_points is None:
+        max_points = class_stream_max_points(datasets, plan)
+    annos = {c: datasets[c].tracklet_anno_list for c in names}
+    scenes = class_scenes(datasets, plan)
+    results = track_classes(models, scenes, max(1, min(len(scenes), sum(max_targets.values()))), max_targets, seed=seed,
+                            max_points=max_points, precision=precision)
+    overlaps = {c: [[] for _ in annos[c]] for c in names}
+    distances = {c: [[] for _ in annos[c]] for c in names}
+    rank = {c: i for i, c in enumerate(names)}
+    with open(out_path, "w") as f:
+        for p, res in zip(plan, results):
+            scene, pos = p["scene"], {fr: t for t, fr in enumerate(p["frames"])}
+            track_id = {(tr["class"], tr["index"]): tr["track_id"] for tr in p["tracklets"]}
+            for t, frame in enumerate(p["frames"]):
+                targets = [{"class": c, "id": track_id[(c, j)], "tracklet": j, "center": b[t].center.tolist(),
+                            "wlh": b[t].wlh.tolist(), "yaw": _yaw(b[t].rotation_matrix, up)}
+                           for (c, j), b in sorted(res.items(), key=lambda kv: (rank[kv[0][0]], kv[0][1])) if t in b]
+                f.write(json.dumps({"scene": scene, "frame": frame, "targets": targets}) + "\n")
+            for tr in p["tracklets"]:
+                c, j = tr["class"], tr["index"]
+                for i, anno in enumerate(annos[c][j]):
+                    gt = datasets[c].box_from_anno(anno)
+                    box = gt if i == 0 else res[(c, j)][pos[datasets[c].anno_frame(anno)[1]]]
+                    overlaps[c][j].append(estimateOverlap(gt, box, dim=dim, up_axis=up))
+                    distances[c][j].append(estimateAccuracy(gt, box, dim=dim, up_axis=up))
+
+    def scores(classes):
+        succ, prec = Success(), Precision()
+        for c in classes:
+            for o, d in zip(overlaps[c], distances[c]):
+                succ(o)
+                prec(d)
+        return {"success": succ.compute(), "precision": prec.compute(), "frames": sum(len(o) for c in classes for o in overlaps[c])}
+
+    out = scores(names)
+    out.update({"scenes": len(plan), "classes": {c: scores([c]) for c in names}})
+    return out
+
+
 def reader(cfg, path, split):
     """The config's dataset reader over a split, for whole-scan tracking (no preloading, no crop)."""
     dataset = cfg.get("dataset", "kitti")
@@ -140,15 +309,29 @@ def main(argv=None):
     from .trainer import load_weights
 
     args = parse_args(argv)
-    cfg = load_config(args.cfg)
-    data = reader(cfg, args.path, args.split)
-    torch.manual_seed(0)
-    model = get_model(cfg.net_model)(cfg).cuda()
-    if args.checkpoint is not None:
-        load_weights(model, load_lightning_checkpoint(args.checkpoint)["state_dict"])
-    out = run(model, data, args.out, max_targets=args.max_targets, max_points=args.max_points, seed=args.seed,
-              precision=args.precision)
-    out.update({"checkpoint": args.checkpoint, "split": args.split, "out": args.out})
+    classes = [(args.cfg, args.checkpoint)] + [(a[0], a[1] if len(a) > 1 else None) for a in args.add_class or ()]
+    cfgs = [load_config(c) for c, _ in classes]
+    check_classes(cfgs, [c for c, _ in classes])
+    models, data = {}, {}
+    for cfg, (_, ckpt) in zip(cfgs, classes):
+        data[cfg.category_name] = reader(cfg, args.path, args.split)
+        torch.manual_seed(0)
+        model = models[cfg.category_name] = get_model(cfg.net_model)(cfg).cuda()
+        if ckpt is not None:
+            load_weights(model, load_lightning_checkpoint(ckpt)["state_dict"])
+    if isinstance(args.max_targets, dict):
+        unknown = set(args.max_targets) - set(models) - {None}
+        if unknown:
+            raise SystemExit(f"--max_targets: no class named {sorted(unknown)}; the classes are {list(models)}")
+    if len(cfgs) == 1:
+        name = cfgs[0].category_name
+        out = run(models[name], data[name], args.out, max_targets=class_targets(args.max_targets, name), max_points=args.max_points,
+                  seed=args.seed, precision=args.precision)
+        out.update({"checkpoint": args.checkpoint, "split": args.split, "out": args.out})
+    else:
+        out = run_classes(models, data, args.out, {c: class_targets(args.max_targets, c) for c in models},
+                          max_points=args.max_points, seed=args.seed, precision=args.precision)
+        out.update({"checkpoint": [c for _, c in classes], "split": args.split, "out": args.out})
     print(json.dumps(out), flush=True)
     return out
 

@@ -27,6 +27,8 @@ neither on its feed, nor on the other feeds, nor on F.  `step(points)` is `put(0
 Device memory: feeds * 2 * max_points * 12 bytes of scans, plus per slot the crop scratch and, for the first-frame template
 modes, max_points * 13 bytes of first-frame crop.  Ground-truth reference boxes (reference_BB 'previous_gt' / 'current_gt') have no meaning on a live stream, and
 shape_aggregation 'all' is not supported here; both are refused."""
+import weakref
+
 import numpy as np
 import torch
 
@@ -49,11 +51,145 @@ def _box_values(box):
     return np.asarray(box.center, np.float64), np.asarray(box.wlh, np.float64), np.asarray(box.rotation_matrix, np.float64)
 
 
+class ScanFeeds:
+    """The scan feeds of one or more live trackers: `feeds` ping-pong buffers (F, 2, max_points, 3) with their point counts, the
+    per-feed parity (host mirrors and the device copy the captured steps read) and the scans staged for the next advance.
+    `put` / `put_raw` stage a feed's next scan; `ingest()` brings every staged scan in with one packed host->device copy and one
+    `o3d_scan_ingest` launch and flips the parity of the feeds that got one.  Trackers built over the same store
+    (`MultiTargetTracker(..., feeds=store)`) read the same scans: one copy and one ingest serve them all.  Since an ingest moves
+    every feed's parity for all of them, only the store's `owner` advances: the first tracker built over it, or the
+    MultiClassTracker that holds the trackers sharing it."""
+
+    def __init__(self, max_points, feeds=1, device="cuda"):
+        self.N = N = int(max_points)
+        self.F = F = int(feeds)
+        dev = torch.device(device)
+        if dev.type == "cuda" and dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        self.dev = dev
+        if N < 1 or F < 1:
+            raise ValueError(f"max_points={N} and feeds={F} must be >= 1")
+        i64 = dict(device=dev, dtype=torch.int64)
+        self.scans = torch.zeros(F, 2, N, 3, device=dev, dtype=torch.float32)
+        self.count = torch.zeros(F, 2, **i64)
+        # per feed: fed by this advance (0 / 1), the half holding its most recent scan, the half holding the scan before it;
+        # written from the host mirrors below before every step
+        self.fstate = torch.tensor([[0] * F, [1] * F, [0] * F], **i64)
+        self.fcur, self.fprev = [1] * F, [0] * F
+        self.feed_seen = [0] * F                          # scans advanced per feed
+        self.scans_seen = 0                               # scans advanced over all feeds
+        self.staged = {}                                  # feed -> None (already in its buffer) or (rows, transforms)
+        self._owner = None                                # weak reference to the one tracker whose advance() ingests
+
+    @property
+    def owner(self):
+        return None if self._owner is None else self._owner()
+
+    @owner.setter
+    def owner(self, tracker):
+        self._owner = None if tracker is None else weakref.ref(tracker)
+
+    def claim(self, tracker):
+        """Make `tracker` the store's owner, the one whose advance() ingests; a store has one owner."""
+        if self.owner is not None and self.owner is not tracker:
+            raise ValueError("these scan feeds already belong to another tracker, which advances them; build the trackers that "
+                             "share them through a MultiClassTracker")
+        self.owner = tracker
+
+    def feed(self, feed):
+        f = int(feed)
+        if not 0 <= f < self.F:
+            raise ValueError(f"feed {f} out of range: the tracker has feeds 0 .. {self.F - 1}")
+        return f
+
+    def _stage(self, feed, n):
+        f = self.feed(feed)
+        if f in self.staged:
+            raise ValueError(f"feed {f} already has a scan staged: advance() before the next put")
+        if n > self.N:
+            raise ValueError(f"max_points: the scan has {n} points, the tracker was built for {self.N}")
+        return f
+
+    def put(self, feed, points, n_valid=None):
+        """Stage the next scan of `feed`: `points` (n, 3), the first `n_valid` valid.  A CUDA tensor is copied into the feed's next
+        buffer at once; a host tensor or array goes through the packed copy and the ingest kernel of the next `ingest()`.  No
+        host sync."""
+        n = points.shape[0]
+        f = self._stage(feed, n)
+        n_valid = n if n_valid is None else min(int(n_valid), n)
+        if isinstance(points, torch.Tensor) and (points.device == self.dev or self.dev.type != "cuda"):
+            nxt = 1 - self.fcur[f]
+            self.scans[f, nxt, :n].copy_(points, non_blocking=True)
+            self.count[f, nxt].fill_(n_valid)
+            self.staged[f] = None
+        else:
+            rows = points.numpy() if isinstance(points, torch.Tensor) else np.asarray(points)
+            self.staged[f] = (rows[:n_valid], ())
+
+    def put_raw(self, feed, rows, transforms=()):
+        """Stage the next scan of `feed` as a reader stores it: `rows` (n, stride) float32 / float64 (x, y, z first, 3 <= stride
+        <= 16) and up to two affine transforms (3x4 or 4x4, applied in order in float64, as the readers apply them on the host).
+        The next `ingest()` moves every staged raw scan to the device in one copy and one `o3d_scan_ingest` launch."""
+        rows = np.asarray(rows)
+        if self.dev.type != "cuda":
+            raise RuntimeError("put_raw: scan ingest runs on the GPU; this tracker is not on a CUDA device")
+        if rows.ndim != 2 or not 3 <= rows.shape[1] <= 16:
+            raise ValueError(f"put_raw: rows of shape {rows.shape}; expected (points, 3 .. 16 values per row)")
+        transforms = [np.asarray(m, np.float64) for m in transforms]
+        if len(transforms) > 2 or any(m.shape not in ((3, 4), (4, 4)) for m in transforms):
+            raise ValueError("put_raw: at most two transforms, each 3x4 or 4x4")
+        f = self._stage(feed, rows.shape[0])
+        self.staged[f] = (rows, transforms)
+
+    def ingest(self):
+        """Bring in every staged scan, on the current stream: the feeds that got one flip their parity and are marked fed in
+        `fstate`, the others hold.  No host sync."""
+        F, staged = self.F, self.staged
+        raw = [(f, 1 - self.fcur[f], v[0], v[1]) for f, v in sorted(staged.items()) if v is not None]
+        for f in staged:
+            self.fprev[f], self.fcur[f] = self.fcur[f], 1 - self.fcur[f]
+            self.feed_seen[f] += 1
+        state = np.array([[int(f in staged) for f in range(F)], self.fcur, self.fprev], dtype=np.int64)
+        if self.dev.type == "cuda":
+            # one host->device copy per step: the feeds' state, the ingest descriptors and every raw scan's rows
+            buf, desc, d0, s0 = ops.pack_scans(raw, head=state.nbytes)
+            buf.numpy()[:state.nbytes] = state.reshape(-1).view(np.uint8)
+            dev = buf.to(self.dev, non_blocking=True)
+            self.fstate.copy_(dev[:state.nbytes].view(torch.int64).view(3, F))
+            if raw:
+                ops.scan_ingest(self.scans, self.count, desc, dev, d0, s0)
+        else:
+            self.fstate.copy_(torch.from_numpy(state))
+        self.scans_seen += len(staged)
+        staged.clear()
+
+
+def capture_step(step, state):
+    """Capture `step()` in a CUDA graph.  The warm-up runs a real step (allocations, weight packing) on a side stream; `state`,
+    the tensors a step advances, is put back after it and after the capture, so the graph's first replay is the first step."""
+    snap = [t.clone() for t in state]
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        step()
+    torch.cuda.current_stream().wait_stream(s)
+    for t, v in zip(state, snap):
+        t.copy_(v)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        step()
+    for t, v in zip(state, snap):
+        t.copy_(v)
+    return graph
+
+
 class MultiTargetTracker:
     """`max_targets` slots over `feeds` scan feeds of at most `max_points` points per scan.  `seed` keys the random draws;
     `use_graph`: capture the step in a CUDA graph on the first advance (eager otherwise).  With one feed, call `step(scan)` for
     every scan of the stream; with several, `put` / `put_raw` the feeds' next scans and `advance()`.  `add(id, box, feed=)` starts
-    a target on its feed's most recent scan, `drop(id)` ends it."""
+    a target on its feed's most recent scan, `drop(id)` ends it.  `feeds` is a number of feeds, or a `ScanFeeds` store the
+    tracker shares with others (MultiClassTracker): only the store's owner advances (its ingest serves every tracker on the
+    store), and `_run()` advances this one tracker's slots."""
 
     def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1, precision="fp32"):
         self.precision = runtime.check_precision(precision)
@@ -71,19 +207,21 @@ class MultiTargetTracker:
             raise ValueError("shape_aggregation 'all' is not supported by the live multi-target tracker")
         self.N = N = int(max_points)
         self.K = K = int(max_targets)
-        self.F = F = int(feeds)
+        shared = isinstance(feeds, ScanFeeds)
+        self.F = F = feeds.F if shared else int(feeds)
         if N < 1 or K < 1 or K > 65535 or F < 1:
             raise ValueError(f"max_points={N}, max_targets={K} and feeds={F} must be >= 1 (max_targets <= 65535)")
+        if shared:
+            if feeds.dev != dev or feeds.N != N:
+                raise ValueError(f"the scan feeds hold {feeds.N} points per scan on {feeds.dev}; the tracker was asked for "
+                                 f"max_points={N} on {dev}")
+            self.scan_feeds = feeds
+        else:
+            self.scan_feeds = ScanFeeds(N, F, dev)
+        if self.scan_feeds.owner is None:
+            self.scan_feeds.claim(self)
         f = dict(device=dev, dtype=torch.float32)
         i64 = dict(device=dev, dtype=torch.int64)
-        self.scans = torch.zeros(F, 2, N, 3, **f)
-        self.count = torch.zeros(F, 2, **i64)
-        # per feed: fed by this advance (0 / 1), the half holding its most recent scan, the half holding the scan before it;
-        # written from the host mirrors below before every step
-        self.fstate = torch.tensor([[0] * F, [1] * F, [0] * F], **i64)
-        self._fcur, self._fprev = [1] * F, [0] * F
-        self.feed_seen = [0] * F                          # scans advanced per feed
-        self._staged = {}                                 # feed -> None (already in its buffer) or (rows, transforms)
         self.slot_feed = torch.zeros(K, **i64)
         self.cur = torch.ones(K, **i64)                  # per slot: scan index (2 * feed + half) of its feed's most recent scan ...
         self.prev = torch.zeros(K, **i64)                # ... and of the scan before it
@@ -101,8 +239,24 @@ class MultiTargetTracker:
             self.first_local = torch.zeros(K, N, 3, **f)
             self.first_keep = torch.zeros(K, N, dtype=torch.bool, device=dev)
         self.slot_of = {}                                 # target id -> slot
-        self.scans_seen = 0
         self.graph = None
+
+    # the feed state lives in the (possibly shared) ScanFeeds store
+    scans = property(lambda self: self.scan_feeds.scans)
+    count = property(lambda self: self.scan_feeds.count)
+    fstate = property(lambda self: self.scan_feeds.fstate)
+    feed_seen = property(lambda self: self.scan_feeds.feed_seen)
+    _fcur = property(lambda self: self.scan_feeds.fcur)
+    _fprev = property(lambda self: self.scan_feeds.fprev)
+    _staged = property(lambda self: self.scan_feeds.staged)
+
+    @property
+    def scans_seen(self):
+        return self.scan_feeds.scans_seen
+
+    @scans_seen.setter
+    def scans_seen(self, n):
+        self.scan_feeds.scans_seen = n
 
     # ------------------------------------------------------------------ one step for all slots, fixed shapes
     def _crop(self, which, box, half, perm, pick, size, prefix=False):
@@ -152,96 +306,44 @@ class MultiTargetTracker:
             self.box_r.copy_(torch.where(a[..., None], new.rot, self.box_r))
             self.first_flag.masked_fill_(adv, 0.0)
 
+    def _state(self):
+        """The slot state one step advances (what the warm-up before a capture must put back)."""
+        return (self.cur, self.prev, self.t, self.box_c, self.box_r, self.first_flag, self.u_lim)
+
     def _capture(self):
-        # the warm-up runs a real step; the state it advances is restored before the captured graph's first replay
-        state = (self.cur, self.prev, self.t, self.box_c, self.box_r, self.first_flag, self.u_lim)
-        snap = [t.clone() for t in state]
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            self._step()                                                       # warm-up (allocations, weight packing)
-        torch.cuda.current_stream().wait_stream(s)
-        for t, v in zip(state, snap):
-            t.copy_(v)
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self._step()
-        for t, v in zip(state, snap):
-            t.copy_(v)
+        self.graph = capture_step(self._step, self._state())
 
-    # ------------------------------------------------------------------ public interface
-    def _feed(self, feed):
-        f = int(feed)
-        if not 0 <= f < self.F:
-            raise ValueError(f"feed {f} out of range: the tracker has feeds 0 .. {self.F - 1}")
-        return f
-
-    def _stage(self, feed, n):
-        f = self._feed(feed)
-        if f in self._staged:
-            raise ValueError(f"feed {f} already has a scan staged: advance() before the next put")
-        if n > self.N:
-            raise ValueError(f"max_points: the scan has {n} points, the tracker was built for {self.N}")
-        return f
-
-    def put(self, feed, points, n_valid=None):
-        """Stage the next scan of `feed`: `points` (n, 3), the first `n_valid` valid.  A CUDA tensor is copied into the feed's next
-        buffer at once; a host tensor or array goes through the packed copy and the ingest kernel of the next `advance()`.  No
-        host sync."""
-        n = points.shape[0]
-        f = self._stage(feed, n)
-        n_valid = n if n_valid is None else min(int(n_valid), n)
-        if isinstance(points, torch.Tensor) and (points.device == self.dev or self.dev.type != "cuda"):
-            nxt = 1 - self._fcur[f]
-            self.scans[f, nxt, :n].copy_(points, non_blocking=True)
-            self.count[f, nxt].fill_(n_valid)
-            self._staged[f] = None
-        else:
-            rows = points.numpy() if isinstance(points, torch.Tensor) else np.asarray(points)
-            self._staged[f] = (rows[:n_valid], ())
-
-    def put_raw(self, feed, rows, transforms=()):
-        """Stage the next scan of `feed` as a reader stores it: `rows` (n, stride) float32 / float64 (x, y, z first, 3 <= stride
-        <= 16) and up to two affine transforms (3x4 or 4x4, applied in order in float64, as the readers apply them on the host).
-        The next `advance()` moves every staged raw scan to the device in one copy and one `o3d_scan_ingest` launch."""
-        rows = np.asarray(rows)
-        if self.dev.type != "cuda":
-            raise RuntimeError("put_raw: scan ingest runs on the GPU; this tracker is not on a CUDA device")
-        if rows.ndim != 2 or not 3 <= rows.shape[1] <= 16:
-            raise ValueError(f"put_raw: rows of shape {rows.shape}; expected (points, 3 .. 16 values per row)")
-        transforms = [np.asarray(m, np.float64) for m in transforms]
-        if len(transforms) > 2 or any(m.shape not in ((3, 4), (4, 4)) for m in transforms):
-            raise ValueError("put_raw: at most two transforms, each 3x4 or 4x4")
-        f = self._stage(feed, rows.shape[0])
-        self._staged[f] = (rows, transforms)
-
-    def advance(self):
-        """Bring in every staged scan and advance the active targets of those feeds to it, in one replay of the captured step;
-        the other feeds hold.  Returns `boxes()`: device views of the slots' state, no host sync."""
-        F, staged = self.F, self._staged
-        raw = [(f, 1 - self._fcur[f], v[0], v[1]) for f, v in sorted(staged.items()) if v is not None]
-        for f in staged:
-            self._fprev[f], self._fcur[f] = self._fcur[f], 1 - self._fcur[f]
-            self.feed_seen[f] += 1
-        state = np.array([[int(f in staged) for f in range(F)], self._fcur, self._fprev], dtype=np.int64)
-        if self.dev.type == "cuda":
-            # one host->device copy per step: the feeds' state, the ingest descriptors and every raw scan's rows
-            buf, desc, d0, s0 = ops.pack_scans(raw, head=state.nbytes)
-            buf.numpy()[:state.nbytes] = state.reshape(-1).view(np.uint8)
-            dev = buf.to(self.dev, non_blocking=True)
-            self.fstate.copy_(dev[:state.nbytes].view(torch.int64).view(3, F))
-            if raw:
-                ops.scan_ingest(self.scans, self.count, desc, dev, d0, s0)
-        else:
-            self.fstate.copy_(torch.from_numpy(state))
+    def _run(self):
+        """Advance the slots to the scans the feed store has just brought in: the captured step's replay, or the eager step."""
         if not self.use_graph:
             self._step()
         else:
             if self.graph is None:
                 self._capture()
             self.graph.replay()
-        self.scans_seen += len(staged)
-        staged.clear()
+
+    # ------------------------------------------------------------------ public interface
+    def _feed(self, feed):
+        return self.scan_feeds.feed(feed)
+
+    def put(self, feed, points, n_valid=None):
+        """Stage the next scan of `feed` (ScanFeeds.put): a CUDA tensor is copied into the feed's next buffer at once, a host
+        tensor or array goes through the packed copy and the ingest kernel of the next `advance()`.  No host sync."""
+        self.scan_feeds.put(feed, points, n_valid)
+
+    def put_raw(self, feed, rows, transforms=()):
+        """Stage the next scan of `feed` as a reader stores it (ScanFeeds.put_raw): the next `advance()` ingests it on the
+        device."""
+        self.scan_feeds.put_raw(feed, rows, transforms)
+
+    def advance(self):
+        """Bring in every staged scan and advance the active targets of those feeds to it, in one replay of the captured step;
+        the other feeds hold.  Returns `boxes()`: device views of the slots' state, no host sync."""
+        if self.scan_feeds.owner is not self:
+            raise RuntimeError("advance(): this tracker shares scan feeds that another tracker owns; an ingest here would move "
+                               "every sharing tracker's scans without advancing them, so advance the owner")
+        self.scan_feeds.ingest()
+        self._run()
         return self.boxes()
 
     def step(self, points, n_valid=None):
@@ -372,30 +474,48 @@ def scene_peak(n_frames, starts, ends):
     return peak
 
 
+def class_peaks(n_frames, starts, ends):
+    """`scene_peak` per class, for targets keyed (class, id): {class: the most targets of that class active at once}."""
+    classes = dict.fromkeys(tid[0] for group in starts.values() for tid, _ in group)
+    return {c: scene_peak(n_frames, {t: [(tid, b) for tid, b in group if tid[0] == c] for t, group in starts.items()}, ends)
+            for c in classes}
+
+
 def feed_schedule(lengths, peaks, feeds, max_targets):
     """When and on which feed every scene runs.  Scenes are admitted longest first (ties in scene order); the next scene waits
     for a free feed and for `peaks[i]` free slots, the most targets it has active at once, which stay reserved until it ends.  A
     feed is reused from the step after its scene's last frame.  Returns [(scene, feed, first step)] in admission order; scene i
-    runs its frame t at step first + t."""
+    runs its frame t at step first + t.  Per class: `max_targets` {class: slots} and `peaks[i]` {class: peak} (class_peaks);
+    a scene then waits until every class has its peak free."""
     n = len(lengths)
+    per_class = isinstance(max_targets, dict)
+    cap = {c: int(k) for c, k in max_targets.items()} if per_class else {None: int(max_targets)}
+    need = [{c: q for c, q in p.items() if q > 0} for p in peaks] if per_class else [{None: p} for p in peaks]
     for i in range(n):
         if lengths[i] < 1:
             raise ValueError(f"scene {i} has no frames")
-        if peaks[i] > max_targets:
-            raise ValueError(f"max_targets={max_targets}: scene {i} has {peaks[i]} targets active at once and can never fit")
+        for c, p in need[i].items():
+            if not per_class:
+                if p > cap[c]:
+                    raise ValueError(f"max_targets={cap[c]}: scene {i} has {p} targets active at once and can never fit")
+            elif p > cap.get(c, 0):
+                raise ValueError(f"max_targets[{c!r}]={cap.get(c, 0)}: scene {i} has {p} targets of class {c!r} active at once "
+                                 f"and can never fit")
     order = sorted(range(n), key=lambda i: -lengths[i])
-    free_feeds, free_slots, running, out = list(range(int(feeds))), int(max_targets), [], []
+    free_feeds, free_slots, running, out = list(range(int(feeds))), dict(cap), [], []
     step, q = 0, 0
     while q < n:
         for e, i, f in [r for r in running if r[0] < step]:
             running.remove((e, i, f))
             free_feeds.append(f)
-            free_slots += peaks[i]
+            for c, p in need[i].items():
+                free_slots[c] += p
         free_feeds.sort()
-        while q < n and free_feeds and peaks[order[q]] <= free_slots:
+        while q < n and free_feeds and all(p <= free_slots[c] for c, p in need[order[q]].items()):
             i = order[q]
             f = free_feeds.pop(0)
-            free_slots -= peaks[i]
+            for c, p in need[i].items():
+                free_slots[c] -= p
             running.append((step + lengths[i] - 1, i, f))
             out.append((i, f, step))
             q += 1
@@ -404,19 +524,8 @@ def feed_schedule(lengths, peaks, feeds, max_targets):
     return out
 
 
-def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32"):
-    """Track many scenes through one tracker with `feeds` scan feeds (`feed_schedule` decides which scene runs when and where).
-    `scenes`: [{"frames": number of scans, "scan": t -> the scene's scan t, either (rows, transforms) for `put_raw` or an (n, 3)
-    tensor / array for `put`, "starts": {t: [(id, Box), ...]}, "ends": {id: last t}}]; a target without an end runs to its scene's
-    last frame, and target ids are unique over all scenes.  `max_points`: the scan buffer's size (required).
-    A host thread reads the next step's scans while the current step runs; the boxes are read back from the device every
-    `chunk` steps.  Returns, per scene, {id: {t: data_classes.Box}} from the frame a target starts on to its last frame."""
-    from concurrent.futures import ThreadPoolExecutor
-
-    from ..datasets.data_classes import Box
-    runtime.check_precision(precision)
-    if max_points is None:
-        raise ValueError("track_feeds: give max_points, the largest scan of the scenes")
+def _scene_targets(scenes):
+    """{target: scene} (ids must be unique over all scenes) and, per scene, {frame: targets dropped after it}."""
     scene_of, last = {}, []
     for i, sc in enumerate(scenes):
         T = int(sc["frames"])
@@ -430,9 +539,19 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
             for tid, _ in group:
                 drops.setdefault(min(sc["ends"].get(tid, T - 1), T - 1), []).append(tid)
         last.append(drops)
+    return scene_of, last
+
+
+def run_scenes(trk, add, drop, scenes, sched, chunk=256):
+    """Drive `trk` (a MultiTargetTracker or a MultiClassTracker) through `scenes` on the feeds and steps of `sched`
+    (feed_schedule); `add(tid, box, feed)` / `drop(tid)` start and end a target, `trk.targets()` maps the live targets to rows of
+    `trk.snapshot()`.  A host thread reads the next step's scans while the current step runs; the boxes are read back from the
+    device every `chunk` steps.  Returns, per scene, {id: {t: data_classes.Box}}."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    from ..datasets.data_classes import Box
+    scene_of, last = _scene_targets(scenes)
     lengths = [int(sc["frames"]) for sc in scenes]
-    peaks = [scene_peak(lengths[i], sc["starts"], sc["ends"]) for i, sc in enumerate(scenes)]
-    sched = feed_schedule(lengths, peaks, feeds, max_targets)
     n_steps = max((s0 + lengths[i] for i, _, s0 in sched), default=0)
     work = [[] for _ in range(n_steps)]                                        # per step: (feed, scene, frame)
     first = {}
@@ -440,7 +559,6 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
         first[i] = s0
         for t in range(lengths[i]):
             work[s0 + t].append((f, i, t))
-    trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, feeds=feeds, precision=precision)
     out = [{} for _ in scenes]
     pending, inflight = [], []
 
@@ -481,14 +599,14 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
             trk.advance()
             for f, i, t, _ in items:
                 for tid, box in scenes[i]["starts"].get(t, ()):
-                    trk.add(tid, box, feed=f)
+                    add(tid, box, f)
             live = trk.targets()
             if live:
                 pending.append((s, live, trk.snapshot()))
             for f, i, t, _ in items:
                 for tid in last[i].get(t, ()):
                     if tid in live:
-                        trk.drop(tid)
+                        drop(tid)
             if len(pending) >= chunk:
                 read_back()
                 if len(inflight) > 1:
@@ -498,3 +616,21 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
     while inflight:
         decode()
     return out
+
+
+def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32"):
+    """Track many scenes through one tracker with `feeds` scan feeds (`feed_schedule` decides which scene runs when and where).
+    `scenes`: [{"frames": number of scans, "scan": t -> the scene's scan t, either (rows, transforms) for `put_raw` or an (n, 3)
+    tensor / array for `put`, "starts": {t: [(id, Box), ...]}, "ends": {id: last t}}]; a target without an end runs to its scene's
+    last frame, and target ids are unique over all scenes.  `max_points`: the scan buffer's size (required).
+    A host thread reads the next step's scans while the current step runs; the boxes are read back from the device every
+    `chunk` steps.  Returns, per scene, {id: {t: data_classes.Box}} from the frame a target starts on to its last frame."""
+    runtime.check_precision(precision)
+    if max_points is None:
+        raise ValueError("track_feeds: give max_points, the largest scan of the scenes")
+    _scene_targets(scenes)
+    lengths = [int(sc["frames"]) for sc in scenes]
+    peaks = [scene_peak(lengths[i], sc["starts"], sc["ends"]) for i, sc in enumerate(scenes)]
+    sched = feed_schedule(lengths, peaks, feeds, max_targets)
+    trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, feeds=feeds, precision=precision)
+    return run_scenes(trk, lambda tid, box, f: trk.add(tid, box, feed=f), trk.drop, scenes, sched, chunk)
