@@ -209,6 +209,20 @@ int o3d_pw_dgrad_tc(const float* g, int ldg, const float* y, int ldy, const floa
  * ---------------------------------------------------------------------------------------------- */
 #define O3D_MAX_LAYERS 8
 
+/* Row counts P at which a stack's kernel plan changes, so that a layer's arithmetic depends on which side of them P lies:
+ *   O3D_TC_MIN_P_INFER / O3D_TC_MIN_P_TRAIN: below it (eval / training mode) no layer runs the tensor-core forward, every
+ *     layer runs the exact-fp32 CUDA-core GEMM;
+ *   O3D_TC_BWD_MIN_P: the tensor-core data gradient, which a lifted stack also needs to keep its first layer's output virtual;
+ *   O3D_FWD_SKINNY_MIN_P: a CUDA-core forward layer with at most 8 input columns and no pooling streams through the skinny
+ *     kernel from here on.
+ * o3d_stack_plan_thresholds(d, out) (declared after o3d_stack_t below) writes to out[0 .. 3] the ones that can change the eval-mode plan of the stack `d`
+ * (whatever its P) and returns how many.  A caller that needs one result at several row counts (the live tracker's occupancy
+ * buckets) keeps every stack on one side of each of them.                                                           */
+#define O3D_TC_MIN_P_TRAIN 128
+#define O3D_TC_MIN_P_INFER 16
+#define O3D_TC_BWD_MIN_P 128
+#define O3D_FWD_SKINNY_MIN_P 4096
+
 /* "Lifted" first layer.  When the first 1x1 convolution of a stack acts on GROUPED rows — QueryAndGroup
  * (pointnet2_utils.py:317-329: [xyz(idx) - centre, features(idx)]), BoxAwareXCorr's top-k grouping (xcorr.py:87-90) or
  * P2B_XCorr's [similarity, template xyz, template feature] fusion tensor (xcorr.py:39-46) — its linearity lets the
@@ -284,6 +298,8 @@ typedef struct o3d_stack_t {
                                  partial tiles and their fixed-order reduction, the lifted layer's gather / scatter passes and
                                  every CUDA-core layer stay fp32.                                                          */
 } o3d_stack_t;
+
+int o3d_stack_plan_thresholds(const o3d_stack_t* d, int* out);   /* see O3D_TC_MIN_P_INFER above */
 
 long long o3d_stack_workspace_bytes(const o3d_stack_t* d, int backward);
 /* Static-weight inference (the B=1 tracking loop): pack the weights / fold the running BN statistics once. */

@@ -71,6 +71,7 @@ PROTOTYPES = {
                              ctypes.c_longlong, _p],
     "o3d_pw_bwd_tc": [_p, _i, _p, _i, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p, _i,
                       _p, ctypes.c_longlong, _p],
+    "o3d_stack_plan_thresholds": [_p, _p],
     "o3d_stack_workspace_bytes": [_p, _i],
     "o3d_stack_prepared_bytes": [_p],
     "o3d_stack_prepare": [_p, _p, _p],

@@ -906,7 +906,7 @@ extern "C" int o3d_pw_fwd(const float* x, int ldx, const float* in_scale, const 
     ActIn ain{x, ldx, in_scale, in_shift, in_relu};
     FwdEpi ep{y, ldy, bias, sum, sumsq, S, ymax, ymin, arg, ldp};
     cudaStream_t st = (cudaStream_t)stream;
-    if (K <= 8 && S == 0 && P >= 4096) {
+    if (K <= 8 && S == 0 && P >= O3D_FWD_SKINNY_MIN_P) {
         if (K <= 4) return launch_fwd_skinny<1>(ain, wt, ldw, P, K, Nw, ep, st);
         return launch_fwd_skinny<2>(ain, wt, ldw, P, K, Nw, ep, st);
     }

@@ -173,9 +173,9 @@ bool make_plan(const o3d_stack_t* d, Plan& p) {
         // (inference: also narrow output layers — 1 / 5 / 9 channels of the heads — as one partly filled channel tile)
         // (inference: any output width — e.g. the vote layer's 3 + 256 channels — as whole + one partly filled channel tile)
         p.tc_f[l] = (d->use_tc & 1) && (p.Nw[l] % 128 == 0 || p.Nw[l] == 64 || !d->training) && p.K[l] >= 32 &&
-                    d->P >= (d->training ? 128 : 16) &&
+                    d->P >= (d->training ? O3D_TC_MIN_P_TRAIN : O3D_TC_MIN_P_INFER) &&
                     !(l == d->n_layers - 1 && d->S > 0 && 64 % d->S != 0);
-        p.tc_b[l] = (d->use_tc & 1) && p.K[l] >= 64 && p.Nw[l] >= 32 && d->P >= 128;
+        p.tc_b[l] = (d->use_tc & 1) && p.K[l] >= 64 && p.Nw[l] >= 32 && d->P >= O3D_TC_BWD_MIN_P;
         p.tc_w[l] = (d->use_tc & 2) && p.Nw[l] >= 64 && p.K[l] >= 64 && d->P >= 4096;
     }
     if (p.lift) {
@@ -285,6 +285,20 @@ extern "C" long long o3d_stack_workspace_bytes(const o3d_stack_t* d, int backwar
     Plan p;
     if (!d || !make_plan(d, p)) return -1;
     return (long long)(backward ? p.bwd_bytes : p.fwd_bytes);
+}
+
+extern "C" int o3d_stack_plan_thresholds(const o3d_stack_t* d, int* out) {
+    if (!d || !out || d->n_layers < 1 || d->n_layers > O3D_MAX_LAYERS) return -1;
+    int n = 0;
+    out[n++] = O3D_TC_MIN_P_INFER;                       // every layer's tensor-core forward test (make_plan)
+    if (d->lift) out[n++] = O3D_TC_BWD_MIN_P;            // the virtual first-layer output needs tc_b (make_plan)
+    // o3d_pw_fwd's skinny kernel: a layer with at most 8 input columns (the first, or one after a layer at most 8 wide) that
+    // is not the pooled last layer
+    for (int l = d->lift ? 1 : 0; l < d->n_layers; ++l) {
+        const int k = l == 0 ? d->K0 : r4(d->cout[l - 1]);
+        if (k <= 8 && !(l == d->n_layers - 1 && d->S > 0)) { out[n++] = O3D_FWD_SKINNY_MIN_P; break; }
+    }
+    return n;
 }
 
 extern "C" long long o3d_stack_prepared_bytes(const o3d_stack_t* d) {

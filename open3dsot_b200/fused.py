@@ -235,6 +235,12 @@ class _StackFn(torch.autograd.Function):
             lf.s, lf.u = _ptr(s), _ptr(u)
             d.lift = ctypes.pointer(lf)
         L = _lib.lib()
+        if runtime.recording_stack_rows():
+            th = (ctypes.c_int * 4)()
+            n = L.o3d_stack_plan_thresholds(ctypes.byref(d), th)
+            if n < 0:
+                raise RuntimeError("fused MLP stack: invalid stack description")
+            runtime.note_stack_rows(P, th[:n])
         need_grad = meta.grad_mode and any(ctx.needs_input_grad)   # (needs_input_grad mirrors requires_grad even under no_grad)
         d.precision = _precision_code(meta.training, need_grad)
         block = None            # inference with static weights: the prepared block, referenced here until the forward is enqueued

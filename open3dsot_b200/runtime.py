@@ -177,6 +177,35 @@ def grad_inplace_scope():
         _GRAD_INPLACE = old
 
 
+# (row count, plan threshold) pairs of the fused MLP stacks that run inside stack_rows_scope() (None outside one).
+_STACK_ROWS = None
+
+
+def recording_stack_rows() -> bool:
+    return _STACK_ROWS is not None
+
+
+def note_stack_rows(P, thresholds) -> None:
+    """Record a stack forward of P rows whose kernel plan changes at the row counts `thresholds`."""
+    if _STACK_ROWS is not None:
+        _STACK_ROWS.update((int(P), int(t)) for t in thresholds)
+
+
+@contextlib.contextmanager
+def stack_rows_scope():
+    """`with runtime.stack_rows_scope() as rows:` — `rows` (a set) collects, for every fused MLP stack forward run inside, its
+    row count P paired with each row count at which that stack's kernel plan changes (include/o3d_b200.h,
+    o3d_stack_plan_thresholds).  A caller that runs one network at several batch sizes reads from it which sizes share one
+    kernel plan."""
+    global _STACK_ROWS
+    old = _STACK_ROWS
+    _STACK_ROWS = set()
+    try:
+        yield _STACK_ROWS
+    finally:
+        _STACK_ROWS = old
+
+
 def tc_level() -> int:
     return _TC
 

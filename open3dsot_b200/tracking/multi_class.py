@@ -1,11 +1,13 @@
-"""Live tracking of several object classes over shared scan feeds: one model per class, one scan ingest, one captured step.
+"""Live tracking of several object classes over shared scan feeds: one model per class, one scan ingest, one step per class.
 
 Every class keeps its own model, config, weights and static-weight caches, and its own `MultiTargetTracker` (its slots, its
-`max_targets`, its template mode, its motion or siamese inputs), all built over one `ScanFeeds` store.  `advance()` brings the
-staged scans in once (one packed host->device copy and one `o3d_scan_ingest` launch for every feed) and replays one captured
-graph in which every class's unchanged step runs as its own branch: the graph forks one side stream per class and joins them at
-the end, the fork / join `fused.run_ahead` uses for the template and search branches.  The classes may be different model
-families (BAT for cars, M2-Track for pedestrians).
+`max_targets`, its template mode, its motion or siamese inputs, its occupancy buckets and their captured steps), all built over
+one `ScanFeeds` store.  `advance()` brings the staged scans in once (one packed host->device copy and one `o3d_scan_ingest`
+launch for every feed), then every class picks the bucket of its own work list and replays that bucket's captured step on its
+own side stream, forked from the current stream before and joined into it after, the fork / join `fused.run_ahead` uses for the
+template and search branches.  A class with nothing to advance replays nothing.  Each class's bucket graphs share one memory
+pool, and the classes keep separate pools, since they replay side by side.  The classes may be different model families (BAT
+for cars, M2-Track for pedestrians).
 
 A target is named (class, id); ids are unique within a class and key the target's draws as in a lone tracker, so its boxes
 depend neither on the other classes nor on their slot counts: they are bitwise what a `MultiTargetTracker` of its class with
@@ -14,7 +16,7 @@ are read in (`up_axis`, `IoU_space`, `degrees`)."""
 import torch
 
 from .. import runtime
-from .multi_tracker import MultiTargetTracker, ScanFeeds, capture_step, class_peaks, feed_schedule, run_scenes
+from .multi_tracker import MultiTargetTracker, ScanFeeds, class_peaks, feed_schedule, run_scenes
 
 SHARED_KEYS = ("up_axis", "IoU_space", "degrees")
 
@@ -45,14 +47,13 @@ class MultiClassTracker:
                     raise ValueError(f"class {n!r}: {key}={b} differs from class {names[0]!r}'s {key}={a}; the classes of one "
                                      f"tracker share the frame their boxes are read in")
         self.dev = dev = next(models[names[0]].parameters()).device
-        self.use_graph = bool(use_graph) and dev.type == "cuda"
         self.scan_feeds = feeds if isinstance(feeds, ScanFeeds) else ScanFeeds(max_points, feeds, dev)
         self.scan_feeds.claim(self)                       # before the class trackers: they share the store, this one advances it
         self.F = self.scan_feeds.F
         self.trackers = {}
         for n in names:
             try:
-                self.trackers[n] = MultiTargetTracker(models[n], max_points, max_targets[n], seed=seed, use_graph=False,
+                self.trackers[n] = MultiTargetTracker(models[n], max_points, max_targets[n], seed=seed, use_graph=use_graph,
                                                       feeds=self.scan_feeds, precision=precision)
             except ValueError as e:
                 self.scan_feeds.owner = None
@@ -63,25 +64,21 @@ class MultiClassTracker:
             self.offset[n], k = k, k + trk.K
         self.K = k
         self._streams = {n: torch.cuda.Stream(device=dev) for n in names} if dev.type == "cuda" else {}
-        self.graph = None
 
-    # ------------------------------------------------------------------ one step: every class's step as its own branch
-    def _step(self):
+    # ------------------------------------------------------------------ one step: every class's bucket step on its own stream
+    def _run(self, fed):
         if not self._streams:
             for trk in self.trackers.values():
-                trk._step()
+                trk._run(fed)
             return
         cur = torch.cuda.current_stream()
         for n, trk in self.trackers.items():
             side = self._streams[n]
             side.wait_stream(cur)
             with torch.cuda.stream(side):
-                trk._step()
+                trk._run(fed)
         for side in self._streams.values():
             cur.wait_stream(side)
-
-    def _capture(self):
-        self.graph = capture_step(self._step, [t for trk in self.trackers.values() for t in trk._state()])
 
     # ------------------------------------------------------------------ public interface
     def _class(self, cls):
@@ -99,15 +96,11 @@ class MultiClassTracker:
         self.scan_feeds.put_raw(feed, rows, transforms)
 
     def advance(self):
-        """Bring in every staged scan (one copy, one ingest) and advance every class's active targets of those feeds to it, in
-        one replay of the captured step.  Returns {class: that class tracker's boxes()}, device views; no host sync."""
+        """Bring in every staged scan (one copy, one ingest) and advance every class's active targets of those feeds to it, each
+        class in one replay of its bucket's captured step.  Returns {class: that class tracker's boxes()}, device views; no host sync."""
+        fed = set(self.scan_feeds.staged)
         self.scan_feeds.ingest()
-        if not self.use_graph:
-            self._step()
-        else:
-            if self.graph is None:
-                self._capture()
-            self.graph.replay()
+        self._run(fed)
         return {n: trk.boxes() for n, trk in self.trackers.items()}
 
     def step(self, points, n_valid=None):

@@ -2,7 +2,7 @@
 
 `DeviceTracker` follows one target and `BatchedDeviceTracker` replays pre-loaded tracklets with ground truth for every frame;
 this tracker takes the scans as they arrive and targets as they appear and disappear:
-  * `step(points)` copies the scan into a static (2, N, 3) ping-pong buffer (the one copy of the scan) and replays one captured
+  * `step(points)` copies the scan into a static (2, N, 3) ping-pong buffer (the one copy of the scan) and replays a captured
     step that advances every active slot to it: search crop of the new scan around the slot's result box, template = the
     first-frame crop (kept per slot) + the previous scan's crop in the result box ('firstandprevious', or either one alone for
     'first' / 'previous'), or for motion models (M2-Track) the previous and current scans' crops, then BoxCloud, the network in
@@ -14,8 +14,15 @@ this tracker takes the scans as they arrive and targets as they appear and disap
     both between steps and without a host synchronisation;
   * a slot's draws are keyed by (seed, target id, frame within the target's track), so a target's result does not depend on its
     slot, on the other targets or on `max_targets`.
-Idle slots run on a fixed dummy box and report nothing: the cost of a step follows `max_targets`, not the number of active
-targets.
+Occupancy buckets.  A step runs over the targets it advances only: the host forms the work list (the active slots whose feed got
+a scan, in slot order) and runs the step at the smallest bucket that holds it, out of the powers of two below `max_targets` and
+`max_targets` itself.  Each bucket has its own captured graph, all captured on the first advance and sharing one memory pool; the
+graph gathers its rows' state (box, key, frame, first-frame flag and prefix, feed) through the work list, uploaded without a
+sync, and scatters the box, frame counter and first-frame flag back into their slots; padding rows read an idle row and write
+nowhere that is read.  Slots never move, so `boxes()` / `snapshot()` keep the slot layout.  Rows of a step are independent, and
+the smallest bucket is one at which every MLP stack keeps the kernel plan it has over all slots (o3d_stack_plan_thresholds), so a
+target's boxes are bitwise the same at every bucket.  A step therefore costs what its bucket costs, not what `max_targets` does;
+an advance with no target to advance runs the ingest alone.
 
 Feeds.  A feed is one sequence of scans: one sensor, or one recorded scene.  With `feeds=F` the scan buffer is (F, 2, N, 3), every
 slot follows one feed, and each feed has its own ping-pong parity.  `put(feed, points)` (xyz) or `put_raw(feed, rows, transforms)`
@@ -164,9 +171,10 @@ class ScanFeeds:
         staged.clear()
 
 
-def capture_step(step, state):
-    """Capture `step()` in a CUDA graph.  The warm-up runs a real step (allocations, weight packing) on a side stream; `state`,
-    the tensors a step advances, is put back after it and after the capture, so the graph's first replay is the first step."""
+def capture_step(step, state, pool=None):
+    """Capture `step()` in a CUDA graph (in the memory pool `pool`, or a private one).  The warm-up runs a real step
+    (allocations, weight packing) on a side stream; `state`, the tensors a step advances, is put back after it and after the
+    capture, so the graph's first replay is the first step."""
     snap = [t.clone() for t in state]
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -176,16 +184,53 @@ def capture_step(step, state):
     for t, v in zip(state, snap):
         t.copy_(v)
     graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
+    with torch.cuda.graph(graph, pool=pool):
         step()
     for t, v in zip(state, snap):
         t.copy_(v)
     return graph
 
 
+# ------------------------------------------------------------------ occupancy buckets
+def occupancy_buckets(K, smallest=1):
+    """The row counts a K-slot tracker's step runs at: the powers of two from `smallest` up to below K, then K itself."""
+    out, b = [], 1
+    while b < K:
+        if b >= smallest:
+            out.append(b)
+        b *= 2
+    return tuple(out) + (K,)
+
+
+def smallest_bucket(K, rows):
+    """The fewest step rows at which every MLP stack of a K-row step keeps its kernel plan.  `rows`: (P, T) pairs from
+    runtime.stack_rows_scope() over that step, a stack's row count P (proportional to the step's rows) with each row count T at
+    which its plan changes (o3d_stack_plan_thresholds).  A stack below T at K is below it at every smaller size; one at or
+    above it must stay there, which takes ceil(T * K / P) rows."""
+    return max([-(-t * K // p) for p, t in rows if p >= t], default=1)
+
+
+def bucket_for(n, buckets):
+    """The smallest bucket that holds n rows."""
+    return next(b for b in buckets if b >= n)
+
+
+def work_slots(slot_feed, fed):
+    """The work list of one advance: the slots of `slot_feed` ({slot: feed} of the active targets) whose feed is in `fed`, in
+    slot order."""
+    return sorted(k for k, f in slot_feed.items() if f in fed)
+
+
+def work_rows(slots, K):
+    """(2, K) int64: the rows a bucket step gathers its state from (the work list, then K, the idle row) and the rows it
+    scatters its results to (the work list, then K + 1, a row nothing reads)."""
+    n = len(slots)
+    return np.array([list(slots) + [K] * (K - n), list(slots) + [K + 1] * (K - n)], dtype=np.int64)
+
+
 class MultiTargetTracker:
     """`max_targets` slots over `feeds` scan feeds of at most `max_points` points per scan.  `seed` keys the random draws;
-    `use_graph`: capture the step in a CUDA graph on the first advance (eager otherwise).  With one feed, call `step(scan)` for
+    `use_graph`: capture the step of every occupancy bucket in a CUDA graph on the first advance (eager otherwise).  With one feed, call `step(scan)` for
     every scan of the stream; with several, `put` / `put_raw` the feeds' next scans and `advance()`.  `add(id, box, feed=)` starts
     a target on its feed's most recent scan, `drop(id)` ends it.  `feeds` is a number of feeds, or a `ScanFeeds` store the
     tracker shares with others (MultiClassTracker): only the store's owner advances (its ingest serves every tracker on the
@@ -222,24 +267,29 @@ class MultiTargetTracker:
             self.scan_feeds.claim(self)
         f = dict(device=dev, dtype=torch.float32)
         i64 = dict(device=dev, dtype=torch.int64)
-        self.slot_feed = torch.zeros(K, **i64)
-        self.cur = torch.ones(K, **i64)                  # per slot: scan index (2 * feed + half) of its feed's most recent scan ...
-        self.prev = torch.zeros(K, **i64)                # ... and of the scan before it
         self.arange = torch.arange(N, device=dev)
-        # slot state; idle slots hold the dummy box
-        self.box_c = torch.zeros(K, 3, **f)
-        self.box_s = torch.ones(K, 3, **f)
-        self.box_r = torch.eye(3, **f).repeat(K, 1, 1)
-        self.first_flag = torch.zeros(K, **f)
-        self.active = torch.zeros(K, dtype=torch.bool, device=dev)
-        self.key = torch.zeros(K, **i64)                  # target id of the slot (the key of its draws)
-        self.t = torch.zeros(K, **i64)                    # frame within the target's track
-        self.u_lim = torch.zeros(K, 2, **f)
+        # Slot state, K + 2 rows: the K slots (the public attributes are views of them), row K the idle state the padding rows of
+        # a bucket step read, row K + 1 where they write.  Idle slots and row K hold the dummy box.
+        self._slot_feed = torch.zeros(K + 2, **i64)
+        self._box_c = torch.zeros(K + 2, 3, **f)
+        self._box_s = torch.ones(K + 2, 3, **f)
+        self._box_r = torch.eye(3, **f).repeat(K + 2, 1, 1)
+        self._first_flag = torch.zeros(K + 2, **f)
+        self._active = torch.zeros(K + 2, dtype=torch.bool, device=dev)
+        self._key = torch.zeros(K + 2, **i64)             # target id of the slot (the key of its draws)
+        self._t = torch.zeros(K + 2, **i64)               # frame within the target's track
+        self.slot_feed, self.box_c, self.box_s, self.box_r = (x[:K] for x in (self._slot_feed, self._box_c, self._box_s, self._box_r))
+        self.first_flag, self.active, self.key, self.t = (x[:K] for x in (self._first_flag, self._active, self._key, self._t))
         if self.mode in ("firstandprevious", "first"):
-            self.first_local = torch.zeros(K, N, 3, **f)
-            self.first_keep = torch.zeros(K, N, dtype=torch.bool, device=dev)
+            self._first_local = torch.zeros(K + 2, N, 3, **f)
+            self._first_keep = torch.zeros(K + 2, N, dtype=torch.bool, device=dev)
+            self.first_local, self.first_keep = self._first_local[:K], self._first_keep[:K]
         self.slot_of = {}                                 # target id -> slot
-        self.graph = None
+        self._feed_of = {}                                # slot -> feed of the active targets (host mirror of slot_feed)
+        # The work list of the next bucket step, (2, K) as work_rows() lays it out; one host->device copy per advance.
+        self._work = torch.zeros(2, K, **i64)
+        self._buckets = None                              # the step sizes (occupancy_buckets), fixed on the first advance
+        self.graphs = {}                                  # bucket -> captured step
 
     # the feed state lives in the (possibly shared) ScanFeeds store
     scans = property(lambda self: self.scan_feeds.scans)
@@ -258,69 +308,123 @@ class MultiTargetTracker:
     def scans_seen(self, n):
         self.scan_feeds.scans_seen = n
 
-    # ------------------------------------------------------------------ one step for all slots, fixed shapes
-    def _crop(self, which, box, half, perm, pick, size, prefix=False):
+    # ------------------------------------------------------------------ one step over a bucket of rows, fixed shapes
+    def _crop(self, r, which, box, half, perm, pick, size, prefix=False):
         scans = self.scans.view(2 * self.F, self.N, 3)
         scans = scans if which is not None else scans[:, :0]
-        frame = which if which is not None else self.cur
-        pre = (self.first_local, self.first_keep) if prefix else (None, None)
-        out, _ = ops.crop_resample(scans, self.count.view(2 * self.F), frame, box.center, box.rot, half, size, self.seed, self.key, self.t, perm,
-                                   pick, *pre)
+        frame = which if which is not None else r["cur"]
+        pre = r["first"] if prefix else (None, None)
+        out, _ = ops.crop_resample(scans, self.count.view(2 * self.F), frame, box.center, box.rot, half, size, self.seed, r["key"],
+                                   r["t"], perm, pick, *pre)
         return out
 
-    def _inputs(self, box):
+    def _inputs(self, r, box):
         cfg = self.cfg
         if self.motion:
             h = _half(box, cfg.bb_scale, cfg.bb_offset)
             n = cfg.point_sample_size
-            prev_pts = self._crop(self.prev, box, h, STREAM_TEMPLATE_PERM, STREAM_TEMPLATE_PICK, n)
-            this_pts = self._crop(self.cur, box, h, STREAM_SEARCH_PERM, STREAM_SEARCH_PICK, n)
-            return motion_data(cfg, box, prev_pts, this_pts, self.first_flag)
-        search = self._crop(self.cur, box, _half(box, cfg.search_bb_scale, cfg.search_bb_offset), STREAM_SEARCH_PERM,
+            prev_pts = self._crop(r, r["prev"], box, h, STREAM_TEMPLATE_PERM, STREAM_TEMPLATE_PICK, n)
+            this_pts = self._crop(r, r["cur"], box, h, STREAM_SEARCH_PERM, STREAM_SEARCH_PICK, n)
+            return motion_data(cfg, box, prev_pts, this_pts, r["first_flag"])
+        search = self._crop(r, r["cur"], box, _half(box, cfg.search_bb_scale, cfg.search_bb_offset), STREAM_SEARCH_PERM,
                             STREAM_SEARCH_PICK, cfg.search_size)
         h = _half(box, cfg.model_bb_scale, cfg.model_bb_offset)
         if self.mode == "first":                          # the first-frame crop alone: no scan in the candidate set
-            template = self._crop(None, box, h, STREAM_TEMPLATE_PERM, STREAM_TEMPLATE_PICK, cfg.template_size, prefix=True)
+            template = self._crop(r, None, box, h, STREAM_TEMPLATE_PERM, STREAM_TEMPLATE_PICK, cfg.template_size, prefix=True)
         else:
-            template = self._crop(self.prev, box, h, STREAM_TEMPLATE_PERM, STREAM_TEMPLATE_PICK, cfg.template_size,
+            template = self._crop(r, r["prev"], box, h, STREAM_TEMPLATE_PERM, STREAM_TEMPLATE_PICK, cfg.template_size,
                                   prefix=self.mode == "firstandprevious")
         data = {"template_points": template, "search_points": search}
         if self.needs_bc:
             data["points2cc_dist_t"] = bx.point_to_box_distance(template, canonical(box))
         return data
 
-    def _step(self):
+    def _step(self, b):
+        """Advance the first `b` rows of the work list `_work`: gather their slots' state, run the network on b rows and scatter
+        the box, frame counter and first-frame flag back.  Padding rows read the idle row K, which is never active, and write
+        row K + 1.  Every intermediate is dropped when the step ends; the results live in the slot state, allocated outside any
+        capture, which is what lets the bucket graphs share one memory pool."""
         cfg = self.cfg
         with torch.no_grad(), runtime.static_weights_scope(), runtime.inference_precision_scope(self.precision):
-            fed, fcur, fprev = self.fstate
-            self.cur.copy_(self.slot_feed * 2 + fcur[self.slot_feed])
-            self.prev.copy_(self.slot_feed * 2 + fprev[self.slot_feed])
-            adv = self.active & (fed[self.slot_feed] != 0)                     # slots of a feed without a new scan hold
-            self.t.add_(adv.long())
-            ops.keyed_uniform(self.key, self.t, self.seed, STREAM_LIMIT_BOX, 2, out=self.u_lim)
-            box = bx.Box(self.box_c, self.box_s, self.box_r)
-            est = best_proposal(self.model(self._inputs(box))["estimation_boxes"])
-            new = bx.offset_box(box, est, degrees=cfg.degrees, use_z=cfg.use_z, limit_box=cfg.limit_box, rand=self.u_lim * 2 - 1)
-            a = adv[:, None]
-            self.box_c.copy_(torch.where(a, new.center, self.box_c))            # idle and holding slots keep their box
-            self.box_r.copy_(torch.where(a[..., None], new.rot, self.box_r))
-            self.first_flag.masked_fill_(adv, 0.0)
+            r, box, dst = self._gather(b)
+            u_lim = ops.keyed_uniform(r["key"], r["t"], self.seed, STREAM_LIMIT_BOX, 2)
+            est = best_proposal(self.model(self._inputs(r, box))["estimation_boxes"])
+            new = bx.offset_box(box, est, degrees=cfg.degrees, use_z=cfg.use_z, limit_box=cfg.limit_box, rand=u_lim * 2 - 1)
+            self._scatter(r, box, new, dst)
+
+    def _gather(self, b):
+        """The state of the first `b` rows of the work list: (rows {cur, prev, key, t, first_flag, adv[, first]}, box, the rows
+        to scatter to)."""
+        src, dst = self._work[0, :b], self._work[1, :b]
+        fed, fcur, fprev = self.fstate
+        feed = self._slot_feed.index_select(0, src)
+        adv = self._active.index_select(0, src) & (fed[feed] != 0)
+        r = {"cur": feed * 2 + fcur[feed], "prev": feed * 2 + fprev[feed], "key": self._key.index_select(0, src),
+             "t": self._t.index_select(0, src) + adv.long(), "first_flag": self._first_flag.index_select(0, src), "adv": adv}
+        if self.mode in ("firstandprevious", "first"):
+            r["first"] = (self._first_local.index_select(0, src), self._first_keep.index_select(0, src))
+        box = bx.Box(self._box_c.index_select(0, src), self._box_s.index_select(0, src), self._box_r.index_select(0, src))
+        return r, box, dst
+
+    def _scatter(self, r, box, new, dst):
+        """Write the advanced rows' box, frame counter and first-frame flag back to their slots (rows that hold keep theirs)."""
+        adv = r["adv"]
+        a = adv[:, None]
+        self._box_c.index_copy_(0, dst, torch.where(a, new.center, box.center))
+        self._box_r.index_copy_(0, dst, torch.where(a[..., None], new.rot, box.rot))
+        self._t.index_copy_(0, dst, r["t"])
+        self._first_flag.index_copy_(0, dst, r["first_flag"].masked_fill(adv, 0.0))
 
     def _state(self):
-        """The slot state one step advances (what the warm-up before a capture must put back)."""
-        return (self.cur, self.prev, self.t, self.box_c, self.box_r, self.first_flag, self.u_lim)
+        """The slot state a step writes (what the warm-up before a capture must put back)."""
+        return (self._t, self._box_c, self._box_r, self._first_flag)
 
-    def _capture(self):
-        self.graph = capture_step(self._step, self._state())
-
-    def _run(self):
-        """Advance the slots to the scans the feed store has just brought in: the captured step's replay, or the eager step."""
-        if not self.use_graph:
-            self._step()
+    def _plan(self):
+        """First advance: the bucket sizes, from the row counts of the network's stacks in one step over all K slots (its
+        writes are put back), then, with graphs, one captured step per bucket, largest first, all in one memory pool: only one
+        of them replays at a time and none reads memory another wrote.  Eager, one step per bucket instead.  Either way only this
+        advance synchronises."""
+        K = self.K
+        if self._buckets is None:
+            snap = [t.clone() for t in self._state()]
+            with runtime.stack_rows_scope() as rows:
+                self._step(K)
+            for t, v in zip(self._state(), snap):
+                t.copy_(v)
+            self._buckets = occupancy_buckets(K, smallest_bucket(K, rows))
+        if self.use_graph:
+            pool = torch.cuda.graph_pool_handle()
+            for b in sorted(self._buckets, reverse=True):
+                self.graphs[b] = capture_step(lambda b=b: self._step(b), self._state(), pool)
         else:
-            if self.graph is None:
-                self._capture()
-            self.graph.replay()
+            # one step at every bucket size (its writes put back), so that the prepared weight blocks of every row count are
+            # built, and synchronise, here rather than on the first advance that reaches that size
+            snap = [t.clone() for t in self._state()]
+            for b in self._buckets:
+                self._step(b)
+                for t, v in zip(self._state(), snap):
+                    t.copy_(v)
+
+    def _run(self, fed):
+        """Advance the active targets of the feeds in `fed` to the scans the feed store has just brought in: upload the work list
+        and replay the captured step of its bucket (or run the eager step at that size).  The first call fixes the buckets and
+        captures every bucket's step, so that later calls never synchronise."""
+        slots = work_slots(self._feed_of, fed)
+        first = self._buckets is None or (self.use_graph and not self.graphs)
+        if not slots and not first:
+            return
+        w = torch.from_numpy(work_rows(slots, self.K))
+        # a fresh pinned buffer for every advance: it is not rewritten before its copy runs
+        self._work.copy_(w.pin_memory() if self.dev.type == "cuda" else w, non_blocking=True)
+        if first:
+            self._plan()
+        if not slots:
+            return
+        b = bucket_for(len(slots), self._buckets)
+        if self.use_graph:
+            self.graphs[b].replay()
+        else:
+            self._step(b)
 
     # ------------------------------------------------------------------ public interface
     def _feed(self, feed):
@@ -342,8 +446,9 @@ class MultiTargetTracker:
         if self.scan_feeds.owner is not self:
             raise RuntimeError("advance(): this tracker shares scan feeds that another tracker owns; an ingest here would move "
                                "every sharing tracker's scans without advancing them, so advance the owner")
+        fed = set(self.scan_feeds.staged)
         self.scan_feeds.ingest()
-        self._run()
+        self._run(fed)
         return self.boxes()
 
     def step(self, points, n_valid=None):
@@ -387,6 +492,7 @@ class MultiTargetTracker:
         self.key[k].fill_(tid)
         self.t[k].zero_()
         self.slot_of[tid] = k
+        self._feed_of[k] = f
 
     def drop(self, target_id):
         """End target `target_id` and free its slot (it returns to the dummy box).  No host sync."""
@@ -394,6 +500,7 @@ class MultiTargetTracker:
         if tid not in self.slot_of:
             raise ValueError(f"target_id {tid} is not active")
         k = self.slot_of.pop(tid)
+        del self._feed_of[k]
         self.active[k].fill_(False)
         self.box_c[k].zero_()
         self.box_s[k].fill_(1.0)
