@@ -438,6 +438,16 @@ typedef struct {
 int o3d_scan_ingest(const o3d_scan_desc_t* desc_host, const o3d_scan_desc_t* desc, int n_desc, const void* slab, long long slab_bytes,
                     int feeds, int max_points, float* scans, long long* count, void* stream);
 
+/* In-box point counts of the live tracker's evidence (nuscenes points_in_box as the inclusive test in the box frame):
+ *   n_in[k] = #{ i < count[frame[k]] : |R[k]^T (scans[frame[k], i, :] - center[k])| <= half[k] per axis }
+ * with the box-frame coordinates in fp32, (dx R[0][j] + dy R[1][j]) + dz R[2][j], every operation rounded on its own (no FMA
+ * contraction): tracking/boxes.py box_point_counts bit for bit, so the counts equal it exactly.  n_in is zeroed inside the call
+ * (an async memset, then one launch); the per-block counts are summed with integer atomics, so the result does not depend on
+ * the order blocks run in.  No host sync; capturable.  scans [S, N, 3], count [S] int64 or NULL (all N valid), frame [K]
+ * int64, center [K, 3], rot [K, 9] row-major with the box axes in its columns, half [K, 3], n_in [K] int32.  K <= 65535. */
+int o3d_box_points(const float* scans, const long long* count, const long long* frame, const float* center, const float* rot,
+                   const float* half, int N, int K, int* n_in, void* stream);
+
 /* Block 6 — split evaluation with K tracklets in flight (tracking/batched_tracker.py).
  *
  * o3d_keyed_uniform: out [K, n] uniform [0, 1) draws of one stream.  Slot k's element e is a pure function of

@@ -62,6 +62,7 @@ PROTOTYPES = {
     "o3d_resample": [_p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p],
     "o3d_crop_resample": [_p, _p, _p, _p, _p, _p, _i, _p, _p, _i, ctypes.c_uint, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p],
     "o3d_scan_ingest": [_p, _p, _i, _p, ctypes.c_longlong, _i, _i, _p, _p, _p],
+    "o3d_box_points": [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p],
     "o3d_lift_stats": [_p, _i, _i, _p, _p, _p, _p, _p],
     "o3d_lift_scatter": [_p, _i, _i, _p, _p, _p, _i, _p, _p, _p, _p],
     "o3d_pw_fwd_tc_lift": [_p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _p, _i, _p, _p, _i, _p, _p, _p, _i, _p],

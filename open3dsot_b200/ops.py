@@ -307,6 +307,27 @@ def crop_resample(scans, count, frame, center, rot, half, size, seed, key, key_f
     return out, n
 
 
+def box_points(scans, count, frame, center, rot, half, out=None):
+    """In-box point counts (csrc/box_points.cu): scans (S, N, 3) fp32 CUDA, count (S,) int64 or None, frame (K,) int64 picks
+    each row's scan; center (K, 3), rot (K, 3, 3), half (K, 3).  Returns (K,) int32 (or writes `out`): the points i <
+    count[frame[k]] with |R^T (p - c)| <= half in every component, exactly `tracking.boxes.box_point_counts`."""
+    _chk_f(scans, "scans")
+    _, N, _ = scans.shape
+    _chk_i64(frame, "frame")
+    if count is not None:
+        _chk_i64(count, "count")
+    K = frame.shape[0]
+    center, rot, half = (t.contiguous().float() for t in (center, rot, half))
+    assert center.shape == (K, 3) and rot.shape == (K, 3, 3) and half.shape == (K, 3)
+    if out is None:
+        out = torch.empty(K, dtype=torch.int32, device=scans.device)
+    _chk_i(out, "out")
+    assert out.shape == (K,)
+    _call("o3d_box_points", scans.data_ptr(), None if count is None else count.data_ptr(), frame.data_ptr(), center.data_ptr(),
+          rot.data_ptr(), half.data_ptr(), N, K, out.data_ptr(), _stream())
+    return out
+
+
 # ------------------------------------------------------------------ scan ingest for the live tracker's feeds (csrc/scan_ingest.cu)
 # o3d_scan_desc_t, field for field
 SCAN_DESC = np.dtype([("offset", "<i8"), ("rows", "<i4"), ("stride", "<i4"), ("is_f64", "<i4"), ("feed", "<i4"), ("half", "<i4"),

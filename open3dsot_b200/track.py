@@ -17,7 +17,14 @@ Several classes: `--add_class CFG [CKPT]` (repeatable) adds a class with its own
 its tracklets, the scene plans are merged so that every scene streams once for all classes, and one `MultiClassTracker`
 (tracking/multi_class.py) advances every class in one captured step per scan.  `--max_targets` is per class (`K`, or `NAME=K`
 for one class).  Every JSON line's targets carry their "class"; Success / Precision are printed over all frames and per class,
-and a class's boxes are those of a run with its config alone at the same --max_points and --max_targets."""
+and a class's boxes are those of a run with its config alone at the same --max_points and --max_targets.
+
+Evidence and lost targets.  Every JSON line's targets carry "points", the points of that frame's scan in the box scaled by 1.25,
+and "score", the model's confidence (BAT / P2B: the best proposal's score; M2-Track: the share of the current frame's sampled
+points segmented as target); both are null on a tracklet's first frame.  `--lost MIN_POINTS PATIENCE` ends a tracklet once
+PATIENCE consecutive frames had fewer than MIN_POINTS points in its box (tracking/multi_tracker.py, decided on the device): its
+lines stop at that frame, its annotated frames after it are scored as failures (overlap 0, distance inf), and the printed
+summary counts the tracklets ended early as "lost"."""
 import argparse
 import json
 import sys
@@ -71,7 +78,17 @@ def parse_args(argv=None):
     p.add_argument('--seed', type=int, default=0, help='key of the random draws')
     p.add_argument('--precision', choices=('fp32', 'bf16'), default='fp32',
                    help='operand precision of the tensor-core layers (bf16: BF16 operands, FP32 accumulation)')
+    # without --lost the namespace has no `lost` (argparse.SUPPRESS): the options of a run without the rule are what they were
+    p.add_argument('--lost', type=int, nargs=2, metavar=('MIN_POINTS', 'PATIENCE'), default=argparse.SUPPRESS,
+                   help='end a tracklet once PATIENCE consecutive frames had fewer than MIN_POINTS scan points in its box '
+                        '(scaled by 1.25); its later annotated frames count as failures')
     args = p.parse_args(argv)
+    if hasattr(args, "lost"):
+        from .tracking.multi_tracker import check_lost_rule
+        try:
+            args.lost = check_lost_rule(args.lost)
+        except ValueError as e:
+            p.error(f"--lost: {e}")
     for extra in args.add_class or ():
         if len(extra) > 2:
             p.error(f"--add_class takes a config and at most one checkpoint, got {extra}")
@@ -184,10 +201,34 @@ def _yaw(rot, up_axis):
     return float(np.arctan2(rot[1, 0], rot[0, 0]))
 
 
-def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, precision="fp32"):
-    """Track every scene of `dataset`'s split and write `out_path`; returns {"success", "precision", "frames", "scenes"}."""
+def _evidence(ev):
+    """A target's JSON evidence: {"points", "score"}, null where the frame has none (a tracklet's first frame)."""
+    points, score = ev
+    return {"points": points if points >= 0 else None, "score": score if np.isfinite(score) else None}
+
+
+def _score_tracklet(boxes, gts, frames, dim, up):
+    """(overlaps, distances) of one tracklet: `gts` its annotated boxes on stream frames `frames`, `boxes` {frame: result box}.
+    The first frame is scored against its own ground truth; a frame with no result (after the tracklet was declared lost) is a
+    failure: overlap 0, distance inf."""
+    from .utils.metrics import estimateAccuracy, estimateOverlap
+    overlaps, distances = [], []
+    for i, (gt, t) in enumerate(zip(gts, frames)):
+        box = gt if i == 0 else boxes.get(t)
+        if box is None:
+            overlaps.append(0.0)
+            distances.append(float("inf"))
+        else:
+            overlaps.append(estimateOverlap(gt, box, dim=dim, up_axis=up))
+            distances.append(estimateAccuracy(gt, box, dim=dim, up_axis=up))
+    return overlaps, distances
+
+
+def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, precision="fp32", lost=None):
+    """Track every scene of `dataset`'s split and write `out_path`; returns {"success", "precision", "frames", "scenes"}, and
+    "lost" with a `lost` rule."""
     from .tracking.multi_tracker import track_feeds
-    from .utils.metrics import Precision, Success, estimateAccuracy, estimateOverlap
+    from .utils.metrics import Precision, Success
 
     cfg = model.config
     dim, up = cfg.IoU_space, cfg.up_axis
@@ -204,39 +245,41 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, preci
             ends[tr["index"]] = pos[tr["end"]]
         scenes.append({"frames": len(p["frames"]), "starts": starts, "ends": ends,
                        "scan": lambda t, p=p: dataset.raw_scan(p["scene"], p["frames"][t])})
-    results = track_feeds(model, scenes, max(1, min(len(scenes), max_targets)), max_targets, seed=seed, max_points=max_points,
-                          precision=precision)
+    results, evidence = track_feeds(model, scenes, max(1, min(len(scenes), max_targets)), max_targets, seed=seed,
+                                    max_points=max_points, precision=precision, lost=lost, evidence=True)
     overlaps, distances = [[] for _ in annos], [[] for _ in annos]
+    ended = 0
     with open(out_path, "w") as f:
-        for p, res in zip(plan, results):
+        for p, res, ev in zip(plan, results, evidence):
             scene, pos = p["scene"], {fr: t for t, fr in enumerate(p["frames"])}
             track_id = {tr["index"]: tr["track_id"] for tr in p["tracklets"]}
             for t, frame in enumerate(p["frames"]):
                 targets = [{"id": track_id[j], "tracklet": j, "center": b[t].center.tolist(), "wlh": b[t].wlh.tolist(),
-                            "yaw": _yaw(b[t].rotation_matrix, up)} for j, b in sorted(res.items()) if t in b]
+                            "yaw": _yaw(b[t].rotation_matrix, up), **_evidence(ev[j][t])} for j, b in sorted(res.items()) if t in b]
                 f.write(json.dumps({"scene": scene, "frame": frame, "targets": targets}) + "\n")
             for tr in p["tracklets"]:
                 j = tr["index"]
-                for i, anno in enumerate(annos[j]):
-                    gt = dataset.box_from_anno(anno)
-                    box = gt if i == 0 else res[j][pos[dataset.anno_frame(anno)[1]]]
-                    overlaps[j].append(estimateOverlap(gt, box, dim=dim, up_axis=up))
-                    distances[j].append(estimateAccuracy(gt, box, dim=dim, up_axis=up))
+                ended += max(res[j]) < pos[tr["end"]]
+                overlaps[j], distances[j] = _score_tracklet(res[j], [dataset.box_from_anno(a) for a in annos[j]],
+                                                            [pos[dataset.anno_frame(a)[1]] for a in annos[j]], dim, up)
     succ, prec = Success(), Precision()
     for j in range(len(annos)):
         succ(overlaps[j])
         prec(distances[j])
-    return {"success": succ.compute(), "precision": prec.compute(), "frames": sum(len(o) for o in overlaps), "scenes": len(plan)}
+    out = {"success": succ.compute(), "precision": prec.compute(), "frames": sum(len(o) for o in overlaps), "scenes": len(plan)}
+    if lost is not None:
+        out["lost"] = ended
+    return out
 
 
-def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0, precision="fp32"):
+def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0, precision="fp32", lost=None):
     """`run` for several classes in one pass over the scans: `models`, `datasets` and `max_targets` are {class: ...} (the class
     is its config's category_name).  Every scene streams once for all classes (class_scene_plan) through one MultiClassTracker;
     a target's draws are keyed by its tracklet's index in its class's reader, as in a one-class run.  Every JSON line's targets
     carry their "class".  Returns {"success", "precision", "frames", "scenes"} over every class's frames, and the same per class
-    under "classes"."""
+    under "classes"; with a `lost` rule (every class's), "lost" counts the tracklets it ended early, overall and per class."""
     from .tracking.multi_class import track_classes
-    from .utils.metrics import Precision, Success, estimateAccuracy, estimateOverlap
+    from .utils.metrics import Precision, Success
 
     names = list(models)
     cfg = models[names[0]].config
@@ -246,27 +289,27 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
         max_points = class_stream_max_points(datasets, plan)
     annos = {c: datasets[c].tracklet_anno_list for c in names}
     scenes = class_scenes(datasets, plan)
-    results = track_classes(models, scenes, max(1, min(len(scenes), sum(max_targets.values()))), max_targets, seed=seed,
-                            max_points=max_points, precision=precision)
+    results, evidence = track_classes(models, scenes, max(1, min(len(scenes), sum(max_targets.values()))), max_targets,
+                                      seed=seed, max_points=max_points, precision=precision, lost=lost, evidence=True)
     overlaps = {c: [[] for _ in annos[c]] for c in names}
     distances = {c: [[] for _ in annos[c]] for c in names}
+    ended = {c: 0 for c in names}
     rank = {c: i for i, c in enumerate(names)}
     with open(out_path, "w") as f:
-        for p, res in zip(plan, results):
+        for p, res, ev in zip(plan, results, evidence):
             scene, pos = p["scene"], {fr: t for t, fr in enumerate(p["frames"])}
             track_id = {(tr["class"], tr["index"]): tr["track_id"] for tr in p["tracklets"]}
             for t, frame in enumerate(p["frames"]):
                 targets = [{"class": c, "id": track_id[(c, j)], "tracklet": j, "center": b[t].center.tolist(),
-                            "wlh": b[t].wlh.tolist(), "yaw": _yaw(b[t].rotation_matrix, up)}
+                            "wlh": b[t].wlh.tolist(), "yaw": _yaw(b[t].rotation_matrix, up), **_evidence(ev[(c, j)][t])}
                            for (c, j), b in sorted(res.items(), key=lambda kv: (rank[kv[0][0]], kv[0][1])) if t in b]
                 f.write(json.dumps({"scene": scene, "frame": frame, "targets": targets}) + "\n")
             for tr in p["tracklets"]:
                 c, j = tr["class"], tr["index"]
-                for i, anno in enumerate(annos[c][j]):
-                    gt = datasets[c].box_from_anno(anno)
-                    box = gt if i == 0 else res[(c, j)][pos[datasets[c].anno_frame(anno)[1]]]
-                    overlaps[c][j].append(estimateOverlap(gt, box, dim=dim, up_axis=up))
-                    distances[c][j].append(estimateAccuracy(gt, box, dim=dim, up_axis=up))
+                ended[c] += max(res[(c, j)]) < pos[tr["end"]]
+                ds = datasets[c]
+                overlaps[c][j], distances[c][j] = _score_tracklet(res[(c, j)], [ds.box_from_anno(a) for a in annos[c][j]],
+                                                                  [pos[ds.anno_frame(a)[1]] for a in annos[c][j]], dim, up)
 
     def scores(classes):
         succ, prec = Success(), Precision()
@@ -274,7 +317,10 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
             for o, d in zip(overlaps[c], distances[c]):
                 succ(o)
                 prec(d)
-        return {"success": succ.compute(), "precision": prec.compute(), "frames": sum(len(o) for c in classes for o in overlaps[c])}
+        out = {"success": succ.compute(), "precision": prec.compute(), "frames": sum(len(o) for c in classes for o in overlaps[c])}
+        if lost is not None:
+            out["lost"] = sum(ended[c] for c in classes)
+        return out
 
     out = scores(names)
     out.update({"scenes": len(plan), "classes": {c: scores([c]) for c in names}})
@@ -309,6 +355,7 @@ def main(argv=None):
     from .trainer import load_weights
 
     args = parse_args(argv)
+    rule = {"lost": args.lost} if hasattr(args, "lost") else {}           # without --lost, run / run_classes as they always were
     classes = [(args.cfg, args.checkpoint)] + [(a[0], a[1] if len(a) > 1 else None) for a in args.add_class or ()]
     cfgs = [load_config(c) for c, _ in classes]
     check_classes(cfgs, [c for c, _ in classes])
@@ -326,11 +373,11 @@ def main(argv=None):
     if len(cfgs) == 1:
         name = cfgs[0].category_name
         out = run(models[name], data[name], args.out, max_targets=class_targets(args.max_targets, name), max_points=args.max_points,
-                  seed=args.seed, precision=args.precision)
+                  seed=args.seed, precision=args.precision, **rule)
         out.update({"checkpoint": args.checkpoint, "split": args.split, "out": args.out})
     else:
         out = run_classes(models, data, args.out, {c: class_targets(args.max_targets, c) for c in models},
-                          max_points=args.max_points, seed=args.seed, precision=args.precision)
+                          max_points=args.max_points, seed=args.seed, precision=args.precision, **rule)
         out.update({"checkpoint": [c for _, c in classes], "split": args.split, "out": args.out})
     print(json.dumps(out), flush=True)
     return out

@@ -60,6 +60,13 @@ def best_proposal(est):
     return est
 
 
+def best_proposal_score(est):
+    """(K, num_proposal, 5) proposals -> (`best_proposal`'s (K, 4) offsets, (K,) the score, column 4, of that proposal)."""
+    best = est[:, :, 4].argmax(1)
+    row = est.gather(1, best[:, None, None].expand(-1, 1, est.shape[-1]))[:, 0]
+    return row[:, :4], row[:, 4]
+
+
 def plan_schedule(lengths, slots):
     """Slot schedule of one chunk.  `lengths`: frames per tracklet, in pool order.  Tracklets are admitted longest first
     (ties in input order), each into the slot that frees first (lowest slot on ties); a tracklet of n frames holds its slot

@@ -128,6 +128,32 @@ def crop_append(scans, box: Box, scale, offset, frame, count, hist, hist_keep, h
     hist_count += keep.sum(1)
 
 
+def inclusive_half(wlh, wlh_factor=1.0):
+    """Half extents (l, w, h on x, y, z) of nuscenes points_in_box's box scaled by `wlh_factor` (its inclusive test)."""
+    return torch.stack([wlh[..., 1], wlh[..., 0], wlh[..., 2]], -1) * (wlh_factor / 2)
+
+
+def box_point_counts(scans, count, frame, center, rot, half, rows=16):
+    """The tensor formulation of `ops.box_points` (csrc/box_points.cu): for every row k, the points i < count[frame[k]] of
+    scans[frame[k]] with |R^T (p - c)| <= half[k] in every component, as (K,) int32.  scans (S, N, 3) fp32, count (S,) or None,
+    frame (K,), center (K, 3), rot (K, 3, 3), half (K, 3).  The box-frame coordinates are `to_box_frame`'s sum over the rows of R
+    in order, (d_x R[0] + d_y R[1]) + d_z R[2], one rounded fp32 operation at a time, which is what the kernel computes.  Runs
+    `rows` rows at a time, so that (rows, N, 3) is the largest intermediate."""
+    N = scans.shape[1]
+    n_valid = torch.full((scans.shape[0],), N, dtype=torch.int64, device=scans.device) if count is None else count.clamp(0, N)
+    idx = torch.arange(N, device=scans.device)
+    out = []
+    for k0 in range(0, frame.shape[0], rows):
+        f = frame[k0:k0 + rows]
+        R = rot[k0:k0 + rows, None]                                          # (r, 1, 3, 3)
+        d = scans[f] - center[k0:k0 + rows, None, :]
+        local = d[..., 0:1] * R[..., 0, :] + d[..., 1:2] * R[..., 1, :]
+        local = local + d[..., 2:3] * R[..., 2, :]
+        inside = (local.abs() <= half[k0:k0 + rows, None, :]).all(-1) & (idx[None, :] < n_valid[f][:, None])
+        out.append(inside.sum(1))
+    return torch.cat(out).to(torch.int32) if out else torch.zeros(0, dtype=torch.int32, device=scans.device)
+
+
 def point_to_box_distance(points, box: Box, wlh_factor=1.0):
     """get_point_to_box_distance (:127-144): (..., N, 9) distances to the centre and the eight corners."""
     ref = torch.cat([box.center[..., None, :], corners(box, wlh_factor)], -2)                  # (..., 9, 3)

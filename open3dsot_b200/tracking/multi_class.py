@@ -16,7 +16,7 @@ are read in (`up_axis`, `IoU_space`, `degrees`)."""
 import torch
 
 from .. import runtime
-from .multi_tracker import MultiTargetTracker, ScanFeeds, class_peaks, feed_schedule, run_scenes
+from .multi_tracker import MultiTargetTracker, ScanFeeds, check_lost_rule, class_peaks, feed_schedule, run_scenes
 
 SHARED_KEYS = ("up_axis", "IoU_space", "degrees")
 
@@ -24,10 +24,11 @@ SHARED_KEYS = ("up_axis", "IoU_space", "degrees")
 class MultiClassTracker:
     """`models` {class name: model}, `max_targets` {class name: slots}, over `feeds` scan feeds (a number, or a `ScanFeeds`
     store) of at most `max_points` points per scan.  `seed`, `use_graph` and `precision` as for MultiTargetTracker, for every
-    class.  `put` / `put_raw` / `advance()` as on MultiTargetTracker; `add(cls, id, box, feed=)` / `drop(cls, id)` start and end
-    a target of a class."""
+    class; `lost` is one end-of-track rule for every class (MultiTargetTracker's `lost=`) or {class: rule}, a class without an
+    entry never losing a target.  `put` / `put_raw` / `advance()` as on MultiTargetTracker; `add(cls, id, box, feed=)` /
+    `drop(cls, id)` start and end a target of a class."""
 
-    def __init__(self, models, max_points, max_targets, feeds=1, seed=0, use_graph=True, precision="fp32"):
+    def __init__(self, models, max_points, max_targets, feeds=1, seed=0, use_graph=True, precision="fp32", lost=None):
         if not models:
             raise ValueError("MultiClassTracker: no classes; give one model per class")
         self.precision = runtime.check_precision(precision)
@@ -38,6 +39,11 @@ class MultiClassTracker:
         for n in max_targets:
             if n not in models:
                 raise ValueError(f"max_targets: class {n!r} has no model")
+        rules = lost if isinstance(lost, dict) else {n: lost for n in names}
+        for n in rules:
+            if n not in models:
+                raise ValueError(f"lost: class {n!r} has no model")
+        rules = {n: check_lost_rule(rules.get(n)) for n in names}
         c0 = models[names[0]].config
         for n in names[1:]:
             c = models[n].config
@@ -54,7 +60,7 @@ class MultiClassTracker:
         for n in names:
             try:
                 self.trackers[n] = MultiTargetTracker(models[n], max_points, max_targets[n], seed=seed, use_graph=use_graph,
-                                                      feeds=self.scan_feeds, precision=precision)
+                                                      feeds=self.scan_feeds, precision=precision, lost=rules[n])
             except ValueError as e:
                 self.scan_feeds.owner = None
                 raise ValueError(f"class {n!r}: {e}") from None
@@ -127,6 +133,25 @@ class MultiClassTracker:
         rows of each."""
         return torch.cat([trk.snapshot() for trk in self.trackers.values()])
 
+    def evidence(self):
+        """Every class's MultiTargetTracker.evidence() rows, (sum of max_targets, 4), the rows of snapshot()."""
+        return torch.cat([trk.evidence() for trk in self.trackers.values()])
+
+    def _record(self):
+        return torch.cat([trk._record() for trk in self.trackers.values()])
+
+    def lost_targets(self):
+        """(class, id) of the active targets their class's rule has declared lost, read back from the device (one sync)."""
+        lost = torch.cat([trk.lost for trk in self.trackers.values()]).cpu().numpy()
+        return sorted(key for key, k in self.targets().items() if lost[k])
+
+    def drop_lost(self):
+        """`drop` every target of `lost_targets()`; returns their (class, id)."""
+        keys = self.lost_targets()
+        for key in keys:
+            self.drop(*key)
+        return keys
+
     def results(self):
         """{(class, target id): data_classes.Box} of the active targets, read back from the device once."""
         from ..datasets.data_classes import Box
@@ -134,11 +159,14 @@ class MultiClassTracker:
         return {key: Box(host[k, 0:3], host[k, 3:6], host[k, 6:15].reshape(3, 3)) for key, k in self.targets().items()}
 
 
-def track_classes(models, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32"):
+def track_classes(models, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32",
+                  lost=None, evidence=False):
     """`track_feeds` for several classes through one MultiClassTracker.  `models` and `max_targets`: {class: model},
     {class: slots}.  A scene's targets are named (class, id): "starts": {t: [((class, id), Box), ...]}, "ends": {(class, id):
     last t}; (class, id) is unique over all scenes.  A scene is admitted when a feed is free and every class has the scene's
-    peak of that class free.  Returns, per scene, {(class, id): {t: data_classes.Box}}."""
+    peak of that class free.  Returns, per scene, {(class, id): {t: data_classes.Box}}.  `lost`: one end-of-track rule or
+    {class: rule} (MultiClassTracker); a lost target's results end at the frame it was declared lost on.  With `evidence`, also
+    returns, per scene, {(class, id): {t: (points in the box, score)}}."""
     runtime.check_precision(precision)
     if max_points is None:
         raise ValueError("track_classes: give max_points, the largest scan of the scenes")
@@ -150,5 +178,7 @@ def track_classes(models, scenes, feeds, max_targets, seed=0, max_points=None, u
                     raise ValueError(f"scene {i}: target {key} is of class {key[0]!r}, which has no model")
     peaks = [class_peaks(lengths[i], sc["starts"], sc["ends"]) for i, sc in enumerate(scenes)]
     sched = feed_schedule(lengths, peaks, feeds, max_targets)
-    trk = MultiClassTracker(models, max_points, max_targets, feeds=feeds, seed=seed, use_graph=use_graph, precision=precision)
-    return run_scenes(trk, lambda key, box, f: trk.add(*key, box, feed=f), lambda key: trk.drop(*key), scenes, sched, chunk)
+    trk = MultiClassTracker(models, max_points, max_targets, feeds=feeds, seed=seed, use_graph=use_graph, precision=precision,
+                            lost=lost)
+    return run_scenes(trk, lambda key, box, f: trk.add(*key, box, feed=f), lambda key: trk.drop(*key), scenes, sched, chunk,
+                      evidence)

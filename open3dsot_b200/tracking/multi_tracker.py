@@ -31,6 +31,13 @@ staged scan in (host scans: one packed host->device copy and one `o3d_scan_inges
 replays the one captured step.  A feed that got no scan since the last `advance()` holds still: its slots keep their box, frame
 counter, first-frame flag and parity.  Since draws are keyed by target id and frame within the track, a target's boxes depend
 neither on its feed, nor on the other feeds, nor on F.  `step(points)` is `put(0, points)` + `advance()` for one feed.
+Evidence and lost targets.  After the box update, every advanced row also records the number of points of the scan it advanced
+on inside its new box scaled by 1.25 (`o3d_box_points`, csrc/box_points.cu) and the model's score (BAT / P2B: the best
+proposal's column 4; M2-Track: the share of the current frame's sampled points segmented as target).  With
+`lost=(min_points, patience)` the step also counts consecutive advances below `min_points` and declares the target lost at
+`patience` of them; a lost target is held from then on (its box, frame counter, first-frame flag and evidence stay those of
+that advance) until the host drops it (`lost_targets()` / `drop_lost()`).  All of it runs inside the captured step, per row, so
+it neither synchronises nor depends on the bucket, K or the other targets.
 Device memory: feeds * 2 * max_points * 12 bytes of scans, plus per slot the crop scratch and, for the first-frame template
 modes, max_points * 13 bytes of first-frame crop.  Ground-truth reference boxes (reference_BB 'previous_gt' / 'current_gt') have no meaning on a live stream, and
 shape_aggregation 'all' is not supported here; both are refused."""
@@ -42,13 +49,34 @@ import torch
 from .. import ops, runtime
 from . import boxes as bx
 from .batched_tracker import (STREAM_LIMIT_BOX, STREAM_SEARCH_PERM, STREAM_SEARCH_PICK, STREAM_TEMPLATE_PERM, STREAM_TEMPLATE_PICK,
-                              best_proposal, canonical, motion_data)
+                              best_proposal, best_proposal_score, canonical, motion_data)
 from .device_tracker import is_motion, tracking_modes
 
 
 def _half(box, scale, offset):
     """crop_in_box_frame's half extents (l, w, h on x, y, z), the same expression so that the crop test is the same."""
     return torch.stack([box.wlh[..., 1], box.wlh[..., 0], box.wlh[..., 2]], -1) * (scale / 2) + offset
+
+
+# nuscenes points_in_box's wlh_factor for the evidence's in-box count: the factor the reference's M2-Track segmentation labels use
+EVIDENCE_WLH_FACTOR = 1.25
+
+
+def check_lost_rule(lost):
+    """`lost=`: None (no target is ever declared lost) or (min_points, patience), ints with min_points >= 0, patience >= 1."""
+    if lost is None:
+        return None
+    try:
+        min_points, patience = lost
+    except (TypeError, ValueError):
+        raise ValueError(f"lost={lost!r}: expected None or (min_points, patience)") from None
+    if isinstance(min_points, bool) or isinstance(patience, bool) or int(min_points) != min_points or int(patience) != patience:
+        raise ValueError(f"lost={lost!r}: min_points and patience are integers")
+    if min_points < 0:
+        raise ValueError(f"lost: min_points={min_points} must be >= 0")
+    if patience < 1:
+        raise ValueError(f"lost: patience={patience} must be >= 1")
+    return int(min_points), int(patience)
 
 
 def _box_values(box):
@@ -234,10 +262,13 @@ class MultiTargetTracker:
     every scan of the stream; with several, `put` / `put_raw` the feeds' next scans and `advance()`.  `add(id, box, feed=)` starts
     a target on its feed's most recent scan, `drop(id)` ends it.  `feeds` is a number of feeds, or a `ScanFeeds` store the
     tracker shares with others (MultiClassTracker): only the store's owner advances (its ingest serves every tracker on the
-    store), and `_run()` advances this one tracker's slots."""
+    store), and `_run()` advances this one tracker's slots.  `lost`: None (no target is ever declared lost) or
+    (min_points, patience), the end-of-track rule the step applies on the device; `boxes()` / `evidence()` report every slot's
+    evidence either way."""
 
-    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1, precision="fp32"):
+    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1, precision="fp32", lost=None):
         self.precision = runtime.check_precision(precision)
+        self.lost_rule = check_lost_rule(lost)
         self.model = model.eval()
         self.cfg = cfg = model.config
         self.dev = dev = next(model.parameters()).device
@@ -278,8 +309,15 @@ class MultiTargetTracker:
         self._active = torch.zeros(K + 2, dtype=torch.bool, device=dev)
         self._key = torch.zeros(K + 2, **i64)             # target id of the slot (the key of its draws)
         self._t = torch.zeros(K + 2, **i64)               # frame within the target's track
+        # Evidence of the last advance: points of its scan in the box scaled by EVIDENCE_WLH_FACTOR (-1 before the first), the
+        # model's score (NaN before the first), consecutive advances below the rule's min_points, and whether the rule fired
+        self._points = torch.full((K + 2,), -1, device=dev, dtype=torch.int32)
+        self._score = torch.full((K + 2,), float("nan"), **f)
+        self._misses = torch.zeros(K + 2, device=dev, dtype=torch.int32)
+        self._lost = torch.zeros(K + 2, dtype=torch.bool, device=dev)
         self.slot_feed, self.box_c, self.box_s, self.box_r = (x[:K] for x in (self._slot_feed, self._box_c, self._box_s, self._box_r))
         self.first_flag, self.active, self.key, self.t = (x[:K] for x in (self._first_flag, self._active, self._key, self._t))
+        self.points, self.score, self.misses, self.lost = (x[:K] for x in (self._points, self._score, self._misses, self._lost))
         if self.mode in ("firstandprevious", "first"):
             self._first_local = torch.zeros(K + 2, N, 3, **f)
             self._first_keep = torch.zeros(K + 2, N, dtype=torch.bool, device=dev)
@@ -348,9 +386,19 @@ class MultiTargetTracker:
         with torch.no_grad(), runtime.static_weights_scope(), runtime.inference_precision_scope(self.precision):
             r, box, dst = self._gather(b)
             u_lim = ops.keyed_uniform(r["key"], r["t"], self.seed, STREAM_LIMIT_BOX, 2)
-            est = best_proposal(self.model(self._inputs(r, box))["estimation_boxes"])
+            out = self.model(self._inputs(r, box))
+            if self.motion:
+                est = best_proposal(out["estimation_boxes"])
+                # the share of the current frame's sampled points segmented as target (argmax: ties go to background)
+                seg = out["seg_logits"][:, :, cfg.point_sample_size:]
+                score = (seg[:, 1] > seg[:, 0]).sum(1).float() / cfg.point_sample_size
+            else:
+                est, score = best_proposal_score(out["estimation_boxes"])
             new = bx.offset_box(box, est, degrees=cfg.degrees, use_z=cfg.use_z, limit_box=cfg.limit_box, rand=u_lim * 2 - 1)
-            self._scatter(r, box, new, dst)
+            scans = self.scans.view(2 * self.F, self.N, 3)
+            points = ops.box_points(scans, self.count.view(2 * self.F), r["cur"], new.center, new.rot,
+                                    bx.inclusive_half(new.wlh, EVIDENCE_WLH_FACTOR))
+            self._scatter(r, box, new, dst, points, score)
 
     def _gather(self, b):
         """The state of the first `b` rows of the work list: (rows {cur, prev, key, t, first_flag, adv[, first]}, box, the rows
@@ -358,7 +406,8 @@ class MultiTargetTracker:
         src, dst = self._work[0, :b], self._work[1, :b]
         fed, fcur, fprev = self.fstate
         feed = self._slot_feed.index_select(0, src)
-        adv = self._active.index_select(0, src) & (fed[feed] != 0)
+        # a lost target holds from the advance it was declared lost on
+        adv = self._active.index_select(0, src) & (fed[feed] != 0) & ~self._lost.index_select(0, src)
         r = {"cur": feed * 2 + fcur[feed], "prev": feed * 2 + fprev[feed], "key": self._key.index_select(0, src),
              "t": self._t.index_select(0, src) + adv.long(), "first_flag": self._first_flag.index_select(0, src), "adv": adv}
         if self.mode in ("firstandprevious", "first"):
@@ -366,18 +415,28 @@ class MultiTargetTracker:
         box = bx.Box(self._box_c.index_select(0, src), self._box_s.index_select(0, src), self._box_r.index_select(0, src))
         return r, box, dst
 
-    def _scatter(self, r, box, new, dst):
-        """Write the advanced rows' box, frame counter and first-frame flag back to their slots (rows that hold keep theirs)."""
+    def _scatter(self, r, box, new, dst, points, score):
+        """Write the advanced rows' box, frame counter, first-frame flag and evidence back to their slots, and apply the end-of-track
+        rule to them (rows that hold keep theirs)."""
         adv = r["adv"]
         a = adv[:, None]
+        src = self._work[0, :adv.shape[0]]
         self._box_c.index_copy_(0, dst, torch.where(a, new.center, box.center))
         self._box_r.index_copy_(0, dst, torch.where(a[..., None], new.rot, box.rot))
         self._t.index_copy_(0, dst, r["t"])
         self._first_flag.index_copy_(0, dst, r["first_flag"].masked_fill(adv, 0.0))
+        self._points.index_copy_(0, dst, torch.where(adv, points, self._points.index_select(0, src)))
+        self._score.index_copy_(0, dst, torch.where(adv, score.float(), self._score.index_select(0, src)))
+        if self.lost_rule is not None:
+            min_points, patience = self.lost_rule
+            misses = self._misses.index_select(0, src)
+            misses = torch.where(adv, torch.where(points < min_points, misses + 1, torch.zeros_like(misses)), misses)
+            self._misses.index_copy_(0, dst, misses)
+            self._lost.index_copy_(0, dst, self._lost.index_select(0, src) | (misses >= patience))
 
     def _state(self):
         """The slot state a step writes (what the warm-up before a capture must put back)."""
-        return (self._t, self._box_c, self._box_r, self._first_flag)
+        return (self._t, self._box_c, self._box_r, self._first_flag, self._points, self._score, self._misses, self._lost)
 
     def _plan(self):
         """First advance: the bucket sizes, from the row counts of the network's stacks in one step over all K slots (its
@@ -491,6 +550,7 @@ class MultiTargetTracker:
         self.active[k].fill_(True)
         self.key[k].fill_(tid)
         self.t[k].zero_()
+        self._reset_evidence(k)
         self.slot_of[tid] = k
         self._feed_of[k] = f
 
@@ -508,13 +568,43 @@ class MultiTargetTracker:
         self.key[k].zero_()
         self.t[k].zero_()
         self.slot_feed[k].zero_()
+        self._reset_evidence(k)
         if self.mode in ("firstandprevious", "first"):
             self.first_keep[k].zero_()
 
+    def _reset_evidence(self, k):
+        self.points[k].fill_(-1)
+        self.score[k].fill_(float("nan"))
+        self.misses[k].zero_()
+        self.lost[k].fill_(False)
+
     def boxes(self):
-        """Device state of the slots: ids (K,) int64 (-1 for an idle slot), center (K, 3), wlh (K, 3), rot (K, 3, 3), active (K,)."""
+        """Device state of the slots: ids (K,) int64 (-1 for an idle slot), center (K, 3), wlh (K, 3), rot (K, 3, 3), active (K,),
+        and the evidence of each slot's last advance: points (K,) int32, score (K,) float32 (-1 / NaN before the first advance)
+        and lost (K,) bool."""
         return {"ids": torch.where(self.active, self.key, torch.full_like(self.key, -1)), "center": self.box_c, "wlh": self.box_s,
-                "rot": self.box_r, "active": self.active}
+                "rot": self.box_r, "active": self.active, "points": self.points, "score": self.score, "lost": self.lost}
+
+    def evidence(self):
+        """A device copy of the slots' evidence, (K, 4) float32 = points in the box, score, consecutive misses, lost (0 / 1)."""
+        return torch.stack([self.points.float(), self.score, self.misses.float(), self.lost.float()], 1)
+
+    def _record(self):
+        """`snapshot()` and `evidence()` side by side, (K, 19), in one copy."""
+        return torch.cat([self.box_c, self.box_s, self.box_r.reshape(self.K, 9), self.points.float()[:, None], self.score[:, None],
+                          self.misses.float()[:, None], self.lost.float()[:, None]], 1)
+
+    def lost_targets(self):
+        """Ids of the active targets the end-of-track rule has declared lost, read back from the device (one sync)."""
+        lost = self.lost.cpu().numpy()
+        return sorted(tid for tid, k in self.slot_of.items() if lost[k])
+
+    def drop_lost(self):
+        """`drop` every target of `lost_targets()`; returns their ids."""
+        ids = self.lost_targets()
+        for tid in ids:
+            self.drop(tid)
+        return ids
 
     def snapshot(self):
         """A device copy of the slots' boxes, (K, 15) = centre, wlh, row-major rotation; `results()` without the read-back."""
@@ -649,11 +739,14 @@ def _scene_targets(scenes):
     return scene_of, last
 
 
-def run_scenes(trk, add, drop, scenes, sched, chunk=256):
+def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
     """Drive `trk` (a MultiTargetTracker or a MultiClassTracker) through `scenes` on the feeds and steps of `sched`
     (feed_schedule); `add(tid, box, feed)` / `drop(tid)` start and end a target, `trk.targets()` maps the live targets to rows of
-    `trk.snapshot()`.  A host thread reads the next step's scans while the current step runs; the boxes are read back from the
-    device every `chunk` steps.  Returns, per scene, {id: {t: data_classes.Box}}."""
+    `trk.snapshot()`.  A host thread reads the next step's scans while the current step runs; the boxes and the evidence are read
+    back from the device together every `chunk` steps.  A target the tracker's end-of-track rule declares lost has its results
+    end at the frame it was declared lost on; its slot is still freed at its planned end, so the schedule stays what
+    `feed_schedule` planned.  Returns, per scene, {id: {t: data_classes.Box}}, and with `evidence`, per scene
+    {id: {t: (points in the box, score)}} as well."""
     from concurrent.futures import ThreadPoolExecutor
 
     from ..datasets.data_classes import Box
@@ -667,6 +760,8 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256):
         for t in range(lengths[i]):
             work[s0 + t].append((f, i, t))
     out = [{} for _ in scenes]
+    ev = [{} for _ in scenes]
+    ended = set()                                                             # targets declared lost, in a decoded step
     pending, inflight = [], []
 
     def load(step):
@@ -689,8 +784,13 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256):
         h = host.double().numpy()
         for (s, live), hs in zip(recs, h):
             for tid, k in live.items():
+                if tid in ended:
+                    continue
                 i = scene_of[tid]
                 out[i].setdefault(tid, {})[s - first[i]] = Box(hs[k, 0:3], hs[k, 3:6], hs[k, 6:15].reshape(3, 3))
+                ev[i].setdefault(tid, {})[s - first[i]] = (int(hs[k, 15]), float(hs[k, 16]))
+                if hs[k, 18] != 0:
+                    ended.add(tid)
 
     with ThreadPoolExecutor(max_workers=1) as pool:
         nxt = pool.submit(load, 0) if n_steps else None
@@ -709,7 +809,7 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256):
                     add(tid, box, f)
             live = trk.targets()
             if live:
-                pending.append((s, live, trk.snapshot()))
+                pending.append((s, live, trk._record()))
             for f, i, t, _ in items:
                 for tid in last[i].get(t, ()):
                     if tid in live:
@@ -722,22 +822,27 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256):
         read_back()
     while inflight:
         decode()
-    return out
+    return (out, ev) if evidence else out
 
 
-def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32"):
+def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32", lost=None,
+                evidence=False):
     """Track many scenes through one tracker with `feeds` scan feeds (`feed_schedule` decides which scene runs when and where).
     `scenes`: [{"frames": number of scans, "scan": t -> the scene's scan t, either (rows, transforms) for `put_raw` or an (n, 3)
     tensor / array for `put`, "starts": {t: [(id, Box), ...]}, "ends": {id: last t}}]; a target without an end runs to its scene's
     last frame, and target ids are unique over all scenes.  `max_points`: the scan buffer's size (required).
     A host thread reads the next step's scans while the current step runs; the boxes are read back from the device every
-    `chunk` steps.  Returns, per scene, {id: {t: data_classes.Box}} from the frame a target starts on to its last frame."""
+    `chunk` steps.  Returns, per scene, {id: {t: data_classes.Box}} from the frame a target starts on to its last frame.
+    `lost`: the tracker's end-of-track rule (MultiTargetTracker); a lost target's results end at the frame it was declared lost
+    on.  With `evidence`, also returns, per scene, {id: {t: (points in the box, score)}} over the same frames."""
     runtime.check_precision(precision)
+    lost = check_lost_rule(lost)
     if max_points is None:
         raise ValueError("track_feeds: give max_points, the largest scan of the scenes")
     _scene_targets(scenes)
     lengths = [int(sc["frames"]) for sc in scenes]
     peaks = [scene_peak(lengths[i], sc["starts"], sc["ends"]) for i, sc in enumerate(scenes)]
     sched = feed_schedule(lengths, peaks, feeds, max_targets)
-    trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, feeds=feeds, precision=precision)
-    return run_scenes(trk, lambda tid, box, f: trk.add(tid, box, feed=f), trk.drop, scenes, sched, chunk)
+    trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, feeds=feeds, precision=precision,
+                             lost=lost)
+    return run_scenes(trk, lambda tid, box, f: trk.add(tid, box, feed=f), trk.drop, scenes, sched, chunk, evidence)
