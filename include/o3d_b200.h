@@ -448,6 +448,51 @@ int o3d_scan_ingest(const o3d_scan_desc_t* desc_host, const o3d_scan_desc_t* des
 int o3d_box_points(const float* scans, const long long* count, const long long* frame, const float* center, const float* rot,
                    const float* half, int N, int K, int* n_in, void* stream);
 
+/* The live tracker's per-row write-back (tracking/multi_tracker.py track_update, the tensor formulation it equals bit for bit):
+ * row i < b reads its slot's state at src[i] and writes it at dst[i] (slots are distinct; padding rows read an idle row and write
+ * one nothing reads).  With adv[i] = 0 the state is copied unchanged.  With adv[i] = 1 (P = the network's box: center / rot,
+ * n = points[i], t' = t[src] + 1):
+ *   points, score <- n, score[i];  first_flag <- 0;  t <- t';  box <- P
+ *   rule:  hit = n >= min_points;  misses <- hit ? 0 : misses + 1;  lost <- lost | misses >= patience (every row)
+ *   coast (needs rule), gap = (float)(t' - hit_t):
+ *     hit:  v = (P.c - hit_c) / gap;  vel <- hit_t == 0 ? v : alpha v + beta vel;  hit_c <- P.c;  hit_t <- t'
+ *     miss: box centre <- hit_c + vel gap, rotation the previous one (vel, hit_c, hit_t hold)
+ *     coasting <- !hit && !lost
+ * Every fp32 operation is rounded on its own (no FMA contraction).  One thread per row, no atomics, no host sync, capturable.
+ * Slot state: box_c [., 3], box_r [., 9] row-major, t / hit_t int64, first_flag / score fp32, points / misses int32, lost /
+ * coasting bool (one byte), vel / hit_c [., 3].  Refused: a null descriptor or pointer, b outside 0 .. 65535, rule / coast not
+ * 0 / 1, coast without rule, min_points < 0 or patience < 1 with the rule, alpha outside (0, 1] with coast.  b = 0 launches
+ * nothing. */
+typedef struct o3d_track_update_t {
+    int b;
+    const long long* src;
+    const long long* dst;
+    const unsigned char* adv;
+    const float* center;       /* [b, 3] the network's box */
+    const float* rot;          /* [b, 9] */
+    const int* points;         /* [b] its in-box count */
+    const float* score;        /* [b] */
+    float* box_c;              /* slot state */
+    float* box_r;
+    long long* t;
+    float* first_flag;
+    int* slot_points;
+    float* slot_score;
+    int* misses;
+    unsigned char* lost;
+    float* vel;
+    float* hit_c;
+    long long* hit_t;
+    unsigned char* coasting;
+    int rule;
+    int min_points;
+    int patience;
+    int coast;
+    float alpha;
+    float beta;
+} o3d_track_update_t;
+int o3d_track_update(const o3d_track_update_t* p, void* stream);
+
 /* Block 6 — split evaluation with K tracklets in flight (tracking/batched_tracker.py).
  *
  * o3d_keyed_uniform: out [K, n] uniform [0, 1) draws of one stream.  Slot k's element e is a pure function of

@@ -63,6 +63,7 @@ PROTOTYPES = {
     "o3d_crop_resample": [_p, _p, _p, _p, _p, _p, _i, _p, _p, _i, ctypes.c_uint, _p, _p, _i, _i, _i, _i, _p, _p, _p, _p],
     "o3d_scan_ingest": [_p, _p, _i, _p, ctypes.c_longlong, _i, _i, _p, _p, _p],
     "o3d_box_points": [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p],
+    "o3d_track_update": [_p, _p],
     "o3d_lift_stats": [_p, _i, _i, _p, _p, _p, _p, _p],
     "o3d_lift_scatter": [_p, _i, _i, _p, _p, _p, _i, _p, _p, _p, _p],
     "o3d_pw_fwd_tc_lift": [_p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _p, _i, _p, _p, _i, _p, _p, _p, _i, _p],
@@ -110,6 +111,14 @@ class StackDesc(ctypes.Structure):
                 ("d_weight", _P8), ("d_bias", _P8), ("d_gamma", _P8), ("d_beta", _P8),
                 ("lift", ctypes.POINTER(LiftDesc)), ("accumulate", _i), ("prepared", _p),
                 ("precision", _i)]
+
+class TrackUpdateDesc(ctypes.Structure):
+    """ctypes mirror of `o3d_track_update_t` (include/o3d_b200.h)."""
+    _fields_ = [("b", _i)] + [(n, _p) for n in ("src", "dst", "adv", "center", "rot", "points", "score", "box_c", "box_r", "t",
+                                                "first_flag", "slot_points", "slot_score", "misses", "lost", "vel", "hit_c",
+                                                "hit_t", "coasting")] + \
+              [("rule", _i), ("min_points", _i), ("patience", _i), ("coast", _i), ("alpha", _f), ("beta", _f)]
+
 
 # o3d_stack_t.precision: 3xTF32 (default), BF16 inference (eval mode only), BF16 training (training mode only)
 PRECISION_TF32X3, PRECISION_BF16, PRECISION_BF16_TRAIN = 0, 1, 2

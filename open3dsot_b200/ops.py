@@ -3,6 +3,8 @@
 torch is used for device memory and the stream only.  Argument checks follow upstream `pointnet2_ops`
 (CHECK_CONTIGUOUS / CHECK_IS_FLOAT / CHECK_IS_INT / CHECK_CUDA -> RuntimeError; "CPU not supported").
 """
+import ctypes
+
 import numpy as np
 import torch
 
@@ -326,6 +328,40 @@ def box_points(scans, count, frame, center, rot, half, out=None):
     _call("o3d_box_points", scans.data_ptr(), None if count is None else count.data_ptr(), frame.data_ptr(), center.data_ptr(),
           rot.data_ptr(), half.data_ptr(), N, K, out.data_ptr(), _stream())
     return out
+
+
+# slot state of the live tracker's write-back: (attribute, dtype, values per row)
+TRACK_SLOTS = (("box_c", torch.float32, 3), ("box_r", torch.float32, 9), ("t", torch.int64, 1), ("first_flag", torch.float32, 1),
+               ("points", torch.int32, 1), ("score", torch.float32, 1), ("misses", torch.int32, 1), ("lost", torch.bool, 1),
+               ("vel", torch.float32, 3), ("hit_c", torch.float32, 3), ("hit_t", torch.int64, 1), ("coasting", torch.bool, 1))
+
+
+def track_update(slots, src, dst, adv, center, rot, points, score, rule=None, coast=None):
+    """The live tracker's per-row write-back in one kernel (csrc/track_update.cu), in place on `slots` (an object with the
+    TRACK_SLOTS attributes, contiguous CUDA tensors of the same number of rows): row i reads slot src[i] and writes slot dst[i].
+    adv (b,) bool; center (b, 3), rot (b, 3, 3), points (b,) int32, score (b,) float32: the network's box and its evidence.
+    `rule`: None or (min_points, patience); `coast`: None or (alpha, beta), float32 values.  Exactly
+    `tracking.multi_tracker.track_update_tensors`."""
+    b = adv.shape[0]
+    rows = slots.box_c.shape[0]
+    for name, dtype, n in TRACK_SLOTS:
+        t = getattr(slots, name)
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dtype or not t.is_contiguous() \
+                or t.shape[0] != rows or t.numel() != rows * n:
+            raise RuntimeError(f"track_update: slot state {name} must be a contiguous {dtype} CUDA tensor of {rows} x {n}")
+    _chk_i64(src, "src")
+    _chk_i64(dst, "dst")
+    _chk_f(center, "center")
+    _chk_f(rot, "rot")
+    _chk_f(score, "score")
+    _chk_i(points, "points")
+    if not adv.is_cuda or adv.dtype != torch.bool or not adv.is_contiguous():
+        raise RuntimeError("adv must be a contiguous bool CUDA tensor")
+    assert src.shape == dst.shape == points.shape == score.shape == (b,) and center.shape == (b, 3) and rot.shape == (b, 3, 3)
+    d = _lib.TrackUpdateDesc(b, src.data_ptr(), dst.data_ptr(), adv.data_ptr(), center.data_ptr(), rot.data_ptr(),
+                             points.data_ptr(), score.data_ptr(), *(getattr(slots, name).data_ptr() for name, _, _ in TRACK_SLOTS),
+                             rule is not None, *(rule or (0, 1)), coast is not None, *(coast or (1.0, 0.0)))
+    _call("o3d_track_update", ctypes.byref(d), _stream())
 
 
 # ------------------------------------------------------------------ scan ingest for the live tracker's feeds (csrc/scan_ingest.cu)

@@ -24,7 +24,10 @@ and "score", the model's confidence (BAT / P2B: the best proposal's score; M2-Tr
 points segmented as target); both are null on a tracklet's first frame.  `--lost MIN_POINTS PATIENCE` ends a tracklet once
 PATIENCE consecutive frames had fewer than MIN_POINTS points in its box (tracking/multi_tracker.py, decided on the device): its
 lines stop at that frame, its annotated frames after it are scored as failures (overlap 0, distance inf), and the printed
-summary counts the tracklets ended early as "lost"."""
+summary counts the tracklets ended early as "lost".  `--coast ALPHA` (with --lost) moves a missed target along its velocity
+instead of writing the network's box (MultiTargetTracker's `coast=`): every JSON line's targets carry "coasting", whether that
+frame's box was coasted, and the summary counts "coasted" (target-frames reported while coasting) and "reacquired" (coasting
+spells that ended in a hit).  Success / Precision score the coasted boxes."""
 import argparse
 import json
 import sys
@@ -82,6 +85,10 @@ def parse_args(argv=None):
     p.add_argument('--lost', type=int, nargs=2, metavar=('MIN_POINTS', 'PATIENCE'), default=argparse.SUPPRESS,
                    help='end a tracklet once PATIENCE consecutive frames had fewer than MIN_POINTS scan points in its box '
                         '(scaled by 1.25); its later annotated frames count as failures')
+    # likewise --coast (SUPPRESS): a run without it has no `coast`
+    p.add_argument('--coast', type=float, metavar='ALPHA', default=argparse.SUPPRESS,
+                   help='with --lost: move a target whose frame is a miss along its velocity (ALPHA, in (0, 1]: the weight of the '
+                        'newest velocity sample) instead of writing the network\'s box')
     args = p.parse_args(argv)
     if hasattr(args, "lost"):
         from .tracking.multi_tracker import check_lost_rule
@@ -89,6 +96,14 @@ def parse_args(argv=None):
             args.lost = check_lost_rule(args.lost)
         except ValueError as e:
             p.error(f"--lost: {e}")
+    if hasattr(args, "coast"):
+        if not hasattr(args, "lost"):
+            p.error("--coast needs --lost MIN_POINTS PATIENCE: the rule decides which frames are misses")
+        from .tracking.multi_tracker import check_coast
+        try:
+            args.coast = check_coast(args.coast, args.lost)
+        except ValueError as e:
+            p.error(f"--coast: {e}")
     for extra in args.add_class or ():
         if len(extra) > 2:
             p.error(f"--add_class takes a config and at most one checkpoint, got {extra}")
@@ -202,9 +217,23 @@ def _yaw(rot, up_axis):
 
 
 def _evidence(ev):
-    """A target's JSON evidence: {"points", "score"}, null where the frame has none (a tracklet's first frame)."""
-    points, score = ev
-    return {"points": points if points >= 0 else None, "score": score if np.isfinite(score) else None}
+    """A target's JSON evidence: {"points", "score"}, null where the frame has none (a tracklet's first frame), and "coasting"
+    for a coasting tracker's evidence (points, score, coasted)."""
+    points, score = ev[:2]
+    out = {"points": points if points >= 0 else None, "score": score if np.isfinite(score) else None}
+    if len(ev) > 2:
+        out["coasting"] = bool(ev[2])
+    return out
+
+
+def _coast_counts(ev, min_points):
+    """(frames reported while coasting, coasting spells that ended in a hit) of one target's evidence {t: (points, score,
+    coasted)} over consecutive frames: a spell ends in a hit when the frame after it is not coasted and has min_points points
+    (a spell can also end in the loss)."""
+    frames = sorted(ev)
+    coasted = sum(bool(ev[t][2]) for t in frames)
+    reacquired = sum(bool(ev[a][2]) and not ev[b][2] and ev[b][0] >= min_points for a, b in zip(frames, frames[1:]))
+    return coasted, reacquired
 
 
 def _score_tracklet(boxes, gts, frames, dim, up):
@@ -224,9 +253,9 @@ def _score_tracklet(boxes, gts, frames, dim, up):
     return overlaps, distances
 
 
-def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, precision="fp32", lost=None):
-    """Track every scene of `dataset`'s split and write `out_path`; returns {"success", "precision", "frames", "scenes"}, and
-    "lost" with a `lost` rule."""
+def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, precision="fp32", lost=None, coast=None):
+    """Track every scene of `dataset`'s split and write `out_path`; returns {"success", "precision", "frames", "scenes"},
+    "lost" with a `lost` rule, and "coasted" / "reacquired" with `coast`."""
     from .tracking.multi_tracker import track_feeds
     from .utils.metrics import Precision, Success
 
@@ -246,9 +275,9 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, preci
         scenes.append({"frames": len(p["frames"]), "starts": starts, "ends": ends,
                        "scan": lambda t, p=p: dataset.raw_scan(p["scene"], p["frames"][t])})
     results, evidence = track_feeds(model, scenes, max(1, min(len(scenes), max_targets)), max_targets, seed=seed,
-                                    max_points=max_points, precision=precision, lost=lost, evidence=True)
+                                    max_points=max_points, precision=precision, lost=lost, evidence=True, coast=coast)
     overlaps, distances = [[] for _ in annos], [[] for _ in annos]
-    ended = 0
+    ended, coasted, reacquired = 0, 0, 0
     with open(out_path, "w") as f:
         for p, res, ev in zip(plan, results, evidence):
             scene, pos = p["scene"], {fr: t for t, fr in enumerate(p["frames"])}
@@ -260,6 +289,9 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, preci
             for tr in p["tracklets"]:
                 j = tr["index"]
                 ended += max(res[j]) < pos[tr["end"]]
+                if coast is not None:
+                    c, r = _coast_counts(ev[j], lost[0])
+                    coasted, reacquired = coasted + c, reacquired + r
                 overlaps[j], distances[j] = _score_tracklet(res[j], [dataset.box_from_anno(a) for a in annos[j]],
                                                             [pos[dataset.anno_frame(a)[1]] for a in annos[j]], dim, up)
     succ, prec = Success(), Precision()
@@ -269,15 +301,18 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, preci
     out = {"success": succ.compute(), "precision": prec.compute(), "frames": sum(len(o) for o in overlaps), "scenes": len(plan)}
     if lost is not None:
         out["lost"] = ended
+    if coast is not None:
+        out.update(coasted=coasted, reacquired=reacquired)
     return out
 
 
-def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0, precision="fp32", lost=None):
+def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0, precision="fp32", lost=None, coast=None):
     """`run` for several classes in one pass over the scans: `models`, `datasets` and `max_targets` are {class: ...} (the class
     is its config's category_name).  Every scene streams once for all classes (class_scene_plan) through one MultiClassTracker;
     a target's draws are keyed by its tracklet's index in its class's reader, as in a one-class run.  Every JSON line's targets
     carry their "class".  Returns {"success", "precision", "frames", "scenes"} over every class's frames, and the same per class
-    under "classes"; with a `lost` rule (every class's), "lost" counts the tracklets it ended early, overall and per class."""
+    under "classes"; with a `lost` rule (every class's), "lost" counts the tracklets it ended early, overall and per class, and
+    with `coast` (every class's), so do "coasted" and "reacquired"."""
     from .tracking.multi_class import track_classes
     from .utils.metrics import Precision, Success
 
@@ -290,10 +325,12 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
     annos = {c: datasets[c].tracklet_anno_list for c in names}
     scenes = class_scenes(datasets, plan)
     results, evidence = track_classes(models, scenes, max(1, min(len(scenes), sum(max_targets.values()))), max_targets,
-                                      seed=seed, max_points=max_points, precision=precision, lost=lost, evidence=True)
+                                      seed=seed, max_points=max_points, precision=precision, lost=lost, evidence=True,
+                                      coast=coast)
     overlaps = {c: [[] for _ in annos[c]] for c in names}
     distances = {c: [[] for _ in annos[c]] for c in names}
     ended = {c: 0 for c in names}
+    coasted, reacquired = {c: 0 for c in names}, {c: 0 for c in names}
     rank = {c: i for i, c in enumerate(names)}
     with open(out_path, "w") as f:
         for p, res, ev in zip(plan, results, evidence):
@@ -307,6 +344,10 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
             for tr in p["tracklets"]:
                 c, j = tr["class"], tr["index"]
                 ended[c] += max(res[(c, j)]) < pos[tr["end"]]
+                if coast is not None:
+                    n_coasted, n_reacquired = _coast_counts(ev[(c, j)], lost[0])
+                    coasted[c] += n_coasted
+                    reacquired[c] += n_reacquired
                 ds = datasets[c]
                 overlaps[c][j], distances[c][j] = _score_tracklet(res[(c, j)], [ds.box_from_anno(a) for a in annos[c][j]],
                                                                   [pos[ds.anno_frame(a)[1]] for a in annos[c][j]], dim, up)
@@ -320,6 +361,8 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
         out = {"success": succ.compute(), "precision": prec.compute(), "frames": sum(len(o) for c in classes for o in overlaps[c])}
         if lost is not None:
             out["lost"] = sum(ended[c] for c in classes)
+        if coast is not None:
+            out.update(coasted=sum(coasted[c] for c in classes), reacquired=sum(reacquired[c] for c in classes))
         return out
 
     out = scores(names)
@@ -356,6 +399,8 @@ def main(argv=None):
 
     args = parse_args(argv)
     rule = {"lost": args.lost} if hasattr(args, "lost") else {}           # without --lost, run / run_classes as they always were
+    if hasattr(args, "coast"):
+        rule["coast"] = args.coast
     classes = [(args.cfg, args.checkpoint)] + [(a[0], a[1] if len(a) > 1 else None) for a in args.add_class or ()]
     cfgs = [load_config(c) for c, _ in classes]
     check_classes(cfgs, [c for c, _ in classes])

@@ -16,7 +16,9 @@ are read in (`up_axis`, `IoU_space`, `degrees`)."""
 import torch
 
 from .. import runtime
-from .multi_tracker import MultiTargetTracker, ScanFeeds, check_lost_rule, class_peaks, feed_schedule, run_scenes
+import numpy as np
+
+from .multi_tracker import MultiTargetTracker, ScanFeeds, check_coast, check_lost_rule, class_peaks, feed_schedule, run_scenes
 
 SHARED_KEYS = ("up_axis", "IoU_space", "degrees")
 
@@ -25,10 +27,11 @@ class MultiClassTracker:
     """`models` {class name: model}, `max_targets` {class name: slots}, over `feeds` scan feeds (a number, or a `ScanFeeds`
     store) of at most `max_points` points per scan.  `seed`, `use_graph` and `precision` as for MultiTargetTracker, for every
     class; `lost` is one end-of-track rule for every class (MultiTargetTracker's `lost=`) or {class: rule}, a class without an
-    entry never losing a target.  `put` / `put_raw` / `advance()` as on MultiTargetTracker; `add(cls, id, box, feed=)` /
-    `drop(cls, id)` start and end a target of a class."""
+    entry never losing a target; `coast` likewise one alpha (MultiTargetTracker's `coast=`) or {class: alpha}, a class without
+    an entry never coasting (a class that coasts needs a rule).  `put` / `put_raw` / `advance()` as on MultiTargetTracker;
+    `add(cls, id, box, feed=)` / `drop(cls, id)` start and end a target of a class."""
 
-    def __init__(self, models, max_points, max_targets, feeds=1, seed=0, use_graph=True, precision="fp32", lost=None):
+    def __init__(self, models, max_points, max_targets, feeds=1, seed=0, use_graph=True, precision="fp32", lost=None, coast=None):
         if not models:
             raise ValueError("MultiClassTracker: no classes; give one model per class")
         self.precision = runtime.check_precision(precision)
@@ -44,6 +47,15 @@ class MultiClassTracker:
             if n not in models:
                 raise ValueError(f"lost: class {n!r} has no model")
         rules = {n: check_lost_rule(rules.get(n)) for n in names}
+        coasts = coast if isinstance(coast, dict) else {n: coast for n in names}
+        for n in coasts:
+            if n not in models:
+                raise ValueError(f"coast: class {n!r} has no model")
+        for n in names:
+            try:
+                coasts[n] = check_coast(coasts.get(n), rules[n])
+            except ValueError as e:
+                raise ValueError(f"class {n!r}: {e}") from None
         c0 = models[names[0]].config
         for n in names[1:]:
             c = models[n].config
@@ -60,7 +72,7 @@ class MultiClassTracker:
         for n in names:
             try:
                 self.trackers[n] = MultiTargetTracker(models[n], max_points, max_targets[n], seed=seed, use_graph=use_graph,
-                                                      feeds=self.scan_feeds, precision=precision, lost=rules[n])
+                                                      feeds=self.scan_feeds, precision=precision, lost=rules[n], coast=coasts[n])
             except ValueError as e:
                 self.scan_feeds.owner = None
                 raise ValueError(f"class {n!r}: {e}") from None
@@ -140,6 +152,9 @@ class MultiClassTracker:
     def _record(self):
         return torch.cat([trk._record() for trk in self.trackers.values()])
 
+    def _coast_rows(self):
+        return np.concatenate([trk._coast_rows() for trk in self.trackers.values()])
+
     def lost_targets(self):
         """(class, id) of the active targets their class's rule has declared lost, read back from the device (one sync)."""
         lost = torch.cat([trk.lost for trk in self.trackers.values()]).cpu().numpy()
@@ -160,13 +175,14 @@ class MultiClassTracker:
 
 
 def track_classes(models, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32",
-                  lost=None, evidence=False):
+                  lost=None, evidence=False, coast=None):
     """`track_feeds` for several classes through one MultiClassTracker.  `models` and `max_targets`: {class: model},
     {class: slots}.  A scene's targets are named (class, id): "starts": {t: [((class, id), Box), ...]}, "ends": {(class, id):
     last t}; (class, id) is unique over all scenes.  A scene is admitted when a feed is free and every class has the scene's
     peak of that class free.  Returns, per scene, {(class, id): {t: data_classes.Box}}.  `lost`: one end-of-track rule or
     {class: rule} (MultiClassTracker); a lost target's results end at the frame it was declared lost on.  With `evidence`, also
-    returns, per scene, {(class, id): {t: (points in the box, score)}}."""
+    returns, per scene, {(class, id): {t: (points in the box, score)}}, with a third value, whether the frame was coasted, for
+    the classes that coast (`coast`: one alpha or {class: alpha}, MultiClassTracker)."""
     runtime.check_precision(precision)
     if max_points is None:
         raise ValueError("track_classes: give max_points, the largest scan of the scenes")
@@ -179,6 +195,6 @@ def track_classes(models, scenes, feeds, max_targets, seed=0, max_points=None, u
     peaks = [class_peaks(lengths[i], sc["starts"], sc["ends"]) for i, sc in enumerate(scenes)]
     sched = feed_schedule(lengths, peaks, feeds, max_targets)
     trk = MultiClassTracker(models, max_points, max_targets, feeds=feeds, seed=seed, use_graph=use_graph, precision=precision,
-                            lost=lost)
+                            lost=lost, coast=coast)
     return run_scenes(trk, lambda key, box, f: trk.add(*key, box, feed=f), lambda key: trk.drop(*key), scenes, sched, chunk,
                       evidence)

@@ -36,12 +36,16 @@ on inside its new box scaled by 1.25 (`o3d_box_points`, csrc/box_points.cu) and 
 proposal's column 4; M2-Track: the share of the current frame's sampled points segmented as target).  With
 `lost=(min_points, patience)` the step also counts consecutive advances below `min_points` and declares the target lost at
 `patience` of them; a lost target is held from then on (its box, frame counter, first-frame flag and evidence stay those of
-that advance) until the host drops it (`lost_targets()` / `drop_lost()`).  All of it runs inside the captured step, per row, so
-it neither synchronises nor depends on the bucket, K or the other targets.
+that advance) until the host drops it (`lost_targets()` / `drop_lost()`).  With `coast=alpha` as well, a miss writes the box
+moved along the target's velocity from its last hit instead of the network's, so the next search is centred where the target
+should be; the first hit again takes it back.  All of it runs inside the captured step, per row, so it neither synchronises nor
+depends on the bucket, K or the other targets: the whole write-back is one `o3d_track_update` launch (csrc/track_update.cu).
 Device memory: feeds * 2 * max_points * 12 bytes of scans, plus per slot the crop scratch and, for the first-frame template
 modes, max_points * 13 bytes of first-frame crop.  Ground-truth reference boxes (reference_BB 'previous_gt' / 'current_gt') have no meaning on a live stream, and
 shape_aggregation 'all' is not supported here; both are refused."""
+import math
 import weakref
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -77,6 +81,94 @@ def check_lost_rule(lost):
     if patience < 1:
         raise ValueError(f"lost: patience={patience} must be >= 1")
     return int(min_points), int(patience)
+
+
+def check_coast(coast, lost):
+    """`coast=`: None (a miss writes the network's box, as without it) or alpha in (0, 1], the weight of the newest velocity
+    sample.  Coasting needs the end-of-track rule `lost` (checked, or None), which decides what a miss is."""
+    if coast is None:
+        return None
+    if isinstance(coast, bool) or not isinstance(coast, (int, float, np.integer, np.floating)) or math.isnan(coast) \
+            or not 0 < coast <= 1:
+        raise ValueError(f"coast={coast!r}: expected None or a number alpha with 0 < alpha <= 1")
+    if lost is None:
+        raise ValueError("coast: coasting moves a target on its misses, which the end-of-track rule defines; give lost="
+                         "(min_points, patience) too")
+    return float(coast)
+
+
+def coast_weights(alpha):
+    """(alpha, beta = 1 - alpha) as the float32 values the write-back's velocity update uses, or None without coasting."""
+    return None if alpha is None else (float(np.float32(alpha)), float(np.float32(1 - alpha)))
+
+
+class Slots(NamedTuple):
+    """The per-slot state the step's write-back reads and writes (ops.TRACK_SLOTS, in its order); rows are slots."""
+    box_c: torch.Tensor        # (R, 3) float32
+    box_r: torch.Tensor        # (R, 3, 3) float32
+    t: torch.Tensor            # (R,) int64: frame within the target's track
+    first_flag: torch.Tensor   # (R,) float32
+    points: torch.Tensor       # (R,) int32
+    score: torch.Tensor        # (R,) float32
+    misses: torch.Tensor       # (R,) int32
+    lost: torch.Tensor         # (R,) bool
+    vel: torch.Tensor          # (R, 3) float32: centre displacement per advance
+    hit_c: torch.Tensor        # (R, 3) float32: centre of the last hit
+    hit_t: torch.Tensor        # (R,) int64: frame of the last hit
+    coasting: torch.Tensor     # (R,) bool
+
+
+def track_update_tensors(slots, src, dst, adv, center, rot, points, score, rule=None, coast=None):
+    """The tensor formulation of the step's per-row write-back (`ops.track_update`, csrc/track_update.cu), in place on `slots`:
+    row i reads slot src[i] and writes slot dst[i].  adv (b,) bool: the row advanced; center (b, 3) / rot (b, 3, 3): the
+    network's box P; points (b,) int32 / score (b,) float32: its evidence.  A row that does not advance keeps its state.  An
+    advanced row takes P's evidence, t + 1 and first_flag 0, and with `rule` = (min_points, patience) counts a miss (points <
+    min_points) or resets the count on a hit; lost |= misses >= patience.  Its box is P, except with `coast` = (alpha, beta)
+    (float32 values) on a miss: then the centre is hit_c + vel * (t' - hit_t) and the rotation the previous one.  A hit with
+    `coast` updates vel (the first sample, hit_t == 0, as is; then alpha * v + beta * vel with v = (P.c - hit_c) / (t' - hit_t))
+    and moves hit_c / hit_t to P.c / t'; coasting = miss and not lost.  Every fp32 operation is one rounded operation."""
+    g = lambda x: x.index_select(0, src)
+    a = adv[:, None]
+    t = g(slots.t) + adv.long()
+    old_c, old_r = g(slots.box_c), g(slots.box_r)
+    misses, lost = g(slots.misses), g(slots.lost)
+    vel, hit_c, hit_t, coasting = g(slots.vel), g(slots.hit_c), g(slots.hit_t), g(slots.coasting)
+    if rule is not None:
+        min_points, patience = rule
+        hit = points >= min_points
+        misses = torch.where(adv, torch.where(hit, torch.zeros_like(misses), misses + 1), misses)
+        lost = lost | (misses >= patience)
+        if coast is not None:
+            alpha, beta = coast                           # float32 values: a float32 tensor times either is one fp32 multiply
+            gap = (t - hit_t).float()[:, None]
+            v = (center - hit_c) / gap
+            v = torch.where((hit_t == 0)[:, None], v, alpha * v + beta * vel)
+            coasted = hit_c + vel * gap
+            center = torch.where(hit[:, None], center, coasted)
+            rot = torch.where(hit[:, None, None], rot, old_r)
+            h = adv & hit
+            vel = torch.where(h[:, None], v, vel)
+            hit_c = torch.where(h[:, None], center, hit_c)
+            hit_t = torch.where(h, t, hit_t)
+            coasting = torch.where(adv, ~hit & ~lost, coasting)
+    slots.box_c.index_copy_(0, dst, torch.where(a, center, old_c))
+    slots.box_r.index_copy_(0, dst, torch.where(a[..., None], rot, old_r))
+    slots.t.index_copy_(0, dst, t)
+    slots.first_flag.index_copy_(0, dst, g(slots.first_flag).masked_fill(adv, 0.0))
+    slots.points.index_copy_(0, dst, torch.where(adv, points, g(slots.points)))
+    slots.score.index_copy_(0, dst, torch.where(adv, score.float(), g(slots.score)))
+    for name, v in (("misses", misses), ("lost", lost), ("vel", vel), ("hit_c", hit_c), ("hit_t", hit_t), ("coasting", coasting)):
+        getattr(slots, name).index_copy_(0, dst, v)
+
+
+def track_update(slots, src, dst, adv, center, rot, points, score, rule=None, coast=None):
+    """The step's per-row write-back (`track_update_tensors`): CUDA slot state through one `o3d_track_update` launch
+    (csrc/track_update.cu), other tensors through the tensor formulation."""
+    if slots.box_c.is_cuda:
+        ops.track_update(slots, src, dst, adv, center.contiguous(), rot.contiguous(), points, score.float().contiguous(), rule,
+                         coast)
+    else:
+        track_update_tensors(slots, src, dst, adv, center, rot, points, score, rule, coast)
 
 
 def _box_values(box):
@@ -264,11 +356,14 @@ class MultiTargetTracker:
     tracker shares with others (MultiClassTracker): only the store's owner advances (its ingest serves every tracker on the
     store), and `_run()` advances this one tracker's slots.  `lost`: None (no target is ever declared lost) or
     (min_points, patience), the end-of-track rule the step applies on the device; `boxes()` / `evidence()` report every slot's
-    evidence either way."""
+    evidence either way.  `coast`: None or alpha in (0, 1] (needs `lost`): a miss moves the box along the target's velocity, the
+    alpha-weighted average of its centre's displacement per advance between hits, instead of writing the network's box."""
 
-    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1, precision="fp32", lost=None):
+    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1, precision="fp32", lost=None, coast=None):
         self.precision = runtime.check_precision(precision)
         self.lost_rule = check_lost_rule(lost)
+        self.coast = check_coast(coast, self.lost_rule)
+        self._coast = coast_weights(self.coast)
         self.model = model.eval()
         self.cfg = cfg = model.config
         self.dev = dev = next(model.parameters()).device
@@ -318,6 +413,15 @@ class MultiTargetTracker:
         self.slot_feed, self.box_c, self.box_s, self.box_r = (x[:K] for x in (self._slot_feed, self._box_c, self._box_s, self._box_r))
         self.first_flag, self.active, self.key, self.t = (x[:K] for x in (self._first_flag, self._active, self._key, self._t))
         self.points, self.score, self.misses, self.lost = (x[:K] for x in (self._points, self._score, self._misses, self._lost))
+        # Coasting (coast=): the velocity (centre displacement per advance), the centre and frame of the last hit, and whether the
+        # last advance coasted
+        self._vel = torch.zeros(K + 2, 3, **f)
+        self._hit_c = torch.zeros(K + 2, 3, **f)
+        self._hit_t = torch.zeros(K + 2, **i64)
+        self._coasting = torch.zeros(K + 2, dtype=torch.bool, device=dev)
+        self.vel, self.hit_c, self.hit_t, self.coasting = (x[:K] for x in (self._vel, self._hit_c, self._hit_t, self._coasting))
+        self._slots = Slots(self._box_c, self._box_r, self._t, self._first_flag, self._points, self._score, self._misses, self._lost,
+                            self._vel, self._hit_c, self._hit_t, self._coasting)
         if self.mode in ("firstandprevious", "first"):
             self._first_local = torch.zeros(K + 2, N, 3, **f)
             self._first_keep = torch.zeros(K + 2, N, dtype=torch.bool, device=dev)
@@ -378,8 +482,8 @@ class MultiTargetTracker:
         return data
 
     def _step(self, b):
-        """Advance the first `b` rows of the work list `_work`: gather their slots' state, run the network on b rows and scatter
-        the box, frame counter and first-frame flag back.  Padding rows read the idle row K, which is never active, and write
+        """Advance the first `b` rows of the work list `_work`: gather their slots' state, run the network on b rows and write
+        the box, frame counter, first-frame flag, evidence and coast state back (`track_update`).  Padding rows read the idle row K, which is never active, and write
         row K + 1.  Every intermediate is dropped when the step ends; the results live in the slot state, allocated outside any
         capture, which is what lets the bucket graphs share one memory pool."""
         cfg = self.cfg
@@ -398,7 +502,8 @@ class MultiTargetTracker:
             scans = self.scans.view(2 * self.F, self.N, 3)
             points = ops.box_points(scans, self.count.view(2 * self.F), r["cur"], new.center, new.rot,
                                     bx.inclusive_half(new.wlh, EVIDENCE_WLH_FACTOR))
-            self._scatter(r, box, new, dst, points, score)
+            track_update(self._slots, self._work[0, :b], dst, r["adv"], new.center, new.rot, points, score, self.lost_rule,
+                         self._coast)
 
     def _gather(self, b):
         """The state of the first `b` rows of the work list: (rows {cur, prev, key, t, first_flag, adv[, first]}, box, the rows
@@ -415,28 +520,9 @@ class MultiTargetTracker:
         box = bx.Box(self._box_c.index_select(0, src), self._box_s.index_select(0, src), self._box_r.index_select(0, src))
         return r, box, dst
 
-    def _scatter(self, r, box, new, dst, points, score):
-        """Write the advanced rows' box, frame counter, first-frame flag and evidence back to their slots, and apply the end-of-track
-        rule to them (rows that hold keep theirs)."""
-        adv = r["adv"]
-        a = adv[:, None]
-        src = self._work[0, :adv.shape[0]]
-        self._box_c.index_copy_(0, dst, torch.where(a, new.center, box.center))
-        self._box_r.index_copy_(0, dst, torch.where(a[..., None], new.rot, box.rot))
-        self._t.index_copy_(0, dst, r["t"])
-        self._first_flag.index_copy_(0, dst, r["first_flag"].masked_fill(adv, 0.0))
-        self._points.index_copy_(0, dst, torch.where(adv, points, self._points.index_select(0, src)))
-        self._score.index_copy_(0, dst, torch.where(adv, score.float(), self._score.index_select(0, src)))
-        if self.lost_rule is not None:
-            min_points, patience = self.lost_rule
-            misses = self._misses.index_select(0, src)
-            misses = torch.where(adv, torch.where(points < min_points, misses + 1, torch.zeros_like(misses)), misses)
-            self._misses.index_copy_(0, dst, misses)
-            self._lost.index_copy_(0, dst, self._lost.index_select(0, src) | (misses >= patience))
-
     def _state(self):
         """The slot state a step writes (what the warm-up before a capture must put back)."""
-        return (self._t, self._box_c, self._box_r, self._first_flag, self._points, self._score, self._misses, self._lost)
+        return tuple(self._slots)
 
     def _plan(self):
         """First advance: the bucket sizes, from the row counts of the network's stacks in one step over all K slots (its
@@ -551,6 +637,7 @@ class MultiTargetTracker:
         self.key[k].fill_(tid)
         self.t[k].zero_()
         self._reset_evidence(k)
+        self.hit_c[k].copy_(self.box_c[k])
         self.slot_of[tid] = k
         self._feed_of[k] = f
 
@@ -577,13 +664,20 @@ class MultiTargetTracker:
         self.score[k].fill_(float("nan"))
         self.misses[k].zero_()
         self.lost[k].fill_(False)
+        self.vel[k].zero_()
+        self.hit_c[k].zero_()
+        self.hit_t[k].zero_()
+        self.coasting[k].fill_(False)
 
     def boxes(self):
         """Device state of the slots: ids (K,) int64 (-1 for an idle slot), center (K, 3), wlh (K, 3), rot (K, 3, 3), active (K,),
         and the evidence of each slot's last advance: points (K,) int32, score (K,) float32 (-1 / NaN before the first advance)
-        and lost (K,) bool."""
+        and lost (K,) bool.  points and score are those of the network's box on every advance, also when the box reported is a
+        coasted one (`coast=`): they describe the proposal that decided the miss.  coasting (K,) bool: the last advance was a
+        miss that moved the box along velocity (K, 3), the centre's displacement per advance (both views of the slot state)."""
         return {"ids": torch.where(self.active, self.key, torch.full_like(self.key, -1)), "center": self.box_c, "wlh": self.box_s,
-                "rot": self.box_r, "active": self.active, "points": self.points, "score": self.score, "lost": self.lost}
+                "rot": self.box_r, "active": self.active, "points": self.points, "score": self.score, "lost": self.lost,
+                "coasting": self.coasting, "velocity": self.vel}
 
     def evidence(self):
         """A device copy of the slots' evidence, (K, 4) float32 = points in the box, score, consecutive misses, lost (0 / 1)."""
@@ -605,6 +699,10 @@ class MultiTargetTracker:
         for tid in ids:
             self.drop(tid)
         return ids
+
+    def _coast_rows(self):
+        """Host flags over the rows of snapshot(): the row's tracker coasts (coast=)."""
+        return np.full(self.K, self.coast is not None)
 
     def snapshot(self):
         """A device copy of the slots' boxes, (K, 15) = centre, wlh, row-major rotation; `results()` without the read-back."""
@@ -746,11 +844,14 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
     back from the device together every `chunk` steps.  A target the tracker's end-of-track rule declares lost has its results
     end at the frame it was declared lost on; its slot is still freed at its planned end, so the schedule stays what
     `feed_schedule` planned.  Returns, per scene, {id: {t: data_classes.Box}}, and with `evidence`, per scene
-    {id: {t: (points in the box, score)}} as well."""
+    {id: {t: (points in the box, score)}} as well; a target of a coasting tracker (coast=) has (points, score, coasted) instead,
+    coasted being whether that frame's box was coasted ((misses > 0) & ~lost: a coasting tracker's misses count is reset by
+    every hit)."""
     from concurrent.futures import ThreadPoolExecutor
 
     from ..datasets.data_classes import Box
     scene_of, last = _scene_targets(scenes)
+    coasts = trk._coast_rows()
     lengths = [int(sc["frames"]) for sc in scenes]
     n_steps = max((s0 + lengths[i] for i, _, s0 in sched), default=0)
     work = [[] for _ in range(n_steps)]                                        # per step: (feed, scene, frame)
@@ -788,7 +889,8 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
                     continue
                 i = scene_of[tid]
                 out[i].setdefault(tid, {})[s - first[i]] = Box(hs[k, 0:3], hs[k, 3:6], hs[k, 6:15].reshape(3, 3))
-                ev[i].setdefault(tid, {})[s - first[i]] = (int(hs[k, 15]), float(hs[k, 16]))
+                e = (int(hs[k, 15]), float(hs[k, 16]))
+                ev[i].setdefault(tid, {})[s - first[i]] = e + (bool(hs[k, 17] > 0 and hs[k, 18] == 0),) if coasts[k] else e
                 if hs[k, 18] != 0:
                     ended.add(tid)
 
@@ -826,7 +928,7 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
 
 
 def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32", lost=None,
-                evidence=False):
+                evidence=False, coast=None):
     """Track many scenes through one tracker with `feeds` scan feeds (`feed_schedule` decides which scene runs when and where).
     `scenes`: [{"frames": number of scans, "scan": t -> the scene's scan t, either (rows, transforms) for `put_raw` or an (n, 3)
     tensor / array for `put`, "starts": {t: [(id, Box), ...]}, "ends": {id: last t}}]; a target without an end runs to its scene's
@@ -834,9 +936,12 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
     A host thread reads the next step's scans while the current step runs; the boxes are read back from the device every
     `chunk` steps.  Returns, per scene, {id: {t: data_classes.Box}} from the frame a target starts on to its last frame.
     `lost`: the tracker's end-of-track rule (MultiTargetTracker); a lost target's results end at the frame it was declared lost
-    on.  With `evidence`, also returns, per scene, {id: {t: (points in the box, score)}} over the same frames."""
+    on.  With `evidence`, also returns, per scene, {id: {t: (points in the box, score)}} over the same frames.  `coast`: the
+    tracker's coasting (MultiTargetTracker); results run on through coasted frames, and the evidence also says whether each frame
+    was coasted (run_scenes)."""
     runtime.check_precision(precision)
     lost = check_lost_rule(lost)
+    coast = check_coast(coast, lost)
     if max_points is None:
         raise ValueError("track_feeds: give max_points, the largest scan of the scenes")
     _scene_targets(scenes)
@@ -844,5 +949,5 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
     peaks = [scene_peak(lengths[i], sc["starts"], sc["ends"]) for i, sc in enumerate(scenes)]
     sched = feed_schedule(lengths, peaks, feeds, max_targets)
     trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, feeds=feeds, precision=precision,
-                             lost=lost)
+                             lost=lost, coast=coast)
     return run_scenes(trk, lambda tid, box, f: trk.add(tid, box, feed=f), trk.drop, scenes, sched, chunk, evidence)
