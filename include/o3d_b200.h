@@ -458,11 +458,16 @@ int o3d_box_points(const float* scans, const long long* count, const long long* 
  *     hit:  v = (P.c - hit_c) / gap;  vel <- hit_t == 0 ? v : alpha v + beta vel;  hit_c <- P.c;  hit_t <- t'
  *     miss: box centre <- hit_c + vel gap, rotation the previous one (vel, hit_c, hit_t hold)
  *     coasting <- !hit && !lost
+ * Detection matches (optional; all four fields null = none, the behaviour above): match [b] int32, the row's detection from
+ * o3d_box_associate (-1: none), match_box [b, 12] its centre and row-major rotation.  An advanced row takes detection <- match[i]
+ * and reacquired <- (match[i] >= 0 and a miss under the rule); a re-acquired row is handled as a hit whose box is the detection's
+ * centre and rotation (the slot keeps its wlh): misses <- 0, and with coast the velocity sample, hit_c / hit_t and coasting
+ * follow the hit rules with P.c = the detection's centre.  A matched hit writes P as without matches.
  * Every fp32 operation is rounded on its own (no FMA contraction).  One thread per row, no atomics, no host sync, capturable.
- * Slot state: box_c [., 3], box_r [., 9] row-major, t / hit_t int64, first_flag / score fp32, points / misses int32, lost /
- * coasting bool (one byte), vel / hit_c [., 3].  Refused: a null descriptor or pointer, b outside 0 .. 65535, rule / coast not
- * 0 / 1, coast without rule, min_points < 0 or patience < 1 with the rule, alpha outside (0, 1] with coast.  b = 0 launches
- * nothing. */
+ * Slot state: box_c [., 3], box_r [., 9] row-major, t / hit_t int64, first_flag / score fp32, points / misses / detection int32,
+ * lost / coasting / reacquired bool (one byte), vel / hit_c [., 3].  Refused: a null descriptor or pointer (the match fields:
+ * some but not all null), b outside 0 .. 65535, rule / coast not 0 / 1, coast without rule, min_points < 0 or patience < 1 with
+ * the rule, alpha outside (0, 1] with coast.  b = 0 launches nothing. */
 typedef struct o3d_track_update_t {
     int b;
     const long long* src;
@@ -490,8 +495,56 @@ typedef struct o3d_track_update_t {
     int coast;
     float alpha;
     float beta;
+    const int* match;          /* [b] o3d_box_associate's match, or NULL (no detections) */
+    const float* match_box;    /* [b, 12] */
+    int* slot_detection;       /* slot state: the last advance's detection index, -1 for none */
+    unsigned char* slot_reacquired;
 } o3d_track_update_t;
 int o3d_track_update(const o3d_track_update_t* p, void* stream);
+
+/* Detection matching of the live tracker (tracking/multi_tracker.py associate_tensors, which it equals exactly), one CTA per
+ * feed, run before o3d_track_update in the same step.  Row i < b of the step belongs to feed[i] and takes part when adv[i]; it
+ * is matched against the centre it would write without detections, pred (o3d_track_update's arithmetic, csrc/track_predict.cuh):
+ * P = center[i] on a hit or without the rule (hit = points[i] >= min_points), and with coast on a miss hit_c + vel * gap with
+ * gap = (float)(t[src[i]] + 1 - hit_t[src[i]]) from the slot state at src[i].  Feed f's detections this advance are
+ * det[f, d, :] for d < count[f] when fed[f] != 0 (none otherwise); a row is 16 floats: centre (3), wlh (3), row-major rotation
+ * with the box axes in its columns (9), score.  Distance: d2 = dx*dx + dy*dy over the plane axes axis0 / axis1, each operation
+ * rounded on its own; a pair is a candidate when d2 <= gate2.  Per feed, the candidates are taken greedily in ascending
+ * (d2, row, detection) order, a pair accepted when its row and its detection are both still free; score plays no part.
+ * Writes, for every row: pred [b, 3] (NaN for a row that does not take part), match [b] int32 (the detection, -1 for none),
+ * match_box [b, 12] (the matched detection's centre and rotation; zeros without a match).  For every fed feed and d < count[f]:
+ * rec_det[f, d] <- det[f, d], rec_slot[f, d] <- src of the row detection d matched, or -1; rec_count[f] <- count[f].  Rows
+ * d >= count[f] and the records of a feed that is not fed are left as they are.  count is read on the device: the caller checks 0 <= count[f] <= D before it
+ * uploads it.  No atomics, no host sync, capturable.  Refused: a null descriptor or pointer, b outside 0 .. 65535, F < 1, D
+ * outside 1 .. 1024, gate2 not finite or <= 0, axis0 / axis1 not distinct values in {0, 1, 2}, rule / coast not 0 / 1, coast
+ * without rule, min_points < 0 with the rule.  b = 0 launches nothing. */
+typedef struct o3d_box_associate_t {
+    int b;                     /* rows of the step */
+    int F;                     /* feeds */
+    int D;                     /* detections per feed, at most (the row stride of det / rec_det / rec_slot) */
+    int axis0, axis1;          /* the plane the distance is measured in */
+    float gate2;               /* squared gate, float32 */
+    int rule, min_points, coast;
+    const long long* src;      /* [b] slot of each row */
+    const long long* feed;     /* [b] feed of each row */
+    const unsigned char* adv;  /* [b] */
+    const float* center;       /* [b, 3] the network's box */
+    const int* points;         /* [b] its in-box count */
+    const long long* t;        /* slot state (read at src[i]): frame counter before this advance */
+    const long long* hit_t;
+    const float* hit_c;        /* [., 3] */
+    const float* vel;          /* [., 3] */
+    const long long* fed;      /* [F] the feed got a scan this advance */
+    const int* count;          /* [F] detections of the feed this advance */
+    const float* det;          /* [F, D, 16] */
+    float* pred;               /* [b, 3] out */
+    int* match;                /* [b] out */
+    float* match_box;          /* [b, 12] out */
+    float* rec_det;            /* [F, D, 16] per-feed records */
+    int* rec_count;            /* [F] */
+    int* rec_slot;             /* [F, D] */
+} o3d_box_associate_t;
+int o3d_box_associate(const o3d_box_associate_t* p, void* stream);
 
 /* Block 6 — split evaluation with K tracklets in flight (tracking/batched_tracker.py).
  *

@@ -64,6 +64,7 @@ PROTOTYPES = {
     "o3d_scan_ingest": [_p, _p, _i, _p, ctypes.c_longlong, _i, _i, _p, _p, _p],
     "o3d_box_points": [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p],
     "o3d_track_update": [_p, _p],
+    "o3d_box_associate": [_p, _p],
     "o3d_lift_stats": [_p, _i, _i, _p, _p, _p, _p, _p],
     "o3d_lift_scatter": [_p, _i, _i, _p, _p, _p, _i, _p, _p, _p, _p],
     "o3d_pw_fwd_tc_lift": [_p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _p, _i, _p, _p, _i, _p, _p, _p, _i, _p],
@@ -117,7 +118,16 @@ class TrackUpdateDesc(ctypes.Structure):
     _fields_ = [("b", _i)] + [(n, _p) for n in ("src", "dst", "adv", "center", "rot", "points", "score", "box_c", "box_r", "t",
                                                 "first_flag", "slot_points", "slot_score", "misses", "lost", "vel", "hit_c",
                                                 "hit_t", "coasting")] + \
-              [("rule", _i), ("min_points", _i), ("patience", _i), ("coast", _i), ("alpha", _f), ("beta", _f)]
+              [("rule", _i), ("min_points", _i), ("patience", _i), ("coast", _i), ("alpha", _f), ("beta", _f)] + \
+              [(n, _p) for n in ("match", "match_box", "slot_detection", "slot_reacquired")]
+
+
+class AssociateDesc(ctypes.Structure):
+    """ctypes mirror of `o3d_box_associate_t` (include/o3d_b200.h)."""
+    _fields_ = [(n, _i) for n in ("b", "F", "D", "axis0", "axis1")] + [("gate2", _f)] + \
+               [(n, _i) for n in ("rule", "min_points", "coast")] + \
+               [(n, _p) for n in ("src", "feed", "adv", "center", "points", "t", "hit_t", "hit_c", "vel", "fed", "count", "det",
+                                  "pred", "match", "match_box", "rec_det", "rec_count", "rec_slot")]
 
 
 # o3d_stack_t.precision: 3xTF32 (default), BF16 inference (eval mode only), BF16 training (training mode only)

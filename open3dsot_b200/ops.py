@@ -336,12 +336,13 @@ TRACK_SLOTS = (("box_c", torch.float32, 3), ("box_r", torch.float32, 9), ("t", t
                ("vel", torch.float32, 3), ("hit_c", torch.float32, 3), ("hit_t", torch.int64, 1), ("coasting", torch.bool, 1))
 
 
-def track_update(slots, src, dst, adv, center, rot, points, score, rule=None, coast=None):
+def track_update(slots, src, dst, adv, center, rot, points, score, rule=None, coast=None, match=None):
     """The live tracker's per-row write-back in one kernel (csrc/track_update.cu), in place on `slots` (an object with the
     TRACK_SLOTS attributes, contiguous CUDA tensors of the same number of rows): row i reads slot src[i] and writes slot dst[i].
     adv (b,) bool; center (b, 3), rot (b, 3, 3), points (b,) int32, score (b,) float32: the network's box and its evidence.
-    `rule`: None or (min_points, patience); `coast`: None or (alpha, beta), float32 values.  Exactly
-    `tracking.multi_tracker.track_update_tensors`."""
+    `rule`: None or (min_points, patience); `coast`: None or (alpha, beta), float32 values.  `match`: None or (match (b,) int32,
+    match_box (b, 12) float32 from `box_associate`, detection and reacquired: the slot state of MATCH_SLOTS, with the rows of
+    `slots`).  Exactly `tracking.multi_tracker.track_update_tensors`."""
     b = adv.shape[0]
     rows = slots.box_c.shape[0]
     for name, dtype, n in TRACK_SLOTS:
@@ -358,10 +359,67 @@ def track_update(slots, src, dst, adv, center, rot, points, score, rule=None, co
     if not adv.is_cuda or adv.dtype != torch.bool or not adv.is_contiguous():
         raise RuntimeError("adv must be a contiguous bool CUDA tensor")
     assert src.shape == dst.shape == points.shape == score.shape == (b,) and center.shape == (b, 3) and rot.shape == (b, 3, 3)
+    ptrs = [None] * 4
+    if match is not None:
+        m, m_box, detection, reacquired = match
+        _chk_i(m, "match")
+        _chk_f(m_box, "match_box")
+        assert m.shape == (b,) and m_box.shape == (b, 12)
+        for t, (name, dtype) in zip((detection, reacquired), MATCH_SLOTS):
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dtype or not t.is_contiguous() or t.shape != (rows,):
+                raise RuntimeError(f"track_update: slot state {name} must be a contiguous {dtype} CUDA tensor of {rows}")
+        ptrs = [t.data_ptr() for t in (m, m_box, detection, reacquired)]
     d = _lib.TrackUpdateDesc(b, src.data_ptr(), dst.data_ptr(), adv.data_ptr(), center.data_ptr(), rot.data_ptr(),
                              points.data_ptr(), score.data_ptr(), *(getattr(slots, name).data_ptr() for name, _, _ in TRACK_SLOTS),
-                             rule is not None, *(rule or (0, 1)), coast is not None, *(coast or (1.0, 0.0)))
+                             rule is not None, *(rule or (0, 1)), coast is not None, *(coast or (1.0, 0.0)), *ptrs)
     _call("o3d_track_update", ctypes.byref(d), _stream())
+
+
+# the write-back's detection state per slot: (attribute, dtype)
+MATCH_SLOTS = (("detection", torch.int32), ("reacquired", torch.bool))
+# values of one detection row: centre (3), wlh (3), row-major rotation with the box axes in its columns (9), score
+DETECTION_VALUES = 16
+MAX_DETECTIONS = 1024
+
+
+def box_associate(src, feed, adv, center, points, slots, fed, count, det, records, gate2, axes, rule=None, coast=False):
+    """Match each feed's detections to the step's advancing rows (csrc/associate.cu, one CTA per feed): greedy in ascending
+    (d2, row, detection) order over the pairs with d2 <= gate2, d2 the squared distance over the plane `axes` between the
+    detection's centre and the centre the row writes without detections (`coast`: whether a miss coasts).  src / feed (b,) int64,
+    adv (b,) bool, center (b, 3) / points (b,) int32: the network's box and its in-box count; `slots`: the slot state (t, hit_t,
+    hit_c, vel attributes); fed (F,) int64, count (F,) int32 (checked on the host before its upload: 0 .. D), det (F, D, 16)
+    float32; `records`: (rec_det (F, D, 16), rec_count (F,) int32, rec_slot (F, D) int32), updated for the fed feeds.  `gate2`: a
+    float32 value; `rule`: None or (min_points, patience).  Returns (pred (b, 3), match (b,) int32, match_box (b, 12)), exactly
+    `tracking.multi_tracker.associate_tensors`."""
+    b = adv.shape[0]
+    _chk_i64(src, "src")
+    _chk_i64(feed, "feed")
+    _chk_i64(fed, "fed")
+    _chk_f(center, "center")
+    _chk_i(points, "points")
+    _chk_i(count, "count")
+    _chk_f(det, "det")
+    if not adv.is_cuda or adv.dtype != torch.bool or not adv.is_contiguous():
+        raise RuntimeError("adv must be a contiguous bool CUDA tensor")
+    F, D, n = det.shape
+    assert n == DETECTION_VALUES and src.shape == feed.shape == points.shape == (b,) and center.shape == (b, 3)
+    assert fed.shape == count.shape == (F,)
+    rec_det, rec_count, rec_slot = records
+    _chk_f(rec_det, "rec_det")
+    _chk_i(rec_count, "rec_count")
+    _chk_i(rec_slot, "rec_slot")
+    assert rec_det.shape == (F, D, n) and rec_count.shape == (F,) and rec_slot.shape == (F, D)
+    for name, chk in (("t", _chk_i64), ("hit_t", _chk_i64), ("hit_c", _chk_f), ("vel", _chk_f)):
+        chk(getattr(slots, name), name)
+    dev = adv.device
+    pred = torch.empty(b, 3, device=dev)
+    match = torch.empty(b, dtype=torch.int32, device=dev)
+    match_box = torch.empty(b, 12, device=dev)
+    d = _lib.AssociateDesc(b, F, D, int(axes[0]), int(axes[1]), float(gate2), rule is not None, (rule or (0, 1))[0], bool(coast),
+                           *(t.data_ptr() for t in (src, feed, adv, center, points, slots.t, slots.hit_t, slots.hit_c, slots.vel,
+                                                    fed, count, det, pred, match, match_box, rec_det, rec_count, rec_slot)))
+    _call("o3d_box_associate", ctypes.byref(d), _stream())
+    return pred, match, match_box
 
 
 # ------------------------------------------------------------------ scan ingest for the live tracker's feeds (csrc/scan_ingest.cu)

@@ -27,7 +27,15 @@ lines stop at that frame, its annotated frames after it are scored as failures (
 summary counts the tracklets ended early as "lost".  `--coast ALPHA` (with --lost) moves a missed target along its velocity
 instead of writing the network's box (MultiTargetTracker's `coast=`): every JSON line's targets carry "coasting", whether that
 frame's box was coasted, and the summary counts "coasted" (target-frames reported while coasting) and "reacquired" (coasting
-spells that ended in a hit).  Success / Precision score the coasted boxes."""
+spells that ended in a hit).  Success / Precision score the coasted boxes.
+
+Detections.  `--detections FILE --detection_gate METRES --max_detections N` gives every scan a 3D detector's boxes: FILE has one
+JSON line per {"scene", "frame", "class", "boxes": [[cx, cy, cz, w, l, h, qw, qx, qy, qz, score], ...]}, the scene id as the
+reader lists it (`scene_list`), the frame as the scene's frames are numbered, the class a config's category_name and the
+quaternion the box's orientation (data_classes.Box).  A scan without a line has no detections.  The tracker matches them to
+its targets (MultiTargetTracker's `detections=`) and re-acquires a missed target at its detection; tracklets still start from
+their first annotated box.  Every JSON line's targets carry "detection", the index of the detection matched on that frame in
+its line's boxes (null: none), and "reacquired"; the summary counts "reacquired_at_detection", the target-frames re-acquired."""
 import argparse
 import json
 import sys
@@ -89,6 +97,14 @@ def parse_args(argv=None):
     p.add_argument('--coast', type=float, metavar='ALPHA', default=argparse.SUPPRESS,
                    help='with --lost: move a target whose frame is a miss along its velocity (ALPHA, in (0, 1]: the weight of the '
                         'newest velocity sample) instead of writing the network\'s box')
+    # --detections and its two settings (SUPPRESS as well): a run without them keeps its options
+    p.add_argument('--detections', type=str, metavar='FILE', default=argparse.SUPPRESS,
+                   help='JSON lines of per-scan detections {"scene", "frame", "class", "boxes": [[cx, cy, cz, w, l, h, qw, qx, qy, '
+                        'qz, score], ...]}: matched to the targets, re-acquiring missed ones')
+    p.add_argument('--detection_gate', type=float, metavar='METRES', default=argparse.SUPPRESS,
+                   help='with --detections: the largest centre distance of a match, in the plane orthogonal to up_axis')
+    p.add_argument('--max_detections', type=int, metavar='N', default=argparse.SUPPRESS,
+                   help='with --detections: the most detections of one scan (1 .. 1024)')
     args = p.parse_args(argv)
     if hasattr(args, "lost"):
         from .tracking.multi_tracker import check_lost_rule
@@ -104,6 +120,15 @@ def parse_args(argv=None):
             args.coast = check_coast(args.coast, args.lost)
         except ValueError as e:
             p.error(f"--coast: {e}")
+    given = [hasattr(args, n) for n in ("detections", "detection_gate", "max_detections")]
+    if any(given) and not all(given):
+        p.error("--detections FILE needs --detection_gate METRES and --max_detections N, and they need it")
+    if all(given):
+        from .tracking.multi_tracker import check_detections
+        try:
+            args.detection_rule = check_detections((args.max_detections, args.detection_gate))
+        except ValueError as e:
+            p.error(f"--detection_gate / --max_detections: {e}")
     for extra in args.add_class or ():
         if len(extra) > 2:
             p.error(f"--add_class takes a config and at most one checkpoint, got {extra}")
@@ -216,14 +241,50 @@ def _yaw(rot, up_axis):
     return float(np.arctan2(rot[1, 0], rot[0, 0]))
 
 
-def _evidence(ev):
+def _evidence(ev, detections=False):
     """A target's JSON evidence: {"points", "score"}, null where the frame has none (a tracklet's first frame), and "coasting"
-    for a coasting tracker's evidence (points, score, coasted)."""
+    for a coasting tracker's evidence (points, score, coasted).  With `detections` the evidence ends with (reacquired,
+    detection): "reacquired" and "detection", null when the frame matched none."""
+    if detections:
+        ev, (reacquired, det) = ev[:-2], ev[-2:]
     points, score = ev[:2]
     out = {"points": points if points >= 0 else None, "score": score if np.isfinite(score) else None}
     if len(ev) > 2:
         out["coasting"] = bool(ev[2])
+    if detections:
+        out.update(detection=det if det >= 0 else None, reacquired=bool(reacquired))
     return out
+
+
+def read_detections(path):
+    """The --detections file: {(scene, frame, class): (M, 16) float32 rows (tracking.multi_tracker.detection_rows)}; the scene
+    id as a string.  Refuses (SystemExit) a malformed line or two lines for the same scan and class."""
+    from .datasets.data_classes import Box
+    from .datasets.nuscenes_data import quat_to_rot
+    from .tracking.multi_tracker import detection_rows
+    out = {}
+    with open(path) as f:
+        for n, line in enumerate(f, 1):
+            if not line.strip():
+                continue
+            try:
+                d = json.loads(line)
+                key = (str(d["scene"]), int(d["frame"]), str(d["class"]))
+                boxes = np.asarray(d["boxes"], np.float64).reshape(-1, 11)
+            except (ValueError, KeyError, TypeError) as e:
+                raise SystemExit(f"{path}:{n}: expected {{\"scene\", \"frame\", \"class\", \"boxes\": [[cx, cy, cz, w, l, h, qw, qx, qy, "
+                                 f"qz, score], ...]}} ({e})") from None
+            if key in out:
+                raise SystemExit(f"{path}:{n}: a second line for scene {key[0]} frame {key[1]} class {key[2]}")
+            if not np.isfinite(boxes).all() or (np.linalg.norm(boxes[:, 6:10], axis=1) == 0).any():
+                raise SystemExit(f"{path}:{n}: every value must be finite and every quaternion non-zero")
+            out[key] = detection_rows([Box(b[0:3], b[3:6], quat_to_rot(b[6:10])) for b in boxes], boxes[:, 10])
+    return out
+
+
+def _scan_detections(table, scene, frame, cls):
+    """One scan's detection rows for a class from `read_detections`' table (none when the file has no line for it)."""
+    return table.get((str(scene), int(frame), cls), np.zeros((0, 16), np.float32))
 
 
 def _coast_counts(ev, min_points):
@@ -253,9 +314,11 @@ def _score_tracklet(boxes, gts, frames, dim, up):
     return overlaps, distances
 
 
-def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, precision="fp32", lost=None, coast=None):
+def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, precision="fp32", lost=None, coast=None,
+        detections=None, scan_detections=None):
     """Track every scene of `dataset`'s split and write `out_path`; returns {"success", "precision", "frames", "scenes"},
-    "lost" with a `lost` rule, and "coasted" / "reacquired" with `coast`."""
+    "lost" with a `lost` rule, and "coasted" / "reacquired" with `coast`.  `detections`: (max_per_scan, gate) and
+    `scan_detections` the `read_detections` table: then also "reacquired_at_detection"."""
     from .tracking.multi_tracker import track_feeds
     from .utils.metrics import Precision, Success
 
@@ -274,17 +337,22 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, preci
             ends[tr["index"]] = pos[tr["end"]]
         scenes.append({"frames": len(p["frames"]), "starts": starts, "ends": ends,
                        "scan": lambda t, p=p: dataset.raw_scan(p["scene"], p["frames"][t])})
+        if detections is not None:
+            scenes[-1]["detections"] = lambda t, p=p: _scan_detections(scan_detections or {}, p["scene"], p["frames"][t],
+                                                                       cfg.category_name)
+    det = {} if detections is None else {"detections": detections}
     results, evidence = track_feeds(model, scenes, max(1, min(len(scenes), max_targets)), max_targets, seed=seed,
-                                    max_points=max_points, precision=precision, lost=lost, evidence=True, coast=coast)
+                                    max_points=max_points, precision=precision, lost=lost, evidence=True, coast=coast, **det)
     overlaps, distances = [[] for _ in annos], [[] for _ in annos]
-    ended, coasted, reacquired = 0, 0, 0
+    ended, coasted, reacquired, at_detection = 0, 0, 0, 0
     with open(out_path, "w") as f:
         for p, res, ev in zip(plan, results, evidence):
             scene, pos = p["scene"], {fr: t for t, fr in enumerate(p["frames"])}
             track_id = {tr["index"]: tr["track_id"] for tr in p["tracklets"]}
             for t, frame in enumerate(p["frames"]):
                 targets = [{"id": track_id[j], "tracklet": j, "center": b[t].center.tolist(), "wlh": b[t].wlh.tolist(),
-                            "yaw": _yaw(b[t].rotation_matrix, up), **_evidence(ev[j][t])} for j, b in sorted(res.items()) if t in b]
+                            "yaw": _yaw(b[t].rotation_matrix, up), **_evidence(ev[j][t], detections is not None)}
+                           for j, b in sorted(res.items()) if t in b]
                 f.write(json.dumps({"scene": scene, "frame": frame, "targets": targets}) + "\n")
             for tr in p["tracklets"]:
                 j = tr["index"]
@@ -292,6 +360,8 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, preci
                 if coast is not None:
                     c, r = _coast_counts(ev[j], lost[0])
                     coasted, reacquired = coasted + c, reacquired + r
+                if detections is not None:
+                    at_detection += sum(bool(e[-2]) for e in ev[j].values())
                 overlaps[j], distances[j] = _score_tracklet(res[j], [dataset.box_from_anno(a) for a in annos[j]],
                                                             [pos[dataset.anno_frame(a)[1]] for a in annos[j]], dim, up)
     succ, prec = Success(), Precision()
@@ -303,16 +373,20 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, preci
         out["lost"] = ended
     if coast is not None:
         out.update(coasted=coasted, reacquired=reacquired)
+    if detections is not None:
+        out["reacquired_at_detection"] = at_detection
     return out
 
 
-def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0, precision="fp32", lost=None, coast=None):
+def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0, precision="fp32", lost=None, coast=None,
+                detections=None, scan_detections=None):
     """`run` for several classes in one pass over the scans: `models`, `datasets` and `max_targets` are {class: ...} (the class
     is its config's category_name).  Every scene streams once for all classes (class_scene_plan) through one MultiClassTracker;
     a target's draws are keyed by its tracklet's index in its class's reader, as in a one-class run.  Every JSON line's targets
     carry their "class".  Returns {"success", "precision", "frames", "scenes"} over every class's frames, and the same per class
     under "classes"; with a `lost` rule (every class's), "lost" counts the tracklets it ended early, overall and per class, and
-    with `coast` (every class's), so do "coasted" and "reacquired"."""
+    with `coast` (every class's), so do "coasted" and "reacquired"; with `detections` (every class's, and `scan_detections` the
+    `read_detections` table), "reacquired_at_detection"."""
     from .tracking.multi_class import track_classes
     from .utils.metrics import Precision, Success
 
@@ -324,13 +398,20 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
         max_points = class_stream_max_points(datasets, plan)
     annos = {c: datasets[c].tracklet_anno_list for c in names}
     scenes = class_scenes(datasets, plan)
+    det = {}
+    if detections is not None:
+        det = {"detections": detections}
+        for sc, p in zip(scenes, plan):
+            sc["detections"] = lambda t, p=p: {c: _scan_detections(scan_detections or {}, p["scene"], p["frames"][t], c)
+                                               for c in names}
     results, evidence = track_classes(models, scenes, max(1, min(len(scenes), sum(max_targets.values()))), max_targets,
                                       seed=seed, max_points=max_points, precision=precision, lost=lost, evidence=True,
-                                      coast=coast)
+                                      coast=coast, **det)
     overlaps = {c: [[] for _ in annos[c]] for c in names}
     distances = {c: [[] for _ in annos[c]] for c in names}
     ended = {c: 0 for c in names}
     coasted, reacquired = {c: 0 for c in names}, {c: 0 for c in names}
+    at_detection = {c: 0 for c in names}
     rank = {c: i for i, c in enumerate(names)}
     with open(out_path, "w") as f:
         for p, res, ev in zip(plan, results, evidence):
@@ -338,7 +419,8 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
             track_id = {(tr["class"], tr["index"]): tr["track_id"] for tr in p["tracklets"]}
             for t, frame in enumerate(p["frames"]):
                 targets = [{"class": c, "id": track_id[(c, j)], "tracklet": j, "center": b[t].center.tolist(),
-                            "wlh": b[t].wlh.tolist(), "yaw": _yaw(b[t].rotation_matrix, up), **_evidence(ev[(c, j)][t])}
+                            "wlh": b[t].wlh.tolist(), "yaw": _yaw(b[t].rotation_matrix, up),
+                            **_evidence(ev[(c, j)][t], detections is not None)}
                            for (c, j), b in sorted(res.items(), key=lambda kv: (rank[kv[0][0]], kv[0][1])) if t in b]
                 f.write(json.dumps({"scene": scene, "frame": frame, "targets": targets}) + "\n")
             for tr in p["tracklets"]:
@@ -348,6 +430,8 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
                     n_coasted, n_reacquired = _coast_counts(ev[(c, j)], lost[0])
                     coasted[c] += n_coasted
                     reacquired[c] += n_reacquired
+                if detections is not None:
+                    at_detection[c] += sum(bool(e[-2]) for e in ev[(c, j)].values())
                 ds = datasets[c]
                 overlaps[c][j], distances[c][j] = _score_tracklet(res[(c, j)], [ds.box_from_anno(a) for a in annos[c][j]],
                                                                   [pos[ds.anno_frame(a)[1]] for a in annos[c][j]], dim, up)
@@ -363,6 +447,8 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
             out["lost"] = sum(ended[c] for c in classes)
         if coast is not None:
             out.update(coasted=sum(coasted[c] for c in classes), reacquired=sum(reacquired[c] for c in classes))
+        if detections is not None:
+            out["reacquired_at_detection"] = sum(at_detection[c] for c in classes)
         return out
 
     out = scores(names)
@@ -401,6 +487,8 @@ def main(argv=None):
     rule = {"lost": args.lost} if hasattr(args, "lost") else {}           # without --lost, run / run_classes as they always were
     if hasattr(args, "coast"):
         rule["coast"] = args.coast
+    if hasattr(args, "detections"):
+        rule.update(detections=args.detection_rule, scan_detections=read_detections(args.detections))
     classes = [(args.cfg, args.checkpoint)] + [(a[0], a[1] if len(a) > 1 else None) for a in args.add_class or ()]
     cfgs = [load_config(c) for c, _ in classes]
     check_classes(cfgs, [c for c, _ in classes])

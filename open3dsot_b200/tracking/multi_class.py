@@ -18,7 +18,8 @@ import torch
 from .. import runtime
 import numpy as np
 
-from .multi_tracker import MultiTargetTracker, ScanFeeds, check_coast, check_lost_rule, class_peaks, feed_schedule, run_scenes
+from .multi_tracker import (MultiTargetTracker, ScanFeeds, check_coast, check_detections, check_lost_rule, class_peaks,
+                            feed_schedule, run_scenes)
 
 SHARED_KEYS = ("up_axis", "IoU_space", "degrees")
 
@@ -28,10 +29,13 @@ class MultiClassTracker:
     store) of at most `max_points` points per scan.  `seed`, `use_graph` and `precision` as for MultiTargetTracker, for every
     class; `lost` is one end-of-track rule for every class (MultiTargetTracker's `lost=`) or {class: rule}, a class without an
     entry never losing a target; `coast` likewise one alpha (MultiTargetTracker's `coast=`) or {class: alpha}, a class without
-    an entry never coasting (a class that coasts needs a rule).  `put` / `put_raw` / `advance()` as on MultiTargetTracker;
-    `add(cls, id, box, feed=)` / `drop(cls, id)` start and end a target of a class."""
+    an entry never coasting (a class that coasts needs a rule); `detections` likewise one (max_per_scan, gate) or
+    {class: (max_per_scan, gate)}, a class without an entry taking no detections.  `put` / `put_raw` / `advance()` as on
+    MultiTargetTracker, with a scan's detections given per class ({class: rows}); `add(cls, id, box, feed=)` / `drop(cls, id)`
+    start and end a target of a class."""
 
-    def __init__(self, models, max_points, max_targets, feeds=1, seed=0, use_graph=True, precision="fp32", lost=None, coast=None):
+    def __init__(self, models, max_points, max_targets, feeds=1, seed=0, use_graph=True, precision="fp32", lost=None, coast=None,
+                 detections=None):
         if not models:
             raise ValueError("MultiClassTracker: no classes; give one model per class")
         self.precision = runtime.check_precision(precision)
@@ -56,6 +60,15 @@ class MultiClassTracker:
                 coasts[n] = check_coast(coasts.get(n), rules[n])
             except ValueError as e:
                 raise ValueError(f"class {n!r}: {e}") from None
+        dets = detections if isinstance(detections, dict) else {n: detections for n in names}
+        for n in dets:
+            if n not in models:
+                raise ValueError(f"detections: class {n!r} has no model")
+        for n in names:
+            try:
+                dets[n] = check_detections(dets.get(n))
+            except ValueError as e:
+                raise ValueError(f"class {n!r}: {e}") from None
         c0 = models[names[0]].config
         for n in names[1:]:
             c = models[n].config
@@ -72,7 +85,8 @@ class MultiClassTracker:
         for n in names:
             try:
                 self.trackers[n] = MultiTargetTracker(models[n], max_points, max_targets[n], seed=seed, use_graph=use_graph,
-                                                      feeds=self.scan_feeds, precision=precision, lost=rules[n], coast=coasts[n])
+                                                      feeds=self.scan_feeds, precision=precision, lost=rules[n], coast=coasts[n],
+                                                      detections=dets[n])
             except ValueError as e:
                 self.scan_feeds.owner = None
                 raise ValueError(f"class {n!r}: {e}") from None
@@ -105,13 +119,35 @@ class MultiClassTracker:
             raise ValueError(f"class {cls!r} is not tracked here; the classes are {list(self.trackers)}")
         return trk
 
-    def put(self, feed, points, n_valid=None):
-        """Stage the next scan of `feed` for every class (ScanFeeds.put).  No host sync."""
-        self.scan_feeds.put(feed, points, n_valid)
+    def _check_detections(self, feed, detections):
+        """A put's {class: rows}, each checked by its class tracker (ValueError) before anything is staged."""
+        if detections is None:
+            return {}
+        if not isinstance(detections, dict):
+            raise ValueError("detections: expected {class: (M, 16) rows}")
+        out = {}
+        for n, rows in detections.items():
+            try:
+                out[n] = self._class(n)._check_detections(feed, rows)
+            except ValueError as e:
+                raise ValueError(f"class {n!r}: {e}") from None
+        return out
 
-    def put_raw(self, feed, rows, transforms=()):
-        """Stage the next scan of `feed` as a reader stores it (ScanFeeds.put_raw); the next `advance()` ingests it."""
+    def put(self, feed, points, n_valid=None, detections=None):
+        """Stage the next scan of `feed` for every class (ScanFeeds.put), with its detections per class ({class: rows}, for the
+        classes built with detections=).  No host sync."""
+        rows = self._check_detections(feed, detections)
+        self.scan_feeds.put(feed, points, n_valid)
+        for n, r in rows.items():
+            self.trackers[n]._stage_detections(feed, r)
+
+    def put_raw(self, feed, rows, transforms=(), detections=None):
+        """Stage the next scan of `feed` as a reader stores it (ScanFeeds.put_raw); the next `advance()` ingests it.  `detections`
+        as for `put`."""
+        det = self._check_detections(feed, detections)
         self.scan_feeds.put_raw(feed, rows, transforms)
+        for n, r in det.items():
+            self.trackers[n]._stage_detections(feed, r)
 
     def advance(self):
         """Bring in every staged scan (one copy, one ingest) and advance every class's active targets of those feeds to it, each
@@ -155,6 +191,26 @@ class MultiClassTracker:
     def _coast_rows(self):
         return np.concatenate([trk._coast_rows() for trk in self.trackers.values()])
 
+    def _match_record(self):
+        return torch.cat([trk._match_record() for trk in self.trackers.values()])
+
+    def _detect_rows(self):
+        return np.concatenate([trk._detect_rows() for trk in self.trackers.values()])
+
+    def unmatched(self):
+        """{class: {feed: [(index, data_classes.Box, score), ...]}}: MultiTargetTracker.unmatched() of every class built with
+        detections=, read back from the device together (one sync)."""
+        classes = [n for n, trk in self.trackers.items() if trk.detections is not None]
+        if not classes:
+            raise ValueError("unmatched(): no class was built with detections=")
+        flats = [self.trackers[n]._unmatched_device() for n in classes]
+        host = torch.cat(flats).cpu().numpy()
+        out, at = {}, 0
+        for n, flat in zip(classes, flats):
+            out[n] = self.trackers[n]._unmatched_decode(host[at:at + flat.numel()])
+            at += flat.numel()
+        return out
+
     def lost_targets(self):
         """(class, id) of the active targets their class's rule has declared lost, read back from the device (one sync)."""
         lost = torch.cat([trk.lost for trk in self.trackers.values()]).cpu().numpy()
@@ -175,14 +231,16 @@ class MultiClassTracker:
 
 
 def track_classes(models, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32",
-                  lost=None, evidence=False, coast=None):
+                  lost=None, evidence=False, coast=None, detections=None):
     """`track_feeds` for several classes through one MultiClassTracker.  `models` and `max_targets`: {class: model},
     {class: slots}.  A scene's targets are named (class, id): "starts": {t: [((class, id), Box), ...]}, "ends": {(class, id):
     last t}; (class, id) is unique over all scenes.  A scene is admitted when a feed is free and every class has the scene's
     peak of that class free.  Returns, per scene, {(class, id): {t: data_classes.Box}}.  `lost`: one end-of-track rule or
     {class: rule} (MultiClassTracker); a lost target's results end at the frame it was declared lost on.  With `evidence`, also
     returns, per scene, {(class, id): {t: (points in the box, score)}}, with a third value, whether the frame was coasted, for
-    the classes that coast (`coast`: one alpha or {class: alpha}, MultiClassTracker)."""
+    the classes that coast (`coast`: one alpha or {class: alpha}, MultiClassTracker).  `detections`: one (max_per_scan, gate) or
+    {class: (max_per_scan, gate)} (MultiClassTracker); a scene's "detections": t -> {class: rows} of its scan t, and the
+    evidence of the classes that take detections ends with (reacquired, detection) (run_scenes)."""
     runtime.check_precision(precision)
     if max_points is None:
         raise ValueError("track_classes: give max_points, the largest scan of the scenes")
@@ -195,6 +253,6 @@ def track_classes(models, scenes, feeds, max_targets, seed=0, max_points=None, u
     peaks = [class_peaks(lengths[i], sc["starts"], sc["ends"]) for i, sc in enumerate(scenes)]
     sched = feed_schedule(lengths, peaks, feeds, max_targets)
     trk = MultiClassTracker(models, max_points, max_targets, feeds=feeds, seed=seed, use_graph=use_graph, precision=precision,
-                            lost=lost, coast=coast)
+                            lost=lost, coast=coast, detections=detections)
     return run_scenes(trk, lambda key, box, f: trk.add(*key, box, feed=f), lambda key: trk.drop(*key), scenes, sched, chunk,
                       evidence)

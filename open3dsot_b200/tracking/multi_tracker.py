@@ -40,6 +40,10 @@ that advance) until the host drops it (`lost_targets()` / `drop_lost()`).  With 
 moved along the target's velocity from its last hit instead of the network's, so the next search is centred where the target
 should be; the first hit again takes it back.  All of it runs inside the captured step, per row, so it neither synchronises nor
 depends on the bucket, K or the other targets: the whole write-back is one `o3d_track_update` launch (csrc/track_update.cu).
+Detections.  With `detections=(max_per_scan, gate)` a scan may come with a 3D detector's boxes (`put(..., detections=)`).  The
+step matches each feed's detections to its advancing rows greedily by plane distance to the centre the row would write without
+them (`o3d_box_associate`, csrc/associate.cu, one launch before the write-back); a matched miss is re-acquired at its
+detection's box, and every feed keeps its most recent advance's detections with the slot each matched, for `unmatched()`.
 Device memory: feeds * 2 * max_points * 12 bytes of scans, plus per slot the crop scratch and, for the first-frame template
 modes, max_points * 13 bytes of first-frame crop.  Ground-truth reference boxes (reference_BB 'previous_gt' / 'current_gt') have no meaning on a live stream, and
 shape_aggregation 'all' is not supported here; both are refused."""
@@ -102,6 +106,78 @@ def coast_weights(alpha):
     return None if alpha is None else (float(np.float32(alpha)), float(np.float32(1 - alpha)))
 
 
+def check_detections(detections):
+    """`detections=`: None (scans carry no detections) or (max_per_scan, gate): an int in 1 .. 1024 and a finite distance in
+    metres > 0.  Returns (max_per_scan, gate) or None."""
+    if detections is None:
+        return None
+    try:
+        max_per_scan, gate = detections
+    except (TypeError, ValueError):
+        raise ValueError(f"detections={detections!r}: expected None or (max_per_scan, gate)") from None
+    if isinstance(max_per_scan, bool) or not isinstance(max_per_scan, (int, np.integer)) \
+            or not 1 <= max_per_scan <= ops.MAX_DETECTIONS:
+        raise ValueError(f"detections: max_per_scan={max_per_scan!r} must be an integer in 1 .. {ops.MAX_DETECTIONS}")
+    if isinstance(gate, bool) or not isinstance(gate, (int, float, np.integer, np.floating)) or not math.isfinite(gate) \
+            or not gate > 0 or not np.float32(gate) > 0:
+        raise ValueError(f"detections: gate={gate!r} must be a finite distance in metres > 0")
+    return int(max_per_scan), float(gate)
+
+
+def detection_gate2(gate):
+    """The squared gate the matching compares with, computed once in float32: float32(gate) * float32(gate)."""
+    g = np.float32(gate)
+    return float(g * g)
+
+
+def plane_axes(up_axis):
+    """The two axes of the plane the matching measures distances in: those where `up_axis` is 0."""
+    axes = tuple(i for i, a in enumerate(up_axis) if a == 0)
+    if len(axes) != 2 or len(up_axis) != 3:
+        raise ValueError(f"up_axis={list(up_axis)}: detection matching needs exactly one non-zero up component")
+    return axes
+
+
+def detection_rows(boxes, scores):
+    """A scan's detections as the (M, 16) float32 array `put(..., detections=)` takes: data_classes.Box objects and their
+    scores -> per row centre (3), wlh (3), row-major rotation with the box axes in its columns (9), score."""
+    boxes, scores = list(boxes), list(scores)
+    if len(boxes) != len(scores):
+        raise ValueError(f"detection_rows: {len(boxes)} boxes and {len(scores)} scores")
+    out = np.zeros((len(boxes), ops.DETECTION_VALUES), np.float32)
+    for i, (b, sc) in enumerate(zip(boxes, scores)):
+        c, s, r = _box_values(b)
+        out[i] = np.concatenate([c, s, r.reshape(-1), [sc]])
+    return out
+
+
+def check_detection_array(rows, max_per_scan):
+    """One scan's detections as staged: an (M, 16) array (numpy or torch) with M <= max_per_scan and every value finite;
+    returns it as a float32 numpy array.  ValueError otherwise."""
+    if isinstance(rows, torch.Tensor):
+        rows = rows.detach().cpu().numpy()
+    try:
+        rows = np.asarray(rows, dtype=np.float32)
+    except (TypeError, ValueError):
+        raise ValueError("detections: expected an (M, 16) array of numbers") from None
+    if rows.size == 0:
+        rows = rows.reshape(0, ops.DETECTION_VALUES)
+    if rows.ndim != 2 or rows.shape[1] != ops.DETECTION_VALUES:
+        raise ValueError(f"detections: shape {rows.shape}; expected (M, {ops.DETECTION_VALUES}): centre, wlh, row-major rotation, "
+                         f"score")
+    if rows.shape[0] > max_per_scan:
+        raise ValueError(f"detections: {rows.shape[0]} detections; the tracker takes at most max_per_scan={max_per_scan}")
+    if not np.isfinite(rows).all():
+        raise ValueError("detections: every value must be finite")
+    return np.ascontiguousarray(rows)
+
+
+class MatchSlots(NamedTuple):
+    """The per-slot detection state the write-back reads and writes with matches (ops.MATCH_SLOTS, in its order)."""
+    detection: torch.Tensor    # (R,) int32: the last advance's detection index in its feed's list, -1 for none
+    reacquired: torch.Tensor   # (R,) bool: the last advance was a miss re-acquired at its detection
+
+
 class Slots(NamedTuple):
     """The per-slot state the step's write-back reads and writes (ops.TRACK_SLOTS, in its order); rows are slots."""
     box_c: torch.Tensor        # (R, 3) float32
@@ -118,7 +194,7 @@ class Slots(NamedTuple):
     coasting: torch.Tensor     # (R,) bool
 
 
-def track_update_tensors(slots, src, dst, adv, center, rot, points, score, rule=None, coast=None):
+def track_update_tensors(slots, src, dst, adv, center, rot, points, score, rule=None, coast=None, match=None):
     """The tensor formulation of the step's per-row write-back (`ops.track_update`, csrc/track_update.cu), in place on `slots`:
     row i reads slot src[i] and writes slot dst[i].  adv (b,) bool: the row advanced; center (b, 3) / rot (b, 3, 3): the
     network's box P; points (b,) int32 / score (b,) float32: its evidence.  A row that does not advance keeps its state.  An
@@ -126,16 +202,29 @@ def track_update_tensors(slots, src, dst, adv, center, rot, points, score, rule=
     min_points) or resets the count on a hit; lost |= misses >= patience.  Its box is P, except with `coast` = (alpha, beta)
     (float32 values) on a miss: then the centre is hit_c + vel * (t' - hit_t) and the rotation the previous one.  A hit with
     `coast` updates vel (the first sample, hit_t == 0, as is; then alpha * v + beta * vel with v = (P.c - hit_c) / (t' - hit_t))
-    and moves hit_c / hit_t to P.c / t'; coasting = miss and not lost.  Every fp32 operation is one rounded operation."""
+    and moves hit_c / hit_t to P.c / t'; coasting = miss and not lost.  `match`: None or (match (b,) int32, match_box (b, 12),
+    detection, reacquired) from `associate_tensors`, with the MatchSlots state: an advanced row records its match, and a matched
+    miss under the rule is re-acquired, handled as a hit whose box P is the detection's centre and rotation.  Every fp32
+    operation is one rounded operation."""
     g = lambda x: x.index_select(0, src)
     a = adv[:, None]
     t = g(slots.t) + adv.long()
     old_c, old_r = g(slots.box_c), g(slots.box_r)
     misses, lost = g(slots.misses), g(slots.lost)
     vel, hit_c, hit_t, coasting = g(slots.vel), g(slots.hit_c), g(slots.hit_t), g(slots.coasting)
+    if match is not None:
+        m, m_box, detection, reacquired = match
+        net_hit = torch.ones_like(adv) if rule is None else points >= rule[0]
+        re = adv & (m >= 0) & ~net_hit
+        center = torch.where(re[:, None], m_box[:, :3], center)
+        rot = torch.where(re[:, None, None], m_box[:, 3:].reshape(-1, 3, 3), rot)
+        detection.index_copy_(0, dst, torch.where(adv, m, g(detection)))
+        reacquired.index_copy_(0, dst, torch.where(adv, re, g(reacquired)))
     if rule is not None:
         min_points, patience = rule
         hit = points >= min_points
+        if match is not None:
+            hit = hit | re
         misses = torch.where(adv, torch.where(hit, torch.zeros_like(misses), misses + 1), misses)
         lost = lost | (misses >= patience)
         if coast is not None:
@@ -161,14 +250,69 @@ def track_update_tensors(slots, src, dst, adv, center, rot, points, score, rule=
         getattr(slots, name).index_copy_(0, dst, v)
 
 
-def track_update(slots, src, dst, adv, center, rot, points, score, rule=None, coast=None):
+def track_update(slots, src, dst, adv, center, rot, points, score, rule=None, coast=None, match=None):
     """The step's per-row write-back (`track_update_tensors`): CUDA slot state through one `o3d_track_update` launch
     (csrc/track_update.cu), other tensors through the tensor formulation."""
     if slots.box_c.is_cuda:
         ops.track_update(slots, src, dst, adv, center.contiguous(), rot.contiguous(), points, score.float().contiguous(), rule,
-                         coast)
+                         coast, match)
     else:
-        track_update_tensors(slots, src, dst, adv, center, rot, points, score, rule, coast)
+        track_update_tensors(slots, src, dst, adv, center, rot, points, score, rule, coast, match)
+
+
+def associate_tensors(src, feed, adv, center, points, slots, fed, count, det, records, gate2, axes, rule=None, coast=False):
+    """The formulation of the step's detection matching (`ops.box_associate`, csrc/associate.cu), which it equals exactly.  Row
+    i of feed feed[i] takes part when adv[i]; it is matched against pred[i], the centre `track_update_tensors` writes without
+    detections: the network's centre on a hit or without the rule, and with `coast` on a miss hit_c + vel * gap of slot src[i].
+    Per fed feed f, with detections det[f, :count[f]]: every (row, detection) pair with d2 = dx*dx + dy*dy <= gate2 over the
+    plane `axes` is a candidate, and the candidates are visited in ascending (d2, row, detection) order, a pair accepted when
+    its row and its detection are both free.  Updates `records` = (rec_det, rec_count, rec_slot) for the fed feeds: their
+    detections and, per detection, the slot of its row or -1.  Returns (pred (b, 3), NaN for the rows that do not take part;
+    match (b,) int32, -1 for none; match_box (b, 12), the matched detection's centre and rotation, zeros without a match)."""
+    b = adv.shape[0]
+    hit = torch.ones_like(adv) if rule is None else points >= rule[0]
+    gap = (slots.t.index_select(0, src) + 1 - slots.hit_t.index_select(0, src)).float()[:, None]
+    coasted = slots.hit_c.index_select(0, src) + slots.vel.index_select(0, src) * gap
+    pred = torch.where(((~hit) & bool(coast))[:, None], coasted, center)
+    pred = torch.where(adv[:, None], pred, torch.full_like(pred, float("nan")))
+    match = torch.full((b,), -1, dtype=torch.int32, device=adv.device)
+    match_box = torch.zeros(b, 12, dtype=torch.float32, device=adv.device)
+    rec_det, rec_count, rec_slot = records
+    a0, a1 = axes
+    fed_h, count_h, feed_h, adv_h, src_h = (x.cpu().numpy() for x in (fed, count, feed, adv, src))
+    for f in np.flatnonzero(fed_h != 0):
+        nd = int(count_h[f])
+        rows = np.flatnonzero(adv_h & (feed_h == f))
+        slot_of = np.full(nd, -1, np.int32)
+        if nd and len(rows):
+            q = det[f, :nd]
+            r = torch.from_numpy(rows).to(adv.device)
+            dx = pred[r, a0][:, None] - q[None, :, a0]
+            dy = pred[r, a1][:, None] - q[None, :, a1]
+            d2 = (dx * dx + dy * dy).cpu().numpy()
+            ri, di = np.nonzero(d2 <= gate2)
+            order = np.lexsort((di, rows[ri], d2[ri, di]))
+            row_free, det_free = np.ones(len(rows), bool), np.ones(nd, bool)
+            for k in order:
+                i, d = ri[k], di[k]
+                if row_free[i] and det_free[d]:
+                    row_free[i] = det_free[d] = False
+                    match[rows[i]] = int(d)
+                    match_box[rows[i]] = torch.cat([det[f, d, 0:3], det[f, d, 6:15]])
+                    slot_of[d] = src_h[rows[i]]
+        rec_det[f, :nd] = det[f, :nd]
+        rec_slot[f, :nd] = torch.from_numpy(slot_of).to(rec_slot.device)
+        rec_count[f] = nd
+    return pred, match, match_box
+
+
+def associate(src, feed, adv, center, points, slots, fed, count, det, records, gate2, axes, rule=None, coast=False):
+    """The step's detection matching (`associate_tensors`): CUDA tensors through one `o3d_box_associate` launch
+    (csrc/associate.cu), other tensors through the formulation."""
+    if adv.is_cuda:
+        return ops.box_associate(src, feed, adv, center.contiguous(), points, slots, fed, count, det, records, gate2, axes, rule,
+                                 coast)
+    return associate_tensors(src, feed, adv, center, points, slots, fed, count, det, records, gate2, axes, rule, coast)
 
 
 def _box_values(box):
@@ -357,13 +501,18 @@ class MultiTargetTracker:
     store), and `_run()` advances this one tracker's slots.  `lost`: None (no target is ever declared lost) or
     (min_points, patience), the end-of-track rule the step applies on the device; `boxes()` / `evidence()` report every slot's
     evidence either way.  `coast`: None or alpha in (0, 1] (needs `lost`): a miss moves the box along the target's velocity, the
-    alpha-weighted average of its centre's displacement per advance between hits, instead of writing the network's box."""
+    alpha-weighted average of its centre's displacement per advance between hits, instead of writing the network's box.
+    `detections`: None or (max_per_scan, gate): `put` / `put_raw` then take each scan's detections, (M, 16) rows
+    (`detection_rows`), matched on the device to the targets of their feed within `gate` metres in the plane orthogonal to the
+    config's up_axis; a matched miss is re-acquired at its detection, and `unmatched()` lists the detections no target took."""
 
-    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1, precision="fp32", lost=None, coast=None):
+    def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1, precision="fp32", lost=None, coast=None,
+                 detections=None):
         self.precision = runtime.check_precision(precision)
         self.lost_rule = check_lost_rule(lost)
         self.coast = check_coast(coast, self.lost_rule)
         self._coast = coast_weights(self.coast)
+        self.detections = check_detections(detections)
         self.model = model.eval()
         self.cfg = cfg = model.config
         self.dev = dev = next(model.parameters()).device
@@ -422,14 +571,36 @@ class MultiTargetTracker:
         self.vel, self.hit_c, self.hit_t, self.coasting = (x[:K] for x in (self._vel, self._hit_c, self._hit_t, self._coasting))
         self._slots = Slots(self._box_c, self._box_r, self._t, self._first_flag, self._points, self._score, self._misses, self._lost,
                             self._vel, self._hit_c, self._hit_t, self._coasting)
+        # Detections (detections=): the last advance's detection of each slot (-1: none) and whether it re-acquired the target
+        self._detection = torch.full((K + 2,), -1, device=dev, dtype=torch.int32)
+        self._reacquired = torch.zeros(K + 2, dtype=torch.bool, device=dev)
+        self.detection, self.reacquired = self._detection[:K], self._reacquired[:K]
+        self._match_slots = MatchSlots(self._detection, self._reacquired)
+        # The work list of the next bucket step, (2, K) as work_rows() lays it out; one host->device copy per advance.  With
+        # detections the same copy brings each feed's detection count and rows: [work | counts (F,) int32 | rows (F, D, 16)].
+        if self.detections is None:
+            self._work = torch.zeros(2, K, **i64)
+        else:
+            D = self.D = self.detections[0]
+            self._gate2 = detection_gate2(self.detections[1])
+            self._axes = plane_axes(cfg.up_axis)
+            self._det_at = 16 * K + -(-4 * F // 16) * 16
+            self._upload = torch.zeros(self._det_at + F * D * 64, device=dev, dtype=torch.uint8)
+            self._work = self._upload[:16 * K].view(torch.int64).view(2, K)
+            self._det_n = self._upload[16 * K:16 * K + 4 * F].view(torch.int32)
+            self._det_in = self._upload[self._det_at:].view(torch.float32).view(F, D, 16)
+            self._det_staged = {}                         # feed -> (M, 16) float32 rows for the next advance
+            # per feed, its most recent fed advance's detections, their count and the slot each matched (-1: none)
+            self._det_rec = torch.zeros(F, D, 16, **f)
+            self._det_count = torch.zeros(F, device=dev, dtype=torch.int32)
+            self._det_slot = torch.full((F, D), -1, device=dev, dtype=torch.int32)
+            self._det_d = torch.arange(D, device=dev, dtype=torch.int32)
         if self.mode in ("firstandprevious", "first"):
             self._first_local = torch.zeros(K + 2, N, 3, **f)
             self._first_keep = torch.zeros(K + 2, N, dtype=torch.bool, device=dev)
             self.first_local, self.first_keep = self._first_local[:K], self._first_keep[:K]
         self.slot_of = {}                                 # target id -> slot
         self._feed_of = {}                                # slot -> feed of the active targets (host mirror of slot_feed)
-        # The work list of the next bucket step, (2, K) as work_rows() lays it out; one host->device copy per advance.
-        self._work = torch.zeros(2, K, **i64)
         self._buckets = None                              # the step sizes (occupancy_buckets), fixed on the first advance
         self.graphs = {}                                  # bucket -> captured step
 
@@ -502,8 +673,14 @@ class MultiTargetTracker:
             scans = self.scans.view(2 * self.F, self.N, 3)
             points = ops.box_points(scans, self.count.view(2 * self.F), r["cur"], new.center, new.rot,
                                     bx.inclusive_half(new.wlh, EVIDENCE_WLH_FACTOR))
+            match = None
+            if self.detections is not None:
+                _, m, m_box = associate(self._work[0, :b], r["feed"], r["adv"], new.center, points, self._slots, self.fstate[0],
+                                        self._det_n, self._det_in, (self._det_rec, self._det_count, self._det_slot), self._gate2,
+                                        self._axes, self.lost_rule, self._coast is not None)
+                match = (m, m_box) + tuple(self._match_slots)
             track_update(self._slots, self._work[0, :b], dst, r["adv"], new.center, new.rot, points, score, self.lost_rule,
-                         self._coast)
+                         self._coast, match)
 
     def _gather(self, b):
         """The state of the first `b` rows of the work list: (rows {cur, prev, key, t, first_flag, adv[, first]}, box, the rows
@@ -514,7 +691,8 @@ class MultiTargetTracker:
         # a lost target holds from the advance it was declared lost on
         adv = self._active.index_select(0, src) & (fed[feed] != 0) & ~self._lost.index_select(0, src)
         r = {"cur": feed * 2 + fcur[feed], "prev": feed * 2 + fprev[feed], "key": self._key.index_select(0, src),
-             "t": self._t.index_select(0, src) + adv.long(), "first_flag": self._first_flag.index_select(0, src), "adv": adv}
+             "t": self._t.index_select(0, src) + adv.long(), "first_flag": self._first_flag.index_select(0, src), "adv": adv,
+             "feed": feed}
         if self.mode in ("firstandprevious", "first"):
             r["first"] = (self._first_local.index_select(0, src), self._first_keep.index_select(0, src))
         box = bx.Box(self._box_c.index_select(0, src), self._box_s.index_select(0, src), self._box_r.index_select(0, src))
@@ -522,7 +700,9 @@ class MultiTargetTracker:
 
     def _state(self):
         """The slot state a step writes (what the warm-up before a capture must put back)."""
-        return tuple(self._slots)
+        if self.detections is None:
+            return tuple(self._slots)
+        return tuple(self._slots) + tuple(self._match_slots) + (self._det_rec, self._det_count, self._det_slot)
 
     def _plan(self):
         """First advance: the bucket sizes, from the row counts of the network's stacks in one step over all K slots (its
@@ -556,14 +736,21 @@ class MultiTargetTracker:
         captures every bucket's step, so that later calls never synchronise."""
         slots = work_slots(self._feed_of, fed)
         first = self._buckets is None or (self.use_graph and not self.graphs)
-        if not slots and not first:
+        detect = self.detections is not None and bool(fed)
+        if not slots and not first and not detect:
             return
-        w = torch.from_numpy(work_rows(slots, self.K))
-        # a fresh pinned buffer for every advance: it is not rewritten before its copy runs
-        self._work.copy_(w.pin_memory() if self.dev.type == "cuda" else w, non_blocking=True)
+        w = work_rows(slots, self.K)
+        if self.detections is None:
+            w = torch.from_numpy(w)
+            # a fresh pinned buffer for every advance: it is not rewritten before its copy runs
+            self._work.copy_(w.pin_memory() if self.dev.type == "cuda" else w, non_blocking=True)
+        else:
+            self._upload_with_detections(w, fed)
         if first:
             self._plan()
         if not slots:
+            if detect:
+                self._record_unmatched()
             return
         b = bucket_for(len(slots), self._buckets)
         if self.use_graph:
@@ -571,19 +758,62 @@ class MultiTargetTracker:
         else:
             self._step(b)
 
+    def _upload_with_detections(self, w, fed):
+        """One host->device copy of the work list `w` and the staged detections of the feeds in `fed` (a fed feed staged without
+        detections has none), from a fresh pinned buffer; only the bytes up to the last staged row are copied."""
+        staged, self._det_staged = self._det_staged, {}
+        F, D = self.F, self.D
+        end = max([self._det_at] + [self._det_at + (f * D + len(rows)) * 64 for f, rows in staged.items() if len(rows)])
+        buf = torch.empty(end, dtype=torch.uint8, pin_memory=self.dev.type == "cuda")
+        host = buf.numpy()
+        host[:16 * self.K] = w.reshape(-1).view(np.uint8)
+        counts = np.array([len(staged.get(f, ())) if f in fed else 0 for f in range(F)], np.int32)
+        host[16 * self.K:16 * self.K + 4 * F] = counts.view(np.uint8)
+        for f, rows in staged.items():
+            if len(rows):
+                at = self._det_at + f * D * 64
+                host[at:at + rows.nbytes] = rows.reshape(-1).view(np.uint8)
+        self._upload[:end].copy_(buf, non_blocking=True)
+
+    def _record_unmatched(self):
+        """An advance that steps no target: record the fed feeds' detections, all unmatched (no host sync)."""
+        fed = self.fstate[0] != 0
+        keep = fed[:, None] & (self._det_d[None] < self._det_n[:, None])
+        self._det_rec.copy_(torch.where(keep[..., None], self._det_in, self._det_rec))
+        self._det_slot.masked_fill_(keep, -1)
+        self._det_count.copy_(torch.where(fed, self._det_n, self._det_count))
+
     # ------------------------------------------------------------------ public interface
     def _feed(self, feed):
         return self.scan_feeds.feed(feed)
 
-    def put(self, feed, points, n_valid=None):
-        """Stage the next scan of `feed` (ScanFeeds.put): a CUDA tensor is copied into the feed's next buffer at once, a host
-        tensor or array goes through the packed copy and the ingest kernel of the next `advance()`.  No host sync."""
-        self.scan_feeds.put(feed, points, n_valid)
+    def _check_detections(self, feed, detections):
+        """A put's detections, checked (ValueError) before anything is staged: None or the float32 (M, 16) rows."""
+        if detections is None:
+            return None
+        if self.detections is None:
+            raise ValueError("detections: this tracker was built without them; give detections=(max_per_scan, gate)")
+        self._feed(feed)
+        return check_detection_array(detections, self.detections[0])
 
-    def put_raw(self, feed, rows, transforms=()):
+    def _stage_detections(self, feed, rows):
+        if rows is not None:
+            self._det_staged[int(feed)] = rows
+
+    def put(self, feed, points, n_valid=None, detections=None):
+        """Stage the next scan of `feed` (ScanFeeds.put): a CUDA tensor is copied into the feed's next buffer at once, a host
+        tensor or array goes through the packed copy and the ingest kernel of the next `advance()`.  `detections`: the scan's
+        detections, (M, 16) rows (`detection_rows`), with `detections=` on.  No host sync."""
+        rows = self._check_detections(feed, detections)
+        self.scan_feeds.put(feed, points, n_valid)
+        self._stage_detections(feed, rows)
+
+    def put_raw(self, feed, rows, transforms=(), detections=None):
         """Stage the next scan of `feed` as a reader stores it (ScanFeeds.put_raw): the next `advance()` ingests it on the
-        device."""
+        device.  `detections` as for `put`."""
+        det = self._check_detections(feed, detections)
         self.scan_feeds.put_raw(feed, rows, transforms)
+        self._stage_detections(feed, det)
 
     def advance(self):
         """Bring in every staged scan and advance the active targets of those feeds to it, in one replay of the captured step;
@@ -668,16 +898,21 @@ class MultiTargetTracker:
         self.hit_c[k].zero_()
         self.hit_t[k].zero_()
         self.coasting[k].fill_(False)
+        if self.detections is not None:
+            self.detection[k].fill_(-1)
+            self.reacquired[k].fill_(False)
 
     def boxes(self):
         """Device state of the slots: ids (K,) int64 (-1 for an idle slot), center (K, 3), wlh (K, 3), rot (K, 3, 3), active (K,),
         and the evidence of each slot's last advance: points (K,) int32, score (K,) float32 (-1 / NaN before the first advance)
         and lost (K,) bool.  points and score are those of the network's box on every advance, also when the box reported is a
         coasted one (`coast=`): they describe the proposal that decided the miss.  coasting (K,) bool: the last advance was a
-        miss that moved the box along velocity (K, 3), the centre's displacement per advance (both views of the slot state)."""
+        miss that moved the box along velocity (K, 3), the centre's displacement per advance (both views of the slot state).
+        detection (K,) int32: the index of the detection the last advance matched in its feed's list (-1: none, and always
+        without `detections=`); reacquired (K,) bool: that advance was a miss re-acquired at its detection's box."""
         return {"ids": torch.where(self.active, self.key, torch.full_like(self.key, -1)), "center": self.box_c, "wlh": self.box_s,
                 "rot": self.box_r, "active": self.active, "points": self.points, "score": self.score, "lost": self.lost,
-                "coasting": self.coasting, "velocity": self.vel}
+                "coasting": self.coasting, "velocity": self.vel, "detection": self.detection, "reacquired": self.reacquired}
 
     def evidence(self):
         """A device copy of the slots' evidence, (K, 4) float32 = points in the box, score, consecutive misses, lost (0 / 1)."""
@@ -687,6 +922,37 @@ class MultiTargetTracker:
         """`snapshot()` and `evidence()` side by side, (K, 19), in one copy."""
         return torch.cat([self.box_c, self.box_s, self.box_r.reshape(self.K, 9), self.points.float()[:, None], self.score[:, None],
                           self.misses.float()[:, None], self.lost.float()[:, None]], 1)
+
+    def _match_record(self):
+        """(K, 2) float32: each slot's detection and reacquired flag, the block run_scenes reads back beside `_record()`."""
+        return torch.stack([self.detection.float(), self.reacquired.float()], 1)
+
+    def _detect_rows(self):
+        """Host flags over the rows of snapshot(): the row's tracker takes detections (detections=)."""
+        return np.full(self.K, self.detections is not None)
+
+    def unmatched(self):
+        """The detections of every feed's most recent fed advance that no target matched, read back from the device (one sync):
+        {feed: [(index in that advance's list, data_classes.Box, score), ...]}.  Start targets from them with `add()`."""
+        if self.detections is None:
+            raise ValueError("unmatched(): this tracker was built without detections=")
+        return self._unmatched_decode(self._unmatched_device().cpu().numpy())
+
+    def _unmatched_device(self):
+        """The feeds' detection records as one flat float32 device tensor: per feed D rows of 16, D slots, the count."""
+        F, D = self.F, self.D
+        return torch.cat([self._det_rec.view(F, D * 16), self._det_slot.float(), self._det_count.float()[:, None]], 1).view(-1)
+
+    def _unmatched_decode(self, flat):
+        from ..datasets.data_classes import Box
+        F, D = self.F, self.D
+        host = flat.reshape(F, D * 17 + 1)
+        out = {}
+        for f in range(F):
+            rec, slot = host[f, :D * 16].reshape(D, 16).astype(np.float64), host[f, D * 16:D * 17]
+            out[f] = [(d, Box(rec[d, 0:3], rec[d, 3:6], rec[d, 6:15].reshape(3, 3)), float(rec[d, 15]))
+                      for d in range(int(host[f, -1])) if slot[d] < 0]
+        return out
 
     def lost_targets(self):
         """Ids of the active targets the end-of-track rule has declared lost, read back from the device (one sync)."""
@@ -846,12 +1112,15 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
     `feed_schedule` planned.  Returns, per scene, {id: {t: data_classes.Box}}, and with `evidence`, per scene
     {id: {t: (points in the box, score)}} as well; a target of a coasting tracker (coast=) has (points, score, coasted) instead,
     coasted being whether that frame's box was coasted ((misses > 0) & ~lost: a coasting tracker's misses count is reset by
-    every hit)."""
+    every hit).  A scene may carry "detections": t -> the (M, 16) detections of its scan t (for a MultiClassTracker
+    {class: rows}), put with the scan when the tracker takes detections; a target of such a tracker has (reacquired, detection) appended to
+    its evidence: whether that frame re-acquired it at a detection and the index of the detection it matched (-1: none)."""
     from concurrent.futures import ThreadPoolExecutor
 
     from ..datasets.data_classes import Box
     scene_of, last = _scene_targets(scenes)
     coasts = trk._coast_rows()
+    detects = trk._detect_rows()
     lengths = [int(sc["frames"]) for sc in scenes]
     n_steps = max((s0 + lengths[i] for i, _, s0 in sched), default=0)
     work = [[] for _ in range(n_steps)]                                        # per step: (feed, scene, frame)
@@ -866,7 +1135,8 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
     pending, inflight = [], []
 
     def load(step):
-        return [(f, i, t, scenes[i]["scan"](t)) for f, i, t in work[step]]
+        return [(f, i, t, scenes[i]["scan"](t), scenes[i]["detections"](t) if "detections" in scenes[i] else None)
+                for f, i, t in work[step]]
 
     def read_back():                                                          # start a chunk's device -> host copy
         snaps = torch.stack([r[2] for r in pending])
@@ -890,7 +1160,8 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
                 i = scene_of[tid]
                 out[i].setdefault(tid, {})[s - first[i]] = Box(hs[k, 0:3], hs[k, 3:6], hs[k, 6:15].reshape(3, 3))
                 e = (int(hs[k, 15]), float(hs[k, 16]))
-                ev[i].setdefault(tid, {})[s - first[i]] = e + (bool(hs[k, 17] > 0 and hs[k, 18] == 0),) if coasts[k] else e
+                e = e + (bool(hs[k, 17] > 0 and hs[k, 18] == 0),) if coasts[k] else e
+                ev[i].setdefault(tid, {})[s - first[i]] = e + (bool(hs[k, 20] != 0), int(hs[k, 19])) if detects[k] else e
                 if hs[k, 18] != 0:
                     ended.add(tid)
 
@@ -900,19 +1171,21 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
             items = nxt.result()
             if s + 1 < n_steps:
                 nxt = pool.submit(load, s + 1)                               # read ahead while this step runs
-            for f, i, t, scan in items:
+            for f, i, t, scan, dets in items:
+                kw = {"detections": dets} if dets is not None and detects.any() else {}
                 if isinstance(scan, tuple):
-                    trk.put_raw(f, *scan)
+                    trk.put_raw(f, *scan, **kw)
                 else:
-                    trk.put(f, torch.as_tensor(scan))
+                    trk.put(f, torch.as_tensor(scan), **kw)
             trk.advance()
-            for f, i, t, _ in items:
+            for f, i, t, _, _ in items:
                 for tid, box in scenes[i]["starts"].get(t, ()):
                     add(tid, box, f)
             live = trk.targets()
             if live:
-                pending.append((s, live, trk._record()))
-            for f, i, t, _ in items:
+                # the detection block travels in the same read-back as the record, after its 19 columns
+                pending.append((s, live, torch.cat([trk._record(), trk._match_record()], 1) if detects.any() else trk._record()))
+            for f, i, t, _, _ in items:
                 for tid in last[i].get(t, ()):
                     if tid in live:
                         drop(tid)
@@ -928,7 +1201,7 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
 
 
 def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32", lost=None,
-                evidence=False, coast=None):
+                evidence=False, coast=None, detections=None):
     """Track many scenes through one tracker with `feeds` scan feeds (`feed_schedule` decides which scene runs when and where).
     `scenes`: [{"frames": number of scans, "scan": t -> the scene's scan t, either (rows, transforms) for `put_raw` or an (n, 3)
     tensor / array for `put`, "starts": {t: [(id, Box), ...]}, "ends": {id: last t}}]; a target without an end runs to its scene's
@@ -938,10 +1211,13 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
     `lost`: the tracker's end-of-track rule (MultiTargetTracker); a lost target's results end at the frame it was declared lost
     on.  With `evidence`, also returns, per scene, {id: {t: (points in the box, score)}} over the same frames.  `coast`: the
     tracker's coasting (MultiTargetTracker); results run on through coasted frames, and the evidence also says whether each frame
-    was coasted (run_scenes)."""
+    was coasted (run_scenes).  `detections`: the tracker's (max_per_scan, gate) (MultiTargetTracker); a scene's "detections":
+    t -> its scan t's (M, 16) detections, put with the scan (births stay the scene's "starts"), and the evidence also says
+    whether each frame was re-acquired at a detection, and which detection it matched (run_scenes)."""
     runtime.check_precision(precision)
     lost = check_lost_rule(lost)
     coast = check_coast(coast, lost)
+    detections = check_detections(detections)
     if max_points is None:
         raise ValueError("track_feeds: give max_points, the largest scan of the scenes")
     _scene_targets(scenes)
@@ -949,5 +1225,5 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
     peaks = [scene_peak(lengths[i], sc["starts"], sc["ends"]) for i, sc in enumerate(scenes)]
     sched = feed_schedule(lengths, peaks, feeds, max_targets)
     trk = MultiTargetTracker(model, max_points, max_targets, seed=seed, use_graph=use_graph, feeds=feeds, precision=precision,
-                             lost=lost, coast=coast)
+                             lost=lost, coast=coast, detections=detections)
     return run_scenes(trk, lambda tid, box, f: trk.add(tid, box, feed=f), trk.drop, scenes, sched, chunk, evidence)
