@@ -546,6 +546,64 @@ typedef struct o3d_box_associate_t {
 } o3d_box_associate_t;
 int o3d_box_associate(const o3d_box_associate_t* p, void* stream);
 
+/* Target births of the live tracker (tracking/multi_tracker.py birth_tensors, which it equals exactly), one CTA for every feed,
+ * run after o3d_box_associate and o3d_track_update in the same step.  The birth list holds R entries (birth_slot[e],
+ * birth_feed[e]): the slots the host reserved for this advance, grouped by ascending feed, padded with birth_feed = -1.  Feed
+ * f's entries are its r_f reserved slots in order.  For every feed with r_f > 0, fed[f] != 0 and count[f] > 0, detection
+ * d < count[f] of det[f] is a candidate when rec_slot[f, d] < 0 (o3d_box_associate left it unmatched), its score det[f, d, 15]
+ * >= min_score, and d2 > gate2 to the pred centre of every row i < b with feed[i] == f and adv[i] (d2 = dx*dx + dy*dy over the
+ * plane axes, dx = pred - det, each operation rounded on its own).  The candidates are ranked by descending score (-0 as +0),
+ * then ascending d, and walked in rank order: a candidate whose d2 (candidate minus born) to a candidate already born from
+ * this feed is <= gate2 is passed over; otherwise it is born into the feed's next reserved slot; the walk ends when the slots
+ * run out.  The n-th birth of the call (feeds ascending, then rank) gets id = id_base + next + n, and next grows by the births.
+ * A birth at entry e, slot k, detection d writes the slot state add(id, box, feed=f) writes (box from the row: centre, wlh,
+ * row-major rotation; first_flag 1, active 1, key id, t 0, slot_feed f, points -1, score NaN, misses 0, lost 0, vel 0,
+ * hit_c = centre, hit_t 0, coasting 0, detection -1, reacquired 0), rec_slot[f, d] <- k and log[e] = (k, id, f, d); every
+ * other log entry is (-1, -1, -1, -1).  The first-frame crop is the caller's.  No atomics, no host sync, capturable.
+ * Refused: a null descriptor or pointer (feed / adv / pred may be null when b = 0), b outside 0 .. 65535, F < 1, D outside
+ * 1 .. 1024, R outside 1 .. 65535, gate2 not finite or <= 0, min_score not finite, axis0 / axis1 not distinct values in
+ * {0, 1, 2}, id_base < 0. */
+typedef struct o3d_track_birth_t {
+    int b;                     /* rows of the step (0: a step that advances no row) */
+    int F;                     /* feeds */
+    int D;                     /* detections per feed, at most (the row stride of det / rec_slot) */
+    int R;                     /* birth list entries */
+    int axis0, axis1;          /* the plane the distance is measured in */
+    float gate2;               /* squared gate, float32 */
+    float min_score;
+    long long id_base;         /* the first born id */
+    const long long* feed;     /* [b] feed of each row */
+    const unsigned char* adv;  /* [b] */
+    const float* pred;         /* [b, 3] o3d_box_associate's pred */
+    const long long* fed;      /* [F] */
+    const int* count;          /* [F] */
+    const float* det;          /* [F, D, 16] */
+    int* rec_slot;             /* [F, D] the matching's records, updated for the born detections */
+    const long long* birth_slot;   /* [R] */
+    const long long* birth_feed;   /* [R] */
+    long long* next;           /* [1] births so far */
+    long long* log;            /* [R, 4] out */
+    float* box_c;              /* slot state, as o3d_track_update's */
+    float* box_s;
+    float* box_r;
+    float* first_flag;
+    unsigned char* active;
+    long long* key;
+    long long* t;
+    long long* slot_feed;
+    int* points;
+    float* score;
+    int* misses;
+    unsigned char* lost;
+    float* vel;
+    float* hit_c;
+    long long* hit_t;
+    unsigned char* coasting;
+    int* detection;
+    unsigned char* reacquired;
+} o3d_track_birth_t;
+int o3d_track_birth(const o3d_track_birth_t* p, void* stream);
+
 /* Block 6 — split evaluation with K tracklets in flight (tracking/batched_tracker.py).
  *
  * o3d_keyed_uniform: out [K, n] uniform [0, 1) draws of one stream.  Slot k's element e is a pure function of

@@ -65,6 +65,7 @@ PROTOTYPES = {
     "o3d_box_points": [_p, _p, _p, _p, _p, _p, _i, _i, _p, _p],
     "o3d_track_update": [_p, _p],
     "o3d_box_associate": [_p, _p],
+    "o3d_track_birth": [_p, _p],
     "o3d_lift_stats": [_p, _i, _i, _p, _p, _p, _p, _p],
     "o3d_lift_scatter": [_p, _i, _i, _p, _p, _p, _i, _p, _p, _p, _p],
     "o3d_pw_fwd_tc_lift": [_p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _p, _i, _p, _p, _i, _p, _p, _p, _i, _p],
@@ -128,6 +129,15 @@ class AssociateDesc(ctypes.Structure):
                [(n, _i) for n in ("rule", "min_points", "coast")] + \
                [(n, _p) for n in ("src", "feed", "adv", "center", "points", "t", "hit_t", "hit_c", "vel", "fed", "count", "det",
                                   "pred", "match", "match_box", "rec_det", "rec_count", "rec_slot")]
+
+
+class BirthDesc(ctypes.Structure):
+    """ctypes mirror of `o3d_track_birth_t` (include/o3d_b200.h)."""
+    _fields_ = [(n, _i) for n in ("b", "F", "D", "R", "axis0", "axis1")] + [("gate2", _f), ("min_score", _f),
+                                                                         ("id_base", ctypes.c_longlong)] + \
+               [(n, _p) for n in ("feed", "adv", "pred", "fed", "count", "det", "rec_slot", "birth_slot", "birth_feed", "next",
+                                  "log", "box_c", "box_s", "box_r", "first_flag", "active", "key", "t", "slot_feed", "points",
+                                  "score", "misses", "lost", "vel", "hit_c", "hit_t", "coasting", "detection", "reacquired")]
 
 
 # o3d_stack_t.precision: 3xTF32 (default), BF16 inference (eval mode only), BF16 training (training mode only)

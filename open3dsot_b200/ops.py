@@ -422,6 +422,47 @@ def box_associate(src, feed, adv, center, points, slots, fed, count, det, record
     return pred, match, match_box
 
 
+# slot state a birth writes, in o3d_track_birth_t's order: (attribute, dtype, values per row)
+BIRTH_SLOTS = (("box_c", torch.float32, 3), ("box_s", torch.float32, 3), ("box_r", torch.float32, 9),
+               ("first_flag", torch.float32, 1), ("active", torch.bool, 1), ("key", torch.int64, 1), ("t", torch.int64, 1),
+               ("slot_feed", torch.int64, 1), ("points", torch.int32, 1), ("score", torch.float32, 1), ("misses", torch.int32, 1),
+               ("lost", torch.bool, 1), ("vel", torch.float32, 3), ("hit_c", torch.float32, 3), ("hit_t", torch.int64, 1),
+               ("coasting", torch.bool, 1), ("detection", torch.int32, 1), ("reacquired", torch.bool, 1))
+
+
+def track_birth(feed, adv, pred, fed, count, det, rec_slot, birth_list, next_id, log, slots, gate2, axes, min_score, id_base):
+    """Start targets from each feed's unmatched detections in one kernel (csrc/track_birth.cu, one CTA): feed (b,) int64, adv
+    (b,) bool, pred (b, 3) float32 from `box_associate`; fed (F,) int64, count (F,) int32, det (F, D, 16) float32, rec_slot (F,
+    D) int32 (updated for the born detections); birth_list (2, R) int64: reserved slots and their feeds (-1: padding); next_id
+    (1,) int64, the births so far (advanced); log (R, 4) int64 out; `slots`: an object with the BIRTH_SLOTS attributes,
+    contiguous CUDA tensors of the same number of rows.  `gate2` / `min_score`: float32 values.  Exactly
+    `tracking.multi_tracker.birth_tensors`."""
+    b = adv.shape[0]
+    rows = slots.box_c.shape[0]
+    for name, dtype, n in BIRTH_SLOTS:
+        t = getattr(slots, name)
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dtype or not t.is_contiguous() \
+                or t.shape[0] != rows or t.numel() != rows * n:
+            raise RuntimeError(f"track_birth: slot state {name} must be a contiguous {dtype} CUDA tensor of {rows} x {n}")
+    for t, name in ((feed, "feed"), (fed, "fed"), (birth_list, "birth_list"), (next_id, "next_id"), (log, "log")):
+        _chk_i64(t, name)
+    _chk_f(pred, "pred")
+    _chk_f(det, "det")
+    _chk_i(count, "count")
+    _chk_i(rec_slot, "rec_slot")
+    if not adv.is_cuda or adv.dtype != torch.bool or not adv.is_contiguous():
+        raise RuntimeError("adv must be a contiguous bool CUDA tensor")
+    F, D, n = det.shape
+    R = birth_list.shape[1]
+    assert n == DETECTION_VALUES and feed.shape == (b,) and pred.shape == (b, 3) and fed.shape == count.shape == (F,)
+    assert rec_slot.shape == (F, D) and birth_list.shape == (2, R) and next_id.shape == (1,) and log.shape == (R, 4)
+    d = _lib.BirthDesc(b, F, D, R, int(axes[0]), int(axes[1]), float(gate2), float(min_score), int(id_base),
+                       *(t.data_ptr() for t in (feed, adv, pred, fed, count, det, rec_slot, birth_list[0], birth_list[1], next_id,
+                                                log)),
+                       *(getattr(slots, name).data_ptr() for name, _, _ in BIRTH_SLOTS))
+    _call("o3d_track_birth", ctypes.byref(d), _stream())
+
+
 # ------------------------------------------------------------------ scan ingest for the live tracker's feeds (csrc/scan_ingest.cu)
 # o3d_scan_desc_t, field for field
 SCAN_DESC = np.dtype([("offset", "<i8"), ("rows", "<i4"), ("stride", "<i4"), ("is_f64", "<i4"), ("feed", "<i4"), ("half", "<i4"),

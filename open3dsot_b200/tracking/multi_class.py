@@ -18,8 +18,8 @@ import torch
 from .. import runtime
 import numpy as np
 
-from .multi_tracker import (MultiTargetTracker, ScanFeeds, check_coast, check_detections, check_lost_rule, class_peaks,
-                            feed_schedule, run_scenes)
+from .multi_tracker import (MultiTargetTracker, ScanFeeds, check_births, check_coast, check_detections, check_lost_rule,
+                            class_peaks, feed_schedule, refuse_births, run_scenes)
 
 SHARED_KEYS = ("up_axis", "IoU_space", "degrees")
 
@@ -30,12 +30,14 @@ class MultiClassTracker:
     class; `lost` is one end-of-track rule for every class (MultiTargetTracker's `lost=`) or {class: rule}, a class without an
     entry never losing a target; `coast` likewise one alpha (MultiTargetTracker's `coast=`) or {class: alpha}, a class without
     an entry never coasting (a class that coasts needs a rule); `detections` likewise one (max_per_scan, gate) or
-    {class: (max_per_scan, gate)}, a class without an entry taking no detections.  `put` / `put_raw` / `advance()` as on
+    {class: (max_per_scan, gate)}, a class without an entry taking no detections; `births` likewise one (min_score, per_scan) or
+    {class: (min_score, per_scan)}, a class without an entry starting no target itself (a class with births needs detections),
+    and `births()` returns {class: MultiTargetTracker.births()} of those classes.  `put` / `put_raw` / `advance()` as on
     MultiTargetTracker, with a scan's detections given per class ({class: rows}); `add(cls, id, box, feed=)` / `drop(cls, id)`
     start and end a target of a class."""
 
     def __init__(self, models, max_points, max_targets, feeds=1, seed=0, use_graph=True, precision="fp32", lost=None, coast=None,
-                 detections=None):
+                 detections=None, births=None):
         if not models:
             raise ValueError("MultiClassTracker: no classes; give one model per class")
         self.precision = runtime.check_precision(precision)
@@ -69,6 +71,15 @@ class MultiClassTracker:
                 dets[n] = check_detections(dets.get(n))
             except ValueError as e:
                 raise ValueError(f"class {n!r}: {e}") from None
+        born = births if isinstance(births, dict) else {n: births for n in names}
+        for n in born:
+            if n not in models:
+                raise ValueError(f"births: class {n!r} has no model")
+        for n in names:
+            try:
+                born[n] = check_births(born.get(n), dets[n])
+            except ValueError as e:
+                raise ValueError(f"class {n!r}: {e}") from None
         c0 = models[names[0]].config
         for n in names[1:]:
             c = models[n].config
@@ -86,7 +97,7 @@ class MultiClassTracker:
             try:
                 self.trackers[n] = MultiTargetTracker(models[n], max_points, max_targets[n], seed=seed, use_graph=use_graph,
                                                       feeds=self.scan_feeds, precision=precision, lost=rules[n], coast=coasts[n],
-                                                      detections=dets[n])
+                                                      detections=dets[n], births=born[n])
             except ValueError as e:
                 self.scan_feeds.owner = None
                 raise ValueError(f"class {n!r}: {e}") from None
@@ -211,6 +222,13 @@ class MultiClassTracker:
             at += flat.numel()
         return out
 
+    def births(self, wait=False):
+        """{class: [(id, feed, slot, detection index), ...]}: MultiTargetTracker.births(wait) of every class built with births=."""
+        classes = [n for n, trk in self.trackers.items() if trk.birth_rule is not None]
+        if not classes:
+            raise ValueError("births(): no class was built with births=")
+        return {n: self.trackers[n].births(wait) for n in classes}
+
     def lost_targets(self):
         """(class, id) of the active targets their class's rule has declared lost, read back from the device (one sync)."""
         lost = torch.cat([trk.lost for trk in self.trackers.values()]).cpu().numpy()
@@ -231,7 +249,7 @@ class MultiClassTracker:
 
 
 def track_classes(models, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32",
-                  lost=None, evidence=False, coast=None, detections=None):
+                  lost=None, evidence=False, coast=None, detections=None, births=None):
     """`track_feeds` for several classes through one MultiClassTracker.  `models` and `max_targets`: {class: model},
     {class: slots}.  A scene's targets are named (class, id): "starts": {t: [((class, id), Box), ...]}, "ends": {(class, id):
     last t}; (class, id) is unique over all scenes.  A scene is admitted when a feed is free and every class has the scene's
@@ -240,7 +258,9 @@ def track_classes(models, scenes, feeds, max_targets, seed=0, max_points=None, u
     returns, per scene, {(class, id): {t: (points in the box, score)}}, with a third value, whether the frame was coasted, for
     the classes that coast (`coast`: one alpha or {class: alpha}, MultiClassTracker).  `detections`: one (max_per_scan, gate) or
     {class: (max_per_scan, gate)} (MultiClassTracker); a scene's "detections": t -> {class: rows} of its scan t, and the
-    evidence of the classes that take detections ends with (reacquired, detection) (run_scenes)."""
+    evidence of the classes that take detections ends with (reacquired, detection) (run_scenes).  `births` is refused, as by
+    track_feeds."""
+    refuse_births(births, "track_classes")
     runtime.check_precision(precision)
     if max_points is None:
         raise ValueError("track_classes: give max_points, the largest scan of the scenes")

@@ -44,6 +44,16 @@ Detections.  With `detections=(max_per_scan, gate)` a scan may come with a 3D de
 step matches each feed's detections to its advancing rows greedily by plane distance to the centre the row would write without
 them (`o3d_box_associate`, csrc/associate.cu, one launch before the write-back); a matched miss is re-acquired at its
 detection's box, and every feed keeps its most recent advance's detections with the slot each matched, for `unmatched()`.
+Births.  With `births=(min_score, per_scan)` as well, the step also starts targets on the device (`o3d_track_birth`,
+csrc/track_birth.cu, one launch after the write-back): per fed feed, the detections the matching left unmatched, scoring at least
+min_score and beyond the gate of every row that took part in it, are walked by descending score (ties by index) and born into
+the slots the host reserved for the feed this advance, skipping one within the gate of a detection already born, until the
+slots run out.  A birth writes what `add()` writes for the detection's box, including the first-frame crop, with id
+BIRTH_ID_BASE + n.  The host reserves up to per_scan of the lowest free slots per feed that staged detections (they travel in the
+advance's one upload) and runs the reserved slots in later work lists, where an unborn one holds; the step's birth log is read
+back without blocking and resolved BIRTH_LAG advances later (`births()`), when the born targets join `targets()` and the unborn
+reservations are freed.  An advance with reservations and no target to step replays a captured birth-only step.  The host's
+state therefore changes at points fixed by the calls alone, however far the device lags.
 Device memory: feeds * 2 * max_points * 12 bytes of scans, plus per slot the crop scratch and, for the first-frame template
 modes, max_points * 13 bytes of first-frame crop.  Ground-truth reference boxes (reference_BB 'previous_gt' / 'current_gt') have no meaning on a live stream, and
 shape_aggregation 'all' is not supported here; both are refused."""
@@ -315,6 +325,127 @@ def associate(src, feed, adv, center, points, slots, fed, count, det, records, g
     return associate_tensors(src, feed, adv, center, points, slots, fed, count, det, records, gate2, axes, rule, coast)
 
 
+# Born targets' ids: BIRTH_ID_BASE + n for the n-th birth of the tracker.  Draws are keyed by (uint32) id, so born ids never share
+# draws with the ids add() takes (0 .. BIRTH_ID_BASE - 1 on a tracker with births).
+BIRTH_ID_BASE = 2 ** 31
+# The births of advance i are read back (and their targets join the host's maps) at the start of advance i + BIRTH_LAG
+BIRTH_LAG = 2
+
+
+def check_births(births, detections):
+    """`births=`: None (targets start only through add()) or (min_score, per_scan): a finite score and an int with 1 <= per_scan
+    <= max_per_scan.  Births start from detections, so they need `detections` (checked, or None).  Returns (min_score as a
+    float32 value, per_scan) or None."""
+    if births is None:
+        return None
+    try:
+        min_score, per_scan = births
+    except (TypeError, ValueError):
+        raise ValueError(f"births={births!r}: expected None or (min_score, per_scan)") from None
+    if detections is None:
+        raise ValueError("births: targets are born from unmatched detections; give detections=(max_per_scan, gate) too")
+    if isinstance(min_score, bool) or not isinstance(min_score, (int, float, np.integer, np.floating)) \
+            or not math.isfinite(min_score) or not abs(min_score) <= float(np.finfo(np.float32).max):
+        raise ValueError(f"births: min_score={min_score!r} must be a finite number")
+    if isinstance(per_scan, bool) or not isinstance(per_scan, (int, np.integer)) or not 1 <= per_scan <= detections[0]:
+        raise ValueError(f"births: per_scan={per_scan!r} must be an integer in 1 .. max_per_scan={detections[0]}")
+    return float(np.float32(min_score)), int(per_scan)
+
+
+def refuse_births(births, name):
+    """track_feeds / track_classes plan every scene's slots from its annotated starts; a birth would take a slot they gave out."""
+    if births is not None:
+        raise ValueError(f"{name}: births= is not supported; the feed schedule reserves each scene's slots from its annotated "
+                         f"starts, so targets start from the scenes' \"starts\" only")
+
+
+class BirthSlots(NamedTuple):
+    """The per-slot state a birth writes (ops.BIRTH_SLOTS, in its order); rows are slots."""
+    box_c: torch.Tensor        # (R, 3) float32
+    box_s: torch.Tensor        # (R, 3) float32
+    box_r: torch.Tensor        # (R, 3, 3) float32
+    first_flag: torch.Tensor   # (R,) float32
+    active: torch.Tensor       # (R,) bool
+    key: torch.Tensor          # (R,) int64
+    t: torch.Tensor            # (R,) int64
+    slot_feed: torch.Tensor    # (R,) int64
+    points: torch.Tensor       # (R,) int32
+    score: torch.Tensor        # (R,) float32
+    misses: torch.Tensor       # (R,) int32
+    lost: torch.Tensor         # (R,) bool
+    vel: torch.Tensor          # (R, 3) float32
+    hit_c: torch.Tensor        # (R, 3) float32
+    hit_t: torch.Tensor        # (R,) int64
+    coasting: torch.Tensor     # (R,) bool
+    detection: torch.Tensor    # (R,) int32
+    reacquired: torch.Tensor   # (R,) bool
+
+
+def birth_tensors(feed, adv, pred, fed, count, det, rec_slot, birth_list, next_id, log, slots, gate2, axes, min_score,
+                  id_base=BIRTH_ID_BASE):
+    """The formulation of the step's target births (`ops.track_birth`, csrc/track_birth.cu), which it equals exactly.  The
+    birth list (2, R) holds the slots reserved for this advance and their feeds (-1: padding), grouped by ascending feed.  Per
+    feed f with reserved slots, fed, with detections det[f, :count[f]]: a detection is a candidate when the matching left it
+    unmatched (rec_slot[f, d] < 0), its score (column 15) >= min_score, and its squared plane distance d2 = dx*dx + dy*dy to
+    pred[i] is > gate2 for every row i of feed f with adv[i] (the rows that took part in the matching).  The candidates are
+    walked by descending score, then ascending index; one within gate2 of a candidate already born from the feed is passed
+    over, the others are born into the feed's reserved slots in order until they run out.  The n-th birth (feeds ascending,
+    then rank) gets id = id_base + next_id + n.  A birth writes the slot state add(id, box, feed=f) writes (`slots`, a
+    BirthSlots; the first-frame crop is the caller's), rec_slot[f, d] = its slot and log[e] = (slot, id, f, d) at its birth list
+    entry e; every other log entry is -1.  next_id grows by the births."""
+    a0, a1 = axes
+    gate2 = np.float32(gate2)
+    feed_h, adv_h, fed_h, count_h = (x.cpu().numpy() for x in (feed, adv, fed, count))
+    pred_h, det_h, rec_h = pred.cpu().numpy(), det.cpu().numpy(), rec_slot.cpu().numpy()
+    bslot, bfeed = birth_list.cpu().numpy()
+    d2 = lambda ax, ay, bx_, by: (ax - bx_) * (ax - bx_) + (ay - by) * (ay - by)
+    n0 = int(next_id[0])
+    out = np.full((birth_list.shape[1], 4), -1, np.int64)
+    born = []                                                                 # (entry, slot, id, feed, detection)
+    for f in range(det_h.shape[0]):
+        entries = np.flatnonzero(bfeed == f)
+        nd = int(count_h[f]) if fed_h[f] else 0
+        if not len(entries) or not nd:
+            continue
+        q = det_h[f, :nd]
+        rows = np.flatnonzero(adv_h & (feed_h == f))
+        near = (d2(pred_h[rows, a0][:, None], pred_h[rows, a1][:, None], q[None, :, a0], q[None, :, a1]) <= gate2).any(0)
+        cand = np.flatnonzero((rec_h[f, :nd] < 0) & (q[:, 15] >= np.float32(min_score)) & ~near)
+        kept = []
+        for d in cand[np.lexsort((cand, -q[cand, 15]))]:
+            if len(kept) == len(entries):
+                break
+            if any(d2(q[d, a0], q[d, a1], q[e, a0], q[e, a1]) <= gate2 for e in kept):
+                continue
+            kept.append(int(d))
+        for e, d in zip(entries, kept):
+            born.append((e, int(bslot[e]), id_base + n0 + len(born), f, d))
+    for e, k, tid, f, d in born:
+        out[e] = (k, tid, f, d)
+        row = det[f, d]
+        slots.box_c[k] = row[0:3]
+        slots.box_s[k] = row[3:6]
+        slots.box_r[k] = row[6:15].view(3, 3)
+        slots.hit_c[k] = row[0:3]
+        for name, v in (("first_flag", 1.0), ("active", True), ("key", tid), ("t", 0), ("slot_feed", f), ("points", -1),
+                        ("score", float("nan")), ("misses", 0), ("lost", False), ("vel", 0.0), ("hit_t", 0), ("coasting", False),
+                        ("detection", -1), ("reacquired", False)):
+            getattr(slots, name)[k].fill_(v)
+        rec_slot[f, d] = k
+    log.copy_(torch.from_numpy(out))
+    next_id += len(born)
+
+
+def track_birth(feed, adv, pred, fed, count, det, rec_slot, birth_list, next_id, log, slots, gate2, axes, min_score):
+    """The step's target births (`birth_tensors`): CUDA tensors through one `o3d_track_birth` launch (csrc/track_birth.cu),
+    other tensors through the formulation."""
+    if fed.is_cuda:
+        ops.track_birth(feed, adv, pred.contiguous(), fed, count, det, rec_slot, birth_list, next_id, log, slots, gate2, axes,
+                        min_score, BIRTH_ID_BASE)
+    else:
+        birth_tensors(feed, adv, pred, fed, count, det, rec_slot, birth_list, next_id, log, slots, gate2, axes, min_score)
+
+
 def _box_values(box):
     """(center, wlh, 3x3 rotation) as float64 numpy arrays from a data_classes.Box or a tracking.boxes.Box."""
     if isinstance(box, bx.Box):
@@ -504,15 +635,19 @@ class MultiTargetTracker:
     alpha-weighted average of its centre's displacement per advance between hits, instead of writing the network's box.
     `detections`: None or (max_per_scan, gate): `put` / `put_raw` then take each scan's detections, (M, 16) rows
     (`detection_rows`), matched on the device to the targets of their feed within `gate` metres in the plane orthogonal to the
-    config's up_axis; a matched miss is re-acquired at its detection, and `unmatched()` lists the detections no target took."""
+    config's up_axis; a matched miss is re-acquired at its detection, and `unmatched()` lists the detections no target took.
+    `births`: None or (min_score, per_scan) (needs `detections`): the step starts a target from each unmatched detection scoring
+    at least min_score beyond the gate of the feed's targets, at most per_scan per feed and advance, into slots the host
+    reserves; `births()` lists them BIRTH_LAG advances later, without a sync."""
 
     def __init__(self, model, max_points, max_targets, seed=0, use_graph=True, feeds=1, precision="fp32", lost=None, coast=None,
-                 detections=None):
+                 detections=None, births=None):
         self.precision = runtime.check_precision(precision)
         self.lost_rule = check_lost_rule(lost)
         self.coast = check_coast(coast, self.lost_rule)
         self._coast = coast_weights(self.coast)
         self.detections = check_detections(detections)
+        self.birth_rule = check_births(births, self.detections)
         self.model = model.eval()
         self.cfg = cfg = model.config
         self.dev = dev = next(model.parameters()).device
@@ -577,17 +712,20 @@ class MultiTargetTracker:
         self.detection, self.reacquired = self._detection[:K], self._reacquired[:K]
         self._match_slots = MatchSlots(self._detection, self._reacquired)
         # The work list of the next bucket step, (2, K) as work_rows() lays it out; one host->device copy per advance.  With
-        # detections the same copy brings each feed's detection count and rows: [work | counts (F,) int32 | rows (F, D, 16)].
+        # detections the same copy brings each feed's detection count and rows: [work | counts (F,) int32 | rows (F, D, 16)],
+        # and with births the birth list after the work list: [work | birth list (2, R) int64 | counts | rows].
         if self.detections is None:
             self._work = torch.zeros(2, K, **i64)
         else:
             D = self.D = self.detections[0]
             self._gate2 = detection_gate2(self.detections[1])
             self._axes = plane_axes(cfg.up_axis)
-            self._det_at = 16 * K + -(-4 * F // 16) * 16
+            R = self.R = 0 if self.birth_rule is None else min(K, self.birth_rule[1] * F)
+            self._n_at = 16 * K + 16 * R
+            self._det_at = self._n_at + -(-4 * F // 16) * 16
             self._upload = torch.zeros(self._det_at + F * D * 64, device=dev, dtype=torch.uint8)
             self._work = self._upload[:16 * K].view(torch.int64).view(2, K)
-            self._det_n = self._upload[16 * K:16 * K + 4 * F].view(torch.int32)
+            self._det_n = self._upload[self._n_at:self._n_at + 4 * F].view(torch.int32)
             self._det_in = self._upload[self._det_at:].view(torch.float32).view(F, D, 16)
             self._det_staged = {}                         # feed -> (M, 16) float32 rows for the next advance
             # per feed, its most recent fed advance's detections, their count and the slot each matched (-1: none)
@@ -599,6 +737,22 @@ class MultiTargetTracker:
             self._first_local = torch.zeros(K + 2, N, 3, **f)
             self._first_keep = torch.zeros(K + 2, N, dtype=torch.bool, device=dev)
             self.first_local, self.first_keep = self._first_local[:K], self._first_keep[:K]
+        if self.birth_rule is not None:
+            # Births (births=): the advance's birth list (reserved slots and their feeds, padded with (K, -1)) in the upload, the
+            # births so far (the id counter), the step's birth log, and a ring of host buffers the logs are read back into
+            self._birth_list = self._upload[16 * K:16 * K + 16 * R].view(torch.int64).view(2, R)
+            self._birth_next = torch.zeros(1, **i64)
+            self._birth_log = torch.full((R, 4), -1, **i64)
+            self._birth_slots = BirthSlots(self._box_c, self._box_s, self._box_r, self._first_flag, self._active, self._key, self._t,
+                                           self._slot_feed, self._points, self._score, self._misses, self._lost, self._vel,
+                                           self._hit_c, self._hit_t, self._coasting, self._detection, self._reacquired)
+            self._birth_ring = [torch.empty(R, 4, dtype=torch.int64, pin_memory=dev.type == "cuda") for _ in range(BIRTH_LAG + 1)]
+            self._advances = 0                            # advances run
+            self._pending = {}                            # reserved slot -> feed, until its advance is resolved
+            self._birth_queue = []                        # (advance, [(slot, feed)], host log, event) not yet resolved
+            self._born = []                               # resolved births not yet returned by births()
+            self._reserved = 0                            # rows reserved so far: a bound on the births, hence on the ids
+            self._birth_graph = None
         self.slot_of = {}                                 # target id -> slot
         self._feed_of = {}                                # slot -> feed of the active targets (host mirror of slot_feed)
         self._buckets = None                              # the step sizes (occupancy_buckets), fixed on the first advance
@@ -675,12 +829,14 @@ class MultiTargetTracker:
                                     bx.inclusive_half(new.wlh, EVIDENCE_WLH_FACTOR))
             match = None
             if self.detections is not None:
-                _, m, m_box = associate(self._work[0, :b], r["feed"], r["adv"], new.center, points, self._slots, self.fstate[0],
+                pred, m, m_box = associate(self._work[0, :b], r["feed"], r["adv"], new.center, points, self._slots, self.fstate[0],
                                         self._det_n, self._det_in, (self._det_rec, self._det_count, self._det_slot), self._gate2,
                                         self._axes, self.lost_rule, self._coast is not None)
                 match = (m, m_box) + tuple(self._match_slots)
             track_update(self._slots, self._work[0, :b], dst, r["adv"], new.center, new.rot, points, score, self.lost_rule,
                          self._coast, match)
+            if self.birth_rule is not None:
+                self._birth_stage(r["feed"], r["adv"], pred)
 
     def _gather(self, b):
         """The state of the first `b` rows of the work list: (rows {cur, prev, key, t, first_flag, adv[, first]}, box, the rows
@@ -698,11 +854,42 @@ class MultiTargetTracker:
         box = bx.Box(self._box_c.index_select(0, src), self._box_s.index_select(0, src), self._box_r.index_select(0, src))
         return r, box, dst
 
+    def _birth_stage(self, feed, adv, pred):
+        """Start targets from the fed feeds' unmatched detections into the slots the birth list reserves (`track_birth`), then
+        take each born target's first-frame crop from its feed's current scan, as add() does, over the R entries of the list
+        (unborn entries write row K + 1, which nothing reads)."""
+        track_birth(feed, adv, pred, self.fstate[0], self._det_n, self._det_in, self._det_slot, self._birth_list, self._birth_next,
+                    self._birth_log, self._birth_slots, self._gate2, self._axes, self.birth_rule[0])
+        if self.mode in ("firstandprevious", "first"):
+            cfg = self.cfg
+            born = self._birth_log[:, 3] >= 0
+            dst = torch.where(born, self._birth_log[:, 0], torch.full_like(self._birth_log[:, 0], self.K + 1))
+            f = self._birth_list[1].clamp(min=0)
+            cur = self.fstate[1][f]
+            b = bx.Box(self._box_c.index_select(0, dst), self._box_s.index_select(0, dst), self._box_r.index_select(0, dst))
+            local, keep, _ = bx.crop_and_center(self.scans[f, cur], b, offset=cfg.model_bb_offset, scale=cfg.model_bb_scale)
+            self._first_local.index_copy_(0, dst, local)
+            self._first_keep.index_copy_(0, dst, keep & (self.arange[None] < self.count[f, cur][:, None]))
+
+    def _birth_only_step(self):
+        """An advance that steps no target but has slots reserved for births: record the fed feeds' detections, all unmatched,
+        and run the birth stage."""
+        with torch.no_grad():
+            self._record_unmatched()
+            none = self._work[0, :0]
+            self._birth_stage(none, none.bool(), self._det_in.new_zeros(0, 3))
+
     def _state(self):
         """The slot state a step writes (what the warm-up before a capture must put back)."""
         if self.detections is None:
             return tuple(self._slots)
-        return tuple(self._slots) + tuple(self._match_slots) + (self._det_rec, self._det_count, self._det_slot)
+        state = tuple(self._slots) + tuple(self._match_slots) + (self._det_rec, self._det_count, self._det_slot)
+        if self.birth_rule is None:
+            return state
+        state += (self._box_s, self._active, self._key, self._slot_feed, self._birth_next, self._birth_log)
+        if self.mode in ("firstandprevious", "first"):
+            state += (self._first_local, self._first_keep)
+        return state
 
     def _plan(self):
         """First advance: the bucket sizes, from the row counts of the network's stacks in one step over all K slots (its
@@ -721,6 +908,8 @@ class MultiTargetTracker:
             pool = torch.cuda.graph_pool_handle()
             for b in sorted(self._buckets, reverse=True):
                 self.graphs[b] = capture_step(lambda b=b: self._step(b), self._state(), pool)
+            if self.birth_rule is not None:
+                self._birth_graph = capture_step(self._birth_only_step, self._state(), pool)
         else:
             # one step at every bucket size (its writes put back), so that the prepared weight blocks of every row count are
             # built, and synchronise, here rather than on the first advance that reaches that size
@@ -734,7 +923,14 @@ class MultiTargetTracker:
         """Advance the active targets of the feeds in `fed` to the scans the feed store has just brought in: upload the work list
         and replay the captured step of its bucket (or run the eager step at that size).  The first call fixes the buckets and
         captures every bucket's step, so that later calls never synchronise."""
-        slots = work_slots(self._feed_of, fed)
+        if self.birth_rule is None:
+            slots, reserved = work_slots(self._feed_of, fed), []
+        else:
+            self._resolve(self._advances - BIRTH_LAG)
+            # pending slots advance like targets: a slot born on the device advances, an unborn one holds
+            slots = work_slots({**self._feed_of, **self._pending}, fed)
+            reserved = self._reserve(fed)
+            self._advances += 1
         first = self._buckets is None or (self.use_graph and not self.graphs)
         detect = self.detections is not None and bool(fed)
         if not slots and not first and not detect:
@@ -745,30 +941,85 @@ class MultiTargetTracker:
             # a fresh pinned buffer for every advance: it is not rewritten before its copy runs
             self._work.copy_(w.pin_memory() if self.dev.type == "cuda" else w, non_blocking=True)
         else:
-            self._upload_with_detections(w, fed)
+            self._upload_with_detections(w, fed, reserved)
         if first:
             self._plan()
         if not slots:
-            if detect:
+            if reserved:
+                if self.use_graph:
+                    self._birth_graph.replay()
+                else:
+                    self._birth_only_step()
+            elif detect:
                 self._record_unmatched()
-            return
-        b = bucket_for(len(slots), self._buckets)
-        if self.use_graph:
-            self.graphs[b].replay()
         else:
-            self._step(b)
+            b = bucket_for(len(slots), self._buckets)
+            if self.use_graph:
+                self.graphs[b].replay()
+            else:
+                self._step(b)
+        if reserved:
+            self._read_births(reserved)
 
-    def _upload_with_detections(self, w, fed):
-        """One host->device copy of the work list `w` and the staged detections of the feeds in `fed` (a fed feed staged without
-        detections has none), from a fresh pinned buffer; only the bytes up to the last staged row are copied."""
+    def _reserve(self, fed):
+        """This advance's birth reservations: for each fed feed in ascending order that staged M > 0 detections, the lowest
+        min(per_scan, M, free) free slots (free: neither a target's nor pending).  [(slot, feed)]; they become pending."""
+        taken = set(self.slot_of.values()) | set(self._pending)
+        free = [k for k in range(self.K) if k not in taken]
+        out = []
+        for f in sorted(fed):
+            n = min(self.birth_rule[1], len(self._det_staged.get(f, ())), len(free) - len(out))
+            out += [(free[len(out) + j], f) for j in range(n)]
+        if self._reserved + len(out) > 2 ** 32 - BIRTH_ID_BASE:
+            raise RuntimeError(f"births: {self._reserved} rows reserved so far; another {len(out)} could take born ids past "
+                               f"2**32, where the draws' (uint32) keys would repeat")
+        self._reserved += len(out)
+        self._pending.update(out)
+        return out
+
+    def _read_births(self, reserved):
+        """Queue this advance's birth log for resolution: copied into the ring's next host buffer without blocking, with an
+        event that marks the copy done."""
+        host = self._birth_ring[self._advances % len(self._birth_ring)]
+        host.copy_(self._birth_log, non_blocking=True)
+        done = None
+        if self.dev.type == "cuda":
+            done = torch.cuda.Event()
+            done.record()
+        self._birth_queue.append((self._advances - 1, reserved, host, done))
+
+    def _resolve(self, upto):
+        """Resolve the queued births of the advances up to `upto`: born targets join the host's maps, unborn reservations are
+        freed.  Waits on an advance's event only if its copy has not completed."""
+        while self._birth_queue and self._birth_queue[0][0] <= upto:
+            _, reserved, host, done = self._birth_queue.pop(0)
+            if done is not None and not done.query():
+                done.synchronize()
+            log = host.numpy()
+            for e, (k, f) in enumerate(reserved):
+                del self._pending[k]
+                if log[e, 3] >= 0:
+                    tid = int(log[e, 1])
+                    self.slot_of[tid] = k
+                    self._feed_of[k] = f
+                    self._born.append((tid, f, k, int(log[e, 3])))
+
+    def _upload_with_detections(self, w, fed, reserved=()):
+        """One host->device copy of the work list `w`, the birth list of the `reserved` (slot, feed) pairs (with births) and the
+        staged detections of the feeds in `fed` (a fed feed staged without detections has none), from a fresh pinned buffer;
+        only the bytes up to the last staged row are copied."""
         staged, self._det_staged = self._det_staged, {}
-        F, D = self.F, self.D
+        F, D, K, R = self.F, self.D, self.K, self.R
         end = max([self._det_at] + [self._det_at + (f * D + len(rows)) * 64 for f, rows in staged.items() if len(rows)])
         buf = torch.empty(end, dtype=torch.uint8, pin_memory=self.dev.type == "cuda")
         host = buf.numpy()
-        host[:16 * self.K] = w.reshape(-1).view(np.uint8)
+        host[:16 * K] = w.reshape(-1).view(np.uint8)
+        if R:
+            wb = np.array([[k for k, _ in reserved] + [K] * (R - len(reserved)), [f for _, f in reserved] + [-1] * (R - len(reserved))],
+                          dtype=np.int64)
+            host[16 * K:16 * K + 16 * R] = wb.reshape(-1).view(np.uint8)
         counts = np.array([len(staged.get(f, ())) if f in fed else 0 for f in range(F)], np.int32)
-        host[16 * self.K:16 * self.K + 4 * F] = counts.view(np.uint8)
+        host[self._n_at:self._n_at + 4 * F] = counts.view(np.uint8)
         for f, rows in staged.items():
             if len(rows):
                 at = self._det_at + f * D * 64
@@ -836,17 +1087,22 @@ class MultiTargetTracker:
 
     def add(self, target_id, box, feed=0):
         """Start target `target_id` on the most recent scan of `feed` with `box` (a data_classes.Box or a tracking.boxes.Box): the
-        box is its result on that scan, and the template's first-frame crop is taken from it.  No host sync."""
+        box is its result on that scan, and the template's first-frame crop is taken from it.  With births, ids are 0 ..
+        BIRTH_ID_BASE - 1 (born targets take the ids above) and the slots reserved for births are not free.  No host sync."""
         tid = int(target_id)
         f = self._feed(feed)
         if tid in self.slot_of:
             raise ValueError(f"target_id {tid} is already active")
-        if len(self.slot_of) >= self.K:
+        pending = {} if self.birth_rule is None else self._pending
+        if self.birth_rule is not None and not 0 <= tid < BIRTH_ID_BASE:
+            raise ValueError(f"target_id {tid}: a tracker with births takes ids 0 .. {BIRTH_ID_BASE - 1}; born targets get "
+                             f"BIRTH_ID_BASE + n")
+        if len(self.slot_of) + len(pending) >= self.K:
             raise ValueError(f"max_targets: all {self.K} slots are taken; drop a target first")
         if (self.scans_seen if self.F == 1 else self.feed_seen[f]) == 0:
             raise RuntimeError(f"add() starts a target on the most recent scan of its feed: call step() / advance() with a scan "
                                f"of feed {f} first")
-        k = min(set(range(self.K)) - set(self.slot_of.values()))
+        k = min(set(range(self.K)) - set(self.slot_of.values()) - set(pending))
         c, s, r = _box_values(box)
         vals = torch.tensor(np.concatenate([c, s, r.reshape(-1)]), dtype=torch.float32)
         if self.dev.type == "cuda":
@@ -952,6 +1208,17 @@ class MultiTargetTracker:
             rec, slot = host[f, :D * 16].reshape(D, 16).astype(np.float64), host[f, D * 16:D * 17]
             out[f] = [(d, Box(rec[d, 0:3], rec[d, 3:6], rec[d, 6:15].reshape(3, 3)), float(rec[d, 15]))
                       for d in range(int(host[f, -1])) if slot[d] < 0]
+        return out
+
+    def births(self, wait=False):
+        """The targets born since the last call, [(id, feed, slot, detection index in its advance's list), ...] in birth order,
+        without a host sync: the births of advance i are resolved at the start of advance i + BIRTH_LAG.  `wait`: first resolve
+        every advance so far, waiting for the device (for the end of a stream)."""
+        if self.birth_rule is None:
+            raise ValueError("births(): this tracker was built without births=")
+        if wait:
+            self._resolve(self._advances)
+        out, self._born = self._born, []
         return out
 
     def lost_targets(self):
@@ -1201,7 +1468,7 @@ def run_scenes(trk, add, drop, scenes, sched, chunk=256, evidence=False):
 
 
 def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_graph=True, chunk=256, precision="fp32", lost=None,
-                evidence=False, coast=None, detections=None):
+                evidence=False, coast=None, detections=None, births=None):
     """Track many scenes through one tracker with `feeds` scan feeds (`feed_schedule` decides which scene runs when and where).
     `scenes`: [{"frames": number of scans, "scan": t -> the scene's scan t, either (rows, transforms) for `put_raw` or an (n, 3)
     tensor / array for `put`, "starts": {t: [(id, Box), ...]}, "ends": {id: last t}}]; a target without an end runs to its scene's
@@ -1213,7 +1480,9 @@ def track_feeds(model, scenes, feeds, max_targets, seed=0, max_points=None, use_
     tracker's coasting (MultiTargetTracker); results run on through coasted frames, and the evidence also says whether each frame
     was coasted (run_scenes).  `detections`: the tracker's (max_per_scan, gate) (MultiTargetTracker); a scene's "detections":
     t -> its scan t's (M, 16) detections, put with the scan (births stay the scene's "starts"), and the evidence also says
-    whether each frame was re-acquired at a detection, and which detection it matched (run_scenes)."""
+    whether each frame was re-acquired at a detection, and which detection it matched (run_scenes).  `births` is refused: the
+    schedule reserves each scene's slots from its annotated starts, which births would not respect."""
+    refuse_births(births, "track_feeds")
     runtime.check_precision(precision)
     lost = check_lost_rule(lost)
     coast = check_coast(coast, lost)
