@@ -618,36 +618,54 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 // ------------------------------------------------------------------------------------------------------------
 // wgrad on the tensor core:  dW[m, n] += sum_p dY[p, m] * X[p, n]  over this CTA's slice of positions, one 128 x 128 tile
 // of dW per CTA.  Both operands are position-major in global memory (channels contiguous) while wgmma takes tf32 operands
-// K-major only, K being the position here: the producers transpose while they store, writing [128 channels x 32 positions]
-// K-major SWIZZLE_128B tiles (element (c, p) at sw128(c, p / 4) + 4 (p % 4)) with 4-byte st.shared.  A warp loads 8
-// positions x 16 channels (64-byte row segments) so that its transposed stores hit 16 banks (2-way conflicts).
+// K-major only, K being the position here.  Per 32-position k-block a stage holds
+//   dY      as it comes, unsplit: rows = positions, 4 SWIZZLE_128B sub-images of 32 channels (WG_DY_SUB bytes each), written
+//           with 16-byte stores.  The consumers read their A fragments (dY^T) from it with ld.shared, split them into hi / lo
+//           in registers and issue register-fed MMAs (wgmma_tf32_rs_n128), so only B is read by the tensor core from shared
+//           memory;
+//   X^T     hi | lo, [128 channels x 32 positions] K-major SWIZZLE_128B tiles written by store_transposed (16-byte stores of
+//           a 4 x 4 block transposed in registers).
 //   warps 0-3, 4-7  consumers: warpgroup h accumulates rows m0 + h*64 .. of the tile (wgmma m64n128k8, 3xTF32), then writes
 //                   its partial tile: plain stores into the split-K workspace part[split][m][n] (summed in a fixed order by
 //                   wgrad_reduce_kernel: deterministic)
-//   warps 8-15      producers: each thread owns 4 channels x 4 positions of both operands per k-block; producer thread 0
-//                   also keeps the L2 prefetch of the slice's rows WG_AHEAD k-blocks ahead of the stores (requesting the whole
-//                   slice up front asks for more than the L2 holds across the grid, and the lines are evicted again before
-//                   their k-block comes up)
-constexpr int WG_STAGES = 3;
+//   warps 8-15      producers: each thread owns 4 channels x 4 consecutive positions of each operand per k-block; producer
+//                   thread 0 also keeps the L2 prefetch of the slice's rows WG_AHEAD k-blocks ahead of the stores (requesting
+//                   the whole slice up front asks for more than the L2 holds across the grid, and the lines are evicted again
+//                   before their k-block comes up)
+// Shared memory: 4 stages x (dY 16 KB | X^T hi 16 KB | X^T lo 16 KB) (BF16: 3 stages x 64 KB) + alignment | barriers.
+constexpr int WG_STAGES = 4;                           // 3xTF32
+constexpr int WG_STAGE_BYTES = 3 * TILE_BYTES;
+constexpr int WG_DY_SUB = TC_K * 128;                  // 4 KB: 32 positions x 32 channels of dY
+constexpr int WG_BF_STAGES = 3;                        // BF16
+constexpr int WG_BF_STAGE_BYTES = 4 * TILE_BYTES;
 constexpr int WG_AHEAD = 4;
 constexpr int WG_THREADS = 512;
-constexpr int WG_SMEM = WG_STAGES * 4 * TILE_BYTES + 1024 + 256;
+constexpr int WG_SMEM = WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
+static_assert(WG_BF_STAGES * WG_BF_STAGE_BYTES == WG_STAGES * WG_STAGE_BYTES, "both precisions use one shared-memory size");
+// 3xTF32: each role declares its register bound (setmaxnreg) where the roles part.  The bound is the launch's own 128 per
+// thread, so nothing moves between the warpgroups, but ptxas then allocates the consumer and producer code separately:
+// without it the lifted instantiation's producers spill (32 bytes) although each role fits in 128 registers on its own.
+// A 120 / 136 split makes the consumers spill inside the MMA loop, and ptxas then serialises the wgmmas.
+constexpr int WG_REGS = 128;
 
+// X^T of one thread: positions p_first + 4 q .. p_first + 4 q + 3 (rows i of `raw`) x channels c_local .. c_local + 3 of a
+// [channels x 32 positions] K-major SWIZZLE_128B tile (element (c, p) at sw128(c, p / 4) + 4 (p % 4); hi at `hi`, lo
+// TILE_BYTES on).  The 4 x 4 block is transposed in registers, so each channel's 4 positions are one 16-byte chunk: 4
+// st.shared.v4 per half.  Channel c's chunk lands in bank group q ^ (c & 7): the 8 lanes of a quarter-warp, same channels
+// and q = 0 .. 7, hit 8 distinct groups.
 template <class L>
 __device__ __forceinline__ void store_transposed(const L& ld, const typename L::template Batch<4>& raw, const typename L::Coef& cf,
-                                                 uint8_t* hi, int c_local, int p_first, int prow0, int pend) {
+                                                 uint8_t* hi, int c_local, int p_first, int q, int pend) {
+    float4 v[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int pl = prow0 + 8 * i;
-        const float4 v = ld.finish(raw, cf, i, p_first + pl, pend);
-        const float e[4] = {v.x, v.y, v.z, v.w};
+    for (int i = 0; i < 4; ++i) v[i] = ld.finish(raw, cf, i, p_first + 4 * q + i, pend);
+    const float4 col[4] = {make_float4(v[0].x, v[1].x, v[2].x, v[3].x), make_float4(v[0].y, v[1].y, v[2].y, v[3].y),
+                           make_float4(v[0].z, v[1].z, v[2].z, v[3].z), make_float4(v[0].w, v[1].w, v[2].w, v[3].w)};
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const uint32_t off = sw128(c_local + j, pl >> 2) + (uint32_t)((pl & 3) * 4);
-            const float h = hi1(e[j]);
-            *reinterpret_cast<float*>(hi + off) = h;
-            *reinterpret_cast<float*>(hi + TILE_BYTES + off) = e[j] - h;
-        }
+    for (int j = 0; j < 4; ++j) {
+        const uint32_t off = sw128(c_local + j, q);
+        *reinterpret_cast<float4*>(hi + off) = hi_part(col[j]);
+        *reinterpret_cast<float4*>(hi + TILE_BYTES + off) = lo_part(col[j]);
     }
 }
 
@@ -671,10 +689,12 @@ template <class XB>
 __global__ void __launch_bounds__(WG_THREADS, 1)
     pw_wgrad_tc_kernel(TcDy da, XB xb, int P, int M, int N, int chunk, float* __restrict__ part) {
     constexpr bool BF = is_bf16<XB>::value;
+    constexpr int STAGES = BF ? WG_BF_STAGES : WG_STAGES;
+    constexpr int STAGE_BYTES = BF ? WG_BF_STAGE_BYTES : WG_STAGE_BYTES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * 4 * TILE_BYTES);
-    uint64_t* empty = full + WG_STAGES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+    uint64_t* empty = full + STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.z * TC_M, n0 = blockIdx.y * TC_N;
@@ -684,7 +704,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
     auto kpos = [&](int i) { return pbeg + i * TC_K; };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < WG_STAGES; ++s) {
+        for (int s = 0; s < STAGES; ++s) {
             o3d_mbar_init(full + s, 256);
             o3d_mbar_init(empty + s, 8);
         }
@@ -693,6 +713,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
     __syncthreads();
 
     if (warp < 8) {
+        if constexpr (!BF) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(WG_REGS));
         const int h = warp >> 2, w = warp & 3;
         float acc[64];
 #pragma unroll
@@ -700,25 +721,57 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
         int stage = 0, phase = 0;
         for (int kb = 0; kb < nkb; ++kb) {
             o3d_mbar_wait(full + stage, phase);
-            const uint32_t sb = o3d_smem_u32(smem + stage * 4 * TILE_BYTES);
-            wgmma_fence_acc(acc);
-            wgmma_fence();
+            const uint32_t sb = o3d_smem_u32(smem + stage * STAGE_BYTES);
             if constexpr (BF) {
+                wgmma_fence_acc(acc);
+                wgmma_fence();
                 const uint32_t ab = sb + h * 2 * WG_BF_SUB;                   // dY channels m0 + h*64 .. : sub-images 2h, 2h+1
 #pragma unroll
                 for (int ks = 0; ks < 2; ++ks)
                     wgmma_bf16_tt_n128(acc, make_desc_sw64_mn(ab + ks * 1024, WG_BF_SUB),
                                        make_desc_sw64_mn(sb + WG_BF_X + ks * 1024, WG_BF_SUB), (kb == 0 && ks == 0) ? 0u : 1u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(acc);
             } else {
-                const uint32_t ab = sb + h * (TILE_BYTES / 2);                 // dY rows (channels) m0 + h*64 ..
-                wgmma_3xtf32_kblock<128>(acc, make_desc(ab), make_desc(ab + TILE_BYTES), make_desc(sb + 2 * TILE_BYTES),
-                                         make_desc(sb + 3 * TILE_BYTES), kb == 0);
+                // A = dY^T fragments of the 4 k-steps: rows (channels) h*64 + 16 w + lane / 4 (+ 8), i.e. sub-image 2 h + w / 2,
+                // columns (positions) 8 ks + lane % 4 (+ 4); split into hi / lo here, as the producers split X^T
+                const uint8_t* dyk = smem + stage * STAGE_BYTES + (2 * h + (w >> 1)) * WG_DY_SUB;
+                const int mc = (16 * w + (lane >> 2)) & 31;
+                uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+                for (int ks = 0; ks < TC_K / 8; ++ks) {
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        const int p = ks * 8 + (lane & 3) + 4 * (i >> 1), m = mc + 8 * (i & 1);
+                        const float x = *reinterpret_cast<const float*>(dyk + sw128(p, m >> 2) + 4 * (m & 3));
+                        const float xh = hi1(x);
+                        ahi[ks][i] = __float_as_uint(xh);
+                        alo[ks][i] = __float_as_uint(x - xh);
+                    }
+                }
+                const uint64_t bhi = make_desc(sb + TILE_BYTES), blo = make_desc(sb + 2 * TILE_BYTES);
+                wgmma_fence_acc(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int ks = 0; ks < TC_K / 8; ++ks) {      // Alo.Bhi + Ahi.Blo + Ahi.Bhi, as wgmma_3xtf32_kblock
+                    const uint64_t adv = (uint64_t)((ks * 32) >> 4);
+                    wgmma_tf32_rs_n128(acc, alo[ks], bhi + adv, (kb == 0 && ks == 0) ? 0u : 1u);
+                    wgmma_tf32_rs_n128(acc, ahi[ks], blo + adv, 1u);
+                    wgmma_tf32_rs_n128(acc, ahi[ks], bhi + adv, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(acc);
+#pragma unroll
+                for (int ks = 0; ks < TC_K / 8; ++ks) {
+                    wgmma_fence_frag(ahi[ks]);
+                    wgmma_fence_frag(alo[ks]);
+                }
             }
-            wgmma_commit();
-            wgmma_wait<0>();
-            wgmma_fence_acc(acc);
+            // after the wait: the stage's dY image (read into the fragments) and X^T (read by the MMAs) are free again
             if (lane == 0) o3d_mbar_arrive(empty + stage);
-            if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
         const int Mt = TC_M * (int)gridDim.z, Nt = TC_N * (int)gridDim.y;
         float* __restrict__ out = part + (size_t)blockIdx.x * Mt * Nt;
@@ -732,15 +785,22 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
             }
         }
     } else {
-        // producers: 8 warps x (8 positions x 4 float4); thread: channels 4*c4 .. 4*c4+3, positions prow0 + 8*i, i < 4
+        if constexpr (!BF) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WG_REGS));
+        // producers, thread = 4 channels x 4 positions of each operand per k-block
+        //   3xTF32  dY: rows 4 pw .. 4 pw + 3 x channels 4 lane .. (16-byte row stores, a quarter-warp covers one 128-byte
+        //           row of a sub-image); X: positions 4 (lane % 8) .. + 3 x channels 4 c4 .. (see store_transposed)
+        //   BF16    both operands: channels 4 c4 .., positions prow0 + 8 i, i < 4
         const int pw = warp - 8;
-        const int c4 = pw * 4 + (lane & 3), prow0 = lane >> 2;
+        const int c4 = BF ? pw * 4 + (lane & 3) : pw * 4 + (lane >> 3), prow0 = lane >> 2;
+        const int ca = BF ? c4 : lane, pa = BF ? prow0 : 4 * pw;              // dY channel quad, first row
+        const int qx = lane & 7, px = BF ? prow0 : 4 * qx;                      // X first row
+        constexpr int RS = BF ? 8 : 1;                                         // row stride of both operands
         const bool pt0 = pw == 0 && lane == 0;
         TcDy::Batch<4> ra = {};
         typename XB::template Batch<4> rb = {};
         auto fetch = [&](int kb) {
-            da.fetch(ra, kpos(kb) + prow0, 8, pend, m0 + c4 * 4, M);
-            xb.fetch(rb, kpos(kb) + prow0, 8, pend, n0 + c4 * 4, N);
+            da.fetch(ra, kpos(kb) + pa, RS, pend, m0 + ca * 4, M);
+            xb.fetch(rb, kpos(kb) + px, RS, pend, n0 + c4 * 4, N);
         };
         auto prefetch = [&](int kb) {
             if (pt0 && kb < nkb) {
@@ -754,20 +814,24 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
         for (int kb = 0; kb < nkb; ++kb) {
             prefetch(kb + WG_AHEAD);
             o3d_mbar_wait(empty + stage, phase ^ 1);
-            uint8_t* sbase = smem + stage * 4 * TILE_BYTES;
+            uint8_t* sbase = smem + stage * STAGE_BYTES;
             // the per-channel coefficients are re-read (L1-resident) per k-block: kept live across the loop they push the
-            // lifted operand's producer past the 128-register budget
+            // lifted operand's producer past its register budget
             if constexpr (BF) {
                 store_rows_bf16(da, ra, da.prep(m0 + c4 * 4, M), sbase, WG_BF_SUB, c4 * 4, kpos(kb), prow0, pend);
                 store_rows_bf16(xb, rb, xb.prep(n0 + c4 * 4, N), sbase + WG_BF_X, WG_BF_SUB, c4 * 4, kpos(kb), prow0, pend);
             } else {
-                store_transposed(da, ra, da.prep(m0 + c4 * 4, M), sbase, c4 * 4, kpos(kb), prow0, pend);
-                store_transposed(xb, rb, xb.prep(n0 + c4 * 4, N), sbase + 2 * TILE_BYTES, c4 * 4, kpos(kb), prow0, pend);
+                const TcDy::Coef cf = da.prep(m0 + ca * 4, M);
+                uint8_t* dy = sbase + (ca >> 3) * WG_DY_SUB;
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                    *reinterpret_cast<float4*>(dy + sw128(pa + i, ca & 7)) = da.finish(ra, cf, i, kpos(kb) + pa + i, pend);
+                store_transposed(xb, rb, xb.prep(n0 + c4 * 4, N), sbase + TILE_BYTES, c4 * 4, kpos(kb), qx, pend);
             }
             o3d_fence_proxy_async();
             o3d_mbar_arrive(full + stage);
             if (kb + 1 < nkb) fetch(kb + 1);
-            if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
     }
 }
@@ -1022,7 +1086,11 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
         // ===================================================== producers (4 warps, 128 threads)
         const int pt = threadIdx.x - 256;
         const int chunk = pt & 7, row0 = (pt >> 3) * 4;               // dY: 4 neighbouring rows, 4 channels of a k-block
-        const int pw = warp - 8, c4 = pw * 4 + (lane & 3), prow0 = lane >> 2;   // X^T: 4 channels x positions prow0 + 8 i
+        // X: 4 channels 4 c4 .. x positions prow0 + 8 i (BF16), or 4 consecutive positions 4 (lane % 8) .. (3xTF32, see
+        // store_transposed)
+        const int pw = warp - 8, c4 = BF ? pw * 4 + (lane & 3) : pw * 4 + (lane >> 3), prow0 = lane >> 2;
+        const int qx = lane & 7, px = BF ? prow0 : 4 * qx;
+        constexpr int RS = BF ? 8 : 1;
         constexpr int NXH = N / 64;                                   // X^T pieces per 32-position k-block (64 channels each)
         const int n_items_x = 2 * NXH;
         // dY items (tile, kb) and X^T items (tile, j = 32-position half, channel half) are two flat sequences, each walked
@@ -1036,7 +1104,7 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
         };
         auto fetch_b = [&](const It& c) {
             if (c.t < n_ptiles)
-                xb.fetch(rb, c.t * BW_TP + (c.i >> (NXH - 1)) * TC_K + prow0, 8, P, (c.i & (NXH - 1)) * 64 + c4 * 4, N);
+                xb.fetch(rb, c.t * BW_TP + (c.i >> (NXH - 1)) * TC_K + px, RS, P, (c.i & (NXH - 1)) * 64 + c4 * 4, N);
         };
         fetch_a(ca);
         fetch_b(cb);
@@ -1077,7 +1145,7 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
                 if constexpr (BF)
                     store_rows_bf16(xb, rb, xb.prep(cl, N), smem + BW_XT + j * (TC_K * TC_BF_ROW), BW_BF_SUB, cl, pt0 + j * TC_K, prow0, P);
                 else
-                    store_transposed(xb, rb, xb.prep(cl, N), smem + BW_XT + j * (2 * TILE_BYTES), cl, pt0 + j * TC_K, prow0, P);
+                    store_transposed(xb, rb, xb.prep(cl, N), smem + BW_XT + j * (2 * TILE_BYTES), cl, pt0 + j * TC_K, qx, P);
                 if (++cb.i == n_items_x) { cb.i = 0; cb.t += gridDim.x; }
                 fetch_b(cb);
             }
