@@ -621,6 +621,63 @@ int o3d_track_metrics(const float* center, const float* rot, const float* wlh, c
                       const double* gt_wlh, const long long* frame, int K, int dim, int up_mask, double* overlap, double* distance,
                       void* stream);
 
+/* Block 7 — multi-object tracking scores (tracking/mot.py reference_counts, which it equals on the integer outputs; csrc/mot_eval.cu).
+ *
+ * o3d_mot_clear: the CLEAR MOT events and identity co-occurrence of S sequences, one CTA per sequence walking its frames in
+ *   order.  Sequence s has frames seq_frame[s] .. seq_frame[s+1] - 1; frame f has the ground-truth boxes frame_gt[f] ..
+ *   frame_gt[f+1] - 1 and the hypothesis boxes frame_hyp[f] .. frame_hyp[f+1] - 1, at most max_gt and max_hyp of them.  A box
+ *   is 15 fp64 values: centre (3), wlh (3), row-major rotation with the box axes in its columns (9).  gt_obj / hyp_idx hold each
+ *   box's dense index within its sequence, 0 .. O_s - 1 and 0 .. H_s - 1 (O_s = obj_off[s+1] - obj_off[s], H_s = hyp_off[s+1] -
+ *   hyp_off[s]); an index appears at most once per frame (the caller checks).
+ *   Pair (object o, hypothesis h) of a frame, in fp64 with every operation rounded on its own: metric 0 (IoU): iou =
+ *   estimateOverlap(gt, hyp, dim, up_axis) (o3d_track_metrics' arithmetic), valid when iou >= threshold, cost 1 - iou; metric 1
+ *   (distance): d = estimateAccuracy(gt, hyp, dim, up_axis), valid when d <= threshold, cost d.  Per frame: (1) carry-over: the
+ *   objects in frame order, each matched to its last matched hypothesis when that is in the frame, still unmatched and valid;
+ *   (2) among the remaining objects and hypotheses, a maximum-cardinality matching over the valid pairs of least total cost:
+ *   scipy.optimize.linear_sum_assignment's shortest augmenting paths, operation for operation, on the remainder with every
+ *   invalid pair at 2 r c + 1 (r = min of its two sizes, c = 1 + the largest |cost| of its valid pairs; unchanged when every
+ *   pair is valid, no matching when none is), its invalid assignments dropped; a new pair is a switch when the object's last
+ *   matched hypothesis exists and differs, else a match; (3) unmatched objects are misses, unmatched hypotheses false positives.
+ *   Writes, per sequence: counts[s, 0..6] = objects, predictions, matches, switches, misses, false positives, fragmentations
+ *   (per object, tracked -> missed transitions between its first and last tracked frames), and cost_sum[s], the matched and
+ *   switched pairs' costs summed in frame order, then object order within a frame.  Per object (row obj_off[s] + o):
+ *   obj[., 0..3] = frames present, frames tracked (matched or switched), its last matched hypothesis (-1: none), the
+ *   fragmentation walk's state.  cooc[cooc_off[s] + o H_s + h] = the frames in which (o, h) is a valid pair (cooc_off[s+1] -
+ *   cooc_off[s] = O_s H_s int32).  Every output is written by the call (nothing needs zeroing), with no atomics: the results
+ *   are bitwise the same run to run and do not depend on the other sequences of the launch.  work [work_rows, max_gt *
+ *   max_hyp] fp64 is scratch: the call runs min(S, work_rows) CTAs, each taking the sequences s = its index mod their number.
+ *   (max_gt + max_hyp) * 96 bytes of dynamic shared memory per CTA, 48 KB at most; no host sync.  dim / up_mask as
+ *   o3d_track_metrics.  Refused: a null descriptor or pointer, S < 0, max_gt or max_hyp outside 0 .. 256, work_rows < 1, metric
+ *   not 0 / 1, threshold outside (0, 1] (IoU) or not finite and > 0 (distance), dim not 2 / 3, up_mask outside 1 .. 7.  S = 0
+ *   launches nothing. */
+#define O3D_MOT_MAX_BOXES 256
+#define O3D_MOT_COUNTERS 7
+typedef struct o3d_mot_clear_t {
+    int S;                     /* sequences */
+    int metric;                /* 0: IoU, 1: centre distance */
+    double threshold;
+    int dim;
+    int up_mask;
+    int max_gt, max_hyp;       /* the most boxes of one frame, each side (the row length of work: max_gt * max_hyp) */
+    int work_rows;
+    const long long* seq_frame;    /* [S + 1] */
+    const long long* frame_gt;     /* [F + 1] */
+    const long long* frame_hyp;    /* [F + 1] */
+    const long long* obj_off;      /* [S + 1] */
+    const long long* hyp_off;      /* [S + 1] */
+    const long long* cooc_off;     /* [S + 1] */
+    const int* gt_obj;         /* [NG] */
+    const int* hyp_idx;        /* [NH] */
+    const double* gt_box;      /* [NG, 15] */
+    const double* hyp_box;     /* [NH, 15] */
+    long long* counts;         /* [S, 7] out */
+    double* cost_sum;          /* [S] out */
+    int* obj;                  /* [sum O_s, 4] out */
+    int* cooc;                 /* [sum O_s H_s] out */
+    double* work;              /* [work_rows, max_gt * max_hyp] scratch */
+} o3d_mot_clear_t;
+int o3d_mot_clear(const o3d_mot_clear_t* p, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

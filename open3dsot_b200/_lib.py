@@ -86,6 +86,7 @@ PROTOTYPES = {
     "o3d_sa_fused_forward": [_p, _p, _p, _p, _p, _i, _i, _i, _i, ctypes.c_float, _i, _i, _p, _i, _p, _p],
     "o3d_keyed_uniform": [_p, _p, _i, ctypes.c_uint, _i, _i, _p, _p],
     "o3d_track_metrics": [_p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p],
+    "o3d_mot_clear": [_p, _p],
 }
 _RESTYPE = {"o3d_last_error": ctypes.c_char_p, "o3d_pw_tc_wtile_bytes": ctypes.c_longlong,
             "o3d_stack_workspace_bytes": ctypes.c_longlong, "o3d_stack_prepared_bytes": ctypes.c_longlong,
@@ -138,6 +139,14 @@ class BirthDesc(ctypes.Structure):
                [(n, _p) for n in ("feed", "adv", "pred", "fed", "count", "det", "rec_slot", "birth_slot", "birth_feed", "next",
                                   "log", "box_c", "box_s", "box_r", "first_flag", "active", "key", "t", "slot_feed", "points",
                                   "score", "misses", "lost", "vel", "hit_c", "hit_t", "coasting", "detection", "reacquired")]
+
+
+class MotClearDesc(ctypes.Structure):
+    """ctypes mirror of `o3d_mot_clear_t` (include/o3d_b200.h)."""
+    _fields_ = [("S", _i), ("metric", _i), ("threshold", _d)] + \
+               [(n, _i) for n in ("dim", "up_mask", "max_gt", "max_hyp", "work_rows")] + \
+               [(n, _p) for n in ("seq_frame", "frame_gt", "frame_hyp", "obj_off", "hyp_off", "cooc_off", "gt_obj", "hyp_idx",
+                                  "gt_box", "hyp_box", "counts", "cost_sum", "obj", "cooc", "work")]
 
 
 # o3d_stack_t.precision: 3xTF32 (default), BF16 inference (eval mode only), BF16 training (training mode only)

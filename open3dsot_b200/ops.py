@@ -558,3 +558,42 @@ def track_metrics(center, rot, wlh, gt_center, gt_rot, gt_wlh, frame, dim, up_ax
     assert rot.shape == (K, 3, 3) and wlh.shape == (K, 3) and frame.shape == (K,)
     _call("o3d_track_metrics", center.data_ptr(), rot.data_ptr(), wlh.data_ptr(), gt_center.data_ptr(), gt_rot.data_ptr(),
           gt_wlh.data_ptr(), frame.data_ptr(), K, int(dim), up_mask(up_axis), overlap.data_ptr(), distance.data_ptr(), _stream())
+
+
+# ------------------------------------------------------------------ multi-object tracking scores (tracking/mot.py)
+MOT_COUNTERS = 7
+MOT_METRICS = ("iou", "distance")
+
+
+def mot_clear(seq_frame, frame_gt, frame_hyp, obj_off, hyp_off, cooc_off, gt_obj, hyp_idx, gt_box, hyp_box, metric, threshold,
+              dim, up_axis, max_gt, max_hyp, work_rows):
+    """The CLEAR MOT events and identity co-occurrence of S sequences in one launch (csrc/mot_eval.cu, one CTA per sequence).
+    Offsets seq_frame (S+1,), frame_gt / frame_hyp (F+1,), obj_off / hyp_off / cooc_off (S+1,) int64; gt_obj (NG,) / hyp_idx
+    (NH,) int32 dense per-sequence indices; gt_box (NG, 15) / hyp_box (NH, 15) fp64 (centre, wlh, row-major rotation); all CUDA.
+    `metric`: "iou" or "distance"; max_gt / max_hyp: the most boxes of one frame (<= 256); work_rows: scratch rows (CTAs).
+    Returns (counts (S, 7) int64, cost_sum (S,) fp64, obj (sum O_s, 4) int32, cooc (sum O_s H_s,) int32), enqueued on the
+    current stream."""
+    for t, name in ((seq_frame, "seq_frame"), (frame_gt, "frame_gt"), (frame_hyp, "frame_hyp"), (obj_off, "obj_off"),
+                    (hyp_off, "hyp_off"), (cooc_off, "cooc_off")):
+        _chk_i64(t, name)
+    _chk_i(gt_obj, "gt_obj")
+    _chk_i(hyp_idx, "hyp_idx")
+    for t, name in ((gt_box, "gt_box"), (hyp_box, "hyp_box")):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float64 or not t.is_contiguous():
+            raise RuntimeError(f"{name} must be a contiguous float64 CUDA tensor")
+    S = seq_frame.shape[0] - 1
+    assert gt_box.shape == (gt_obj.shape[0], 15) and hyp_box.shape == (hyp_idx.shape[0], 15)
+    assert obj_off.shape == hyp_off.shape == cooc_off.shape == (S + 1,) and frame_gt.shape == frame_hyp.shape
+    dev = seq_frame.device
+    n_obj, n_cooc = int(obj_off[-1]), int(cooc_off[-1])
+    counts = torch.empty(S, MOT_COUNTERS, dtype=torch.int64, device=dev)
+    cost_sum = torch.empty(S, dtype=torch.float64, device=dev)
+    obj = torch.empty(max(n_obj, 1), 4, dtype=torch.int32, device=dev)
+    cooc = torch.empty(max(n_cooc, 1), dtype=torch.int32, device=dev)
+    work = torch.empty(max(int(work_rows), 1), max(int(max_gt) * int(max_hyp), 1), dtype=torch.float64, device=dev)
+    d = _lib.MotClearDesc(S, MOT_METRICS.index(metric), float(threshold), int(dim), up_mask(up_axis), int(max_gt), int(max_hyp),
+                          int(work_rows),
+                          *(t.data_ptr() for t in (seq_frame, frame_gt, frame_hyp, obj_off, hyp_off, cooc_off, gt_obj, hyp_idx,
+                                                   gt_box, hyp_box, counts, cost_sum, obj, cooc, work)))
+    _call("o3d_mot_clear", ctypes.byref(d), _stream())
+    return counts, cost_sum, obj[:n_obj], cooc[:n_cooc]

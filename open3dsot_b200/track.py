@@ -35,7 +35,15 @@ reader lists it (`scene_list`), the frame as the scene's frames are numbered, th
 quaternion the box's orientation (data_classes.Box).  A scan without a line has no detections.  The tracker matches them to
 its targets (MultiTargetTracker's `detections=`) and re-acquires a missed target at its detection; tracklets still start from
 their first annotated box.  Every JSON line's targets carry "detection", the index of the detection matched on that frame in
-its line's boxes (null: none), and "reacquired"; the summary counts "reacquired_at_detection", the target-frames re-acquired."""
+its line's boxes (null: none), and "reacquired"; the summary counts "reacquired_at_detection", the target-frames re-acquired.
+
+Multi-object scores.  `--mot {iou,distance} THRESHOLD` scores the run as multi-object tracking (tracking/mot.py: CLEAR MOT and
+IDF1, on the device) with the config's IoU_space and up_axis: each scene is a sequence over its streamed frames, its ground
+truth the split's annotations on the frame (object id: the tracklet's index) and its hypotheses every box the run reported on
+the frame (id: the target's tracklet index).  A box reported on a frame where its tracklet has no annotation is a false positive
+(nuScenes' min_points=1 filtering of the evaluation splits can leave such frames).  The summary gains "mot": {"total",
+"sequences"}; with several classes, each class is scored against its own ground truth under "classes", and "mot": {"total"} at
+the top sums them."""
 import argparse
 import json
 import sys
@@ -105,6 +113,10 @@ def parse_args(argv=None):
                    help='with --detections: the largest centre distance of a match, in the plane orthogonal to up_axis')
     p.add_argument('--max_detections', type=int, metavar='N', default=argparse.SUPPRESS,
                    help='with --detections: the most detections of one scan (1 .. 1024)')
+    # --mot as well (SUPPRESS): a run without it is scored as it always was
+    p.add_argument('--mot', nargs=2, metavar=('METRIC', 'THRESHOLD'), default=argparse.SUPPRESS,
+                   help='also score the run as multi-object tracking (CLEAR MOT, IDF1): METRIC iou (a pair matches when its '
+                        'IoU >= THRESHOLD) or distance (centre distance <= THRESHOLD)')
     args = p.parse_args(argv)
     if hasattr(args, "lost"):
         from .tracking.multi_tracker import check_lost_rule
@@ -129,10 +141,22 @@ def parse_args(argv=None):
             args.detection_rule = check_detections((args.max_detections, args.detection_gate))
         except ValueError as e:
             p.error(f"--detection_gate / --max_detections: {e}")
+    if hasattr(args, "mot"):
+        try:
+            args.mot = check_mot(args.mot)
+        except ValueError as e:
+            p.error(f"--mot: {e}")
     for extra in args.add_class or ():
         if len(extra) > 2:
             p.error(f"--add_class takes a config and at most one checkpoint, got {extra}")
     return args
+
+
+def check_mot(mot):
+    """--mot METRIC THRESHOLD as (metric, threshold): ValueError for an unknown metric or a threshold out of its range."""
+    from .tracking.mot import check_scoring
+    metric, threshold = mot
+    return check_scoring(metric, threshold)[:2]
 
 
 # reader settings that decide which scans a scene's frames are and in which frame their points are: the classes of one run share
@@ -314,11 +338,36 @@ def _score_tracklet(boxes, gts, frames, dim, up):
     return overlaps, distances
 
 
+def mot_sequences(plan, results, dataset, cls=None):
+    """The scenes of a run as tracking.mot sequences, one per scene over its streamed frames: ground truth, the annotations of
+    the scene's tracklets on the frame with the tracklet index as id; hypotheses, every box of `results` (track_feeds' per-scene
+    {target: {frame: Box}}) on the frame with the target's tracklet index as id.  `cls`: one class of a run_classes plan and
+    results (targets keyed (class, index))."""
+    annos = dataset.tracklet_anno_list
+    seqs = []
+    for p, res in zip(plan, results):
+        gt = {}
+        for tr in p["tracklets"]:
+            if cls is None or tr["class"] == cls:
+                for a in annos[tr["index"]]:
+                    gt.setdefault(dataset.anno_frame(a)[1], []).append((tr["index"], dataset.box_from_anno(a)))
+        hyp = sorted((k, b) for k, b in res.items() if cls is None or k[0] == cls)
+        seqs.append([(gt.get(fr, []), [(k if cls is None else k[1], b[t]) for k, b in hyp if t in b])
+                     for t, fr in enumerate(p["frames"])])
+    return seqs
+
+
+def _mot(mot, seqs, dim, up):
+    from .tracking.mot import mot_metrics
+    return mot_metrics(seqs, mot[0], mot[1], dim, up)
+
+
 def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, precision="fp32", lost=None, coast=None,
-        detections=None, scan_detections=None):
+        detections=None, scan_detections=None, mot=None):
     """Track every scene of `dataset`'s split and write `out_path`; returns {"success", "precision", "frames", "scenes"},
     "lost" with a `lost` rule, and "coasted" / "reacquired" with `coast`.  `detections`: (max_per_scan, gate) and
-    `scan_detections` the `read_detections` table: then also "reacquired_at_detection"."""
+    `scan_detections` the `read_detections` table: then also "reacquired_at_detection".  `mot`: (metric, threshold): then
+    also "mot", the run's tracking.mot scores (mot_sequences)."""
     from .tracking.multi_tracker import track_feeds
     from .utils.metrics import Precision, Success
 
@@ -375,18 +424,21 @@ def run(model, dataset, out_path, max_targets=64, max_points=None, seed=0, preci
         out.update(coasted=coasted, reacquired=reacquired)
     if detections is not None:
         out["reacquired_at_detection"] = at_detection
+    if mot is not None:
+        out["mot"] = _mot(mot, mot_sequences(plan, results, dataset), dim, up)
     return out
 
 
 def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0, precision="fp32", lost=None, coast=None,
-                detections=None, scan_detections=None):
+                detections=None, scan_detections=None, mot=None):
     """`run` for several classes in one pass over the scans: `models`, `datasets` and `max_targets` are {class: ...} (the class
     is its config's category_name).  Every scene streams once for all classes (class_scene_plan) through one MultiClassTracker;
     a target's draws are keyed by its tracklet's index in its class's reader, as in a one-class run.  Every JSON line's targets
     carry their "class".  Returns {"success", "precision", "frames", "scenes"} over every class's frames, and the same per class
     under "classes"; with a `lost` rule (every class's), "lost" counts the tracklets it ended early, overall and per class, and
     with `coast` (every class's), so do "coasted" and "reacquired"; with `detections` (every class's, and `scan_detections` the
-    `read_detections` table), "reacquired_at_detection"."""
+    `read_detections` table), "reacquired_at_detection"; with `mot`, each class's tracking.mot scores against its own ground
+    truth under "classes" and "mot": {"total"} over every class's sequences."""
     from .tracking.multi_class import track_classes
     from .utils.metrics import Precision, Success
 
@@ -453,6 +505,11 @@ def run_classes(models, datasets, out_path, max_targets, max_points=None, seed=0
 
     out = scores(names)
     out.update({"scenes": len(plan), "classes": {c: scores([c]) for c in names}})
+    if mot is not None:
+        from .tracking.mot import total_scores
+        for c in names:
+            out["classes"][c]["mot"] = _mot(mot, mot_sequences(plan, results, datasets[c], cls=c), dim, up)
+        out["mot"] = {"total": total_scores([s for c in names for s in out["classes"][c]["mot"]["sequences"]], mot[0])}
     return out
 
 
@@ -489,6 +546,8 @@ def main(argv=None):
         rule["coast"] = args.coast
     if hasattr(args, "detections"):
         rule.update(detections=args.detection_rule, scan_detections=read_detections(args.detections))
+    if hasattr(args, "mot"):
+        rule["mot"] = args.mot
     classes = [(args.cfg, args.checkpoint)] + [(a[0], a[1] if len(a) > 1 else None) for a in args.add_class or ()]
     cfgs = [load_config(c) for c, _ in classes]
     check_classes(cfgs, [c for c, _ in classes])

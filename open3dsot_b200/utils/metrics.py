@@ -49,8 +49,9 @@ def _intersection_area(pa, pb):
     return _poly_area(poly)
 
 
-def estimateOverlap(box_a, box_b, dim=2, up_axis=(0, -1, 0)):
-    pa, pb = _footprint(box_a, up_axis), _footprint(box_b, up_axis)
+def estimateOverlap(box_a, box_b, dim=2, up_axis=(0, -1, 0), footprints=None):
+    """`footprints`: the boxes' `_footprint`s when the caller already has them (one per box, not one per pair)."""
+    pa, pb = footprints if footprints is not None else (_footprint(box_a, up_axis), _footprint(box_b, up_axis))
     inter = _intersection_area(pa, pb)
     if dim == 2:
         union = _poly_area(pa) + _poly_area(pb) - inter
